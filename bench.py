@@ -1,14 +1,14 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the NERRF AI hot path on B200 (driver contract).
+"""bench.py -- headline benchmark of the NERRF AI hot path on H100.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     torchrun --nproc-per-node N ... bench.py --gpus N ...
 
 Metric (BASELINE.json): GraphSAGE-T edges/sec (+ MCTS rollouts/sec, reported under "mcts") on the
 1M-node / 10M-edge synthetic temporal graph, 3-layer inference (configs[1]).  One "step" = one
 full GraphSAGE_T.forward (3 fused gather+aggregate+GEMM layers + node head) over the graph.
 
-  value      graph resident in HBM, CUDA-event timed, whole job (all ranks), max over ranks
+  value      graph resident in HBM, CUDA-event timed over --steps K steps, whole job (all ranks), max over ranks
   e2e        the same forward from HOST buffers: N=1 through nerrf_sage_session_forward_host (pinned host graph -> H2D
              -> forward -> D2H node scores, every step); N>1 every rank uploads only ITS rows / edge block and the
              ranks complete each other's features over NVLink (nerrf_b200.dist.ShardedSage.sharded_upload)
@@ -21,6 +21,10 @@ full GraphSAGE_T.forward (3 fused gather+aggregate+GEMM layers + node head) over
              a failed check makes the process exit non-zero
   cpu_baseline / --impl reference   the oracle's C/OpenMP restatement over the FULL graph on the box's host cores
              (kind "port": the reference ships no implementation of this path, SURVEY.md 0)
+--dump-outputs DIR (N=1): after the timed steps, the last step's outputs as float32 .npy files: score.npy (node scores,
+             [N]) and h_sample.npy (the final embeddings of a fixed, seeded sample of 65536 rows, [65536, 128]), plus
+             h_sample_rows.npy (those row ids, float64).  The inputs are seeded, so two builds can be compared output
+             for output.
 N > 1: weak scaling -- the graph grows to N x (1M nodes, 10M edges), 1-D edge-block sharded with row-aligned cuts, one
 embedding exchange per layer fused into the layer kernel (nerrf_b200/dist.py).  Extra objects of the N>1 line:
 "trace_graph" (trace-structured graph, component-aware cuts), "cfg4" (BASELINE configs[3]: 10M / 100M strong-scaled
@@ -58,12 +62,22 @@ def algorithmic_bytes_forward(E, N):
     return b + 4 * N
 
 
+def kernel_launches_per_step(model, rowptr):
+    """Kernels one forward step launches: per layer the tensor-core layer and the split of its weights into bf16 terms
+    (the fp32 CUDA-core layer: the layer alone, plus the node-head kernel after the last one); on graphs with rows of
+    more than 128 in-edges the tensor-core layer adds the hub-row pre-pass (a scan before the first layer, a chunk kernel
+    before every layer)."""
+    if model.algo == "ffma":
+        return LAYERS + 1
+    return 2 * LAYERS + (1 + LAYERS if model._has_hub_rows(rowptr) else 0)
+
+
 def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 class ClockSampler(threading.Thread):
@@ -116,7 +130,7 @@ def workload_config(n_gpus):
                         f"({gen}, src=floor(N*u^3), dst~U), F_in={F_IN}, H={HIDDEN}",
             "nodes": N_NODES * n_gpus, "edges": N_EDGES * n_gpus, "layers": LAYERS,
             "parallelism": "single GPU" if n_gpus == 1 else f"1-D edge-block shards x{n_gpus}, one embedding exchange per layer",
-            "l2": "inputs exceed L2 (graph 0.2 GB + activations 0.5 GB/layer per GPU vs 126 MB); no flush"}
+            "l2": "inputs exceed L2 (graph 0.2 GB + activations 0.5 GB/layer per GPU vs 50 MB); no flush"}
 
 
 # ------------------------------------------------------------------------------------------ oracle side (checker / CPU arm)
@@ -254,10 +268,12 @@ def run_single(args, dev, local_rank):
     torch.cuda.synchronize()
     t_start.record()
     for i in range(K):
-        step(i)
+        last = step(i)
     t_end.record()
     torch.cuda.synchronize()
     clocks = sampler.result()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, *last)
     total_ms = t_start.elapsed_time(t_end)
     layer_ms = np.array([[ev[i][l].elapsed_time(ev[i][l + 1]) for l in range(LAYERS)] for i in range(K)])
     ms_per_step = total_ms / K
@@ -269,15 +285,11 @@ def run_single(args, dev, local_rank):
     dom_bytes = algorithmic_bytes_layer(E, N, HIDDEN)
     achieved = dom_bytes / (dom_ms * 1e-3) / 1e9
     traffic = traffic_l1 = None
-    tp = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tp):
-        traffic = json.load(open(tp)).get("sage_layer_F128_dram_bytes_per_launch")
-        traffic_l1 = json.load(open(tp)).get("sage_layer_F32_dram_bytes_per_launch")
     l1_bytes = algorithmic_bytes_layer(E, N, F_IN)
     l1_ms = float(layer_ms[:, 0].mean())
     roofline = {"bound": "hbm", "kernel": "fused GraphSAGE-T layer F=128 (gather+aggregate+GEMM)",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
-                "traffic_source": "ncu --set full capture of the same kernel and graph (profiles/traffic.json); not measured in this run",
+                "traffic_source": "not measured",
                 "layer_F32": {"kernel": "the same kernel at F=32 (layer 1, quad-mode gather)", "algorithmic_bytes_per_launch": l1_bytes,
                               "kernel_ms": l1_ms, "achieved": l1_bytes / (l1_ms * 1e-3) / 1e9, "frac": l1_bytes / (l1_ms * 1e-3) / 1e9 / peak,
                               "traffic": traffic_l1},
@@ -348,11 +360,24 @@ def run_single(args, dev, local_rank):
     line = {"metric": "graphsage_t_edges_per_sec", "value": value, "unit": "edges/s", "n_gpus": 1, "steps": K, "warmup": W,
             "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32",
             "data": "synthetic", "config": workload_config(1), "roofline": roofline, "cpu_baseline": cpu, "e2e": e2e,
-            "gpu_launches": K * LAYERS, "clocks": clocks, "parity": parity, "variants": variants, "mcts": mcts_info,
+            "gpu_launches": K * kernel_launches_per_step(model, rp), "clocks": clocks, "parity": parity, "variants": variants, "mcts": mcts_info,
             "lstm": lstm_info, "graph_build": graph_info, "cfg5": cfg5, "algo": args.algo}
     if cfg5 is not None:
         ok = ok and cfg5.get("ok", True)
     return line, ok
+
+
+DUMP_SAMPLE_ROWS, DUMP_SEED = 65536, 12345
+
+
+def dump_outputs(out_dir, h, score):
+    """The timed path's last outputs (see the module docstring): 4 MB of scores + a 32 MB seeded row sample of h."""
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    rows = np.sort(np.random.default_rng(DUMP_SEED).choice(h.shape[0], size=min(DUMP_SAMPLE_ROWS, h.shape[0]), replace=False))
+    np.save(os.path.join(out_dir, "score.npy"), score.float().cpu().numpy())
+    np.save(os.path.join(out_dir, "h_sample.npy"), h[torch.from_numpy(rows).to(h.device)].float().cpu().numpy())
+    np.save(os.path.join(out_dir, "h_sample_rows.npy"), rows.astype(np.float64))
 
 
 def run_graph_variants(dev, model, peak, reps=5):
@@ -415,9 +440,8 @@ def run_multi(args, world, rank, local_rank, dev):
     layer_wall = [tr["compute_ms"][l] + tr["exchange_ms"][l] for l in range(LAYERS)]
     nvlink = {"egress_bytes_per_layer_rank0": eg, "mean_ingress_bytes_per_layer": ing,
               "achieved_egress_gbps_per_exchanged_layer": [eg / (layer_wall[l] * 1e-3) / 1e9 for l in range(LAYERS - 1)],
-              "peak_per_direction_gbps": 900.0, "measured_peer_copy_gbps": 770.0,
-              "bound_ms_per_exchanged_layer": max(eg, ing) / 900e9 * 1e3,
-              "bound_ms_per_exchanged_layer_at_measured_peer_copy": max(eg, ing) / 770e9 * 1e3,
+              "peak_per_direction_gbps": 450.0,
+              "bound_ms_per_exchanged_layer": max(eg, ing) / 450e9 * 1e3,
               "weak_scaling_ceiling": "random vertex relabeling makes every rank read the same hub-heavy ~55 % of all rows: a rank must "
                                       "RECEIVE that many 512-byte rows per exchanged layer whatever the transport (P2P, multicast), so "
                                       "step time >= 2 x ingress / link rate + the last layer; trace_graph is the same metric on the workload "
@@ -472,6 +496,7 @@ def run_multi(args, world, rank, local_rank, dev):
                          "frac": dom_bytes / (dom_ms * 1e-3) / 1e9 / peak, "traffic": None, "peak_source": peak_src,
                          "per_layer_compute_ms": tr["compute_ms"], "per_layer_exchange_ms": tr["exchange_ms"],
                          "per_rank_segments_ms": tr["per_rank_segments_ms"], "exchange_bytes_per_layer": int(N * HIDDEN * 4)}
+    launches = kernel_launches_per_step(model, rowptr)
     del ss, rowptr, col, ew, x, x_keep, hx_own, hcol, hew
     torch.cuda.empty_cache()
 
@@ -499,7 +524,7 @@ def run_multi(args, world, rank, local_rank, dev):
             "vs_baseline": None, "dtype": "f32",
             "data": "synthetic (torch CUDA generator, same distribution as the N=1 graph, random vertex relabeling for shard balance)",
             "config": dict(workload_config(world), exchange=exchange_desc), "roofline": headline_roofline, "cpu_baseline": None,
-            "e2e": e2e, "gpu_launches": K * LAYERS, "clocks": clocks, "parity": parity, "nvlink": nvlink,
+            "e2e": e2e, "gpu_launches": K * launches, "clocks": clocks, "parity": parity, "nvlink": nvlink,
             "trace_graph": trace_graph, "cfg4": cfg4, "cfg5": cfg5, "mcts": mcts_local, "algo": args.algo}
     return line, ok
 
@@ -632,7 +657,7 @@ def run_cfg5(dev, dist_rw, n_procs=10400, n_attacked=40):
                           "seconds_total); per tick the window is a slice of the time-sorted index array and node interning (hash "
                           "table), per-node features, edge assembly and the CSR sort run on the GPU",
            "not_timed": {"train_s": t_train, "trace_generation_s": t_gen,
-                         "train": "ai/train.py, 25 epochs on the GPU: GraphSAGE-T layers forward (tcgen05) and backward (csrc/sage_bwd.cu) through the C-ABI"},
+                         "train": "ai/train.py, 25 epochs on the GPU: GraphSAGE-T layers forward (wgmma) and backward (csrc/sage_bwd.cu) through the C-ABI"},
            "ok": True}
     return out
 
@@ -772,6 +797,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--algo", default="auto", choices=["auto", "ffma", "umma", "umma2"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="N=1: write the last timed step's outputs (node scores, a seeded row sample of h) as .npy into DIR")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-cfg4", action="store_true", help="N>1: skip the 10M/100M strong-scaling run")
     ap.add_argument("--no-cfg5", action="store_true", help="skip the streamed fleet-trace end-to-end run")
@@ -780,6 +807,10 @@ def main():
                          "peer-mapped buffers over NVLink, only the rows a peer references); p2p-all = same, every row "
                          "to every peer; multicast = NVSwitch multimem.st; allgather / broadcast / allreduce = NCCL")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and (args.gpus != 1 or args.impl != "ours"):
+        ap.error("--dump-outputs needs --gpus 1 --impl ours")
     if args.impl == "reference":
         run_reference(args)
     else:

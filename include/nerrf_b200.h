@@ -1,4 +1,4 @@
-/* nerrf_b200 -- C-ABI of the B200-native NERRF AI hot path.
+/* nerrf_b200 -- C-ABI of the H100-native NERRF AI hot path.
  *
  * The reference (Itz-Agasta/nerrf @ a38ae13) has NO FFI / plugin interface for this path
  * (SURVEY.md 8b): the ai/ module it names (README.md:72-76) was never written.  The entry
@@ -32,13 +32,13 @@ extern "C" {
 #define NERRF_OK 0
 #define NERRF_ERR_INVALID (-1)   /* bad argument (shape, alignment, unsupported size)      */
 #define NERRF_ERR_CUDA (-2)      /* a CUDA runtime call / kernel launch failed              */
-#define NERRF_ERR_NODEVICE (-3)  /* no sm_100 device                                        */
+#define NERRF_ERR_NODEVICE (-3)  /* no sm_90 device                                         */
 #define NERRF_ERR_WORKSPACE (-4) /* workspace too small                                     */
 
 /* algo selector for the GraphSAGE-T layer */
 #define NERRF_SAGE_ALGO_AUTO 0
 #define NERRF_SAGE_ALGO_FFMA 1   /* fused gather+aggregate -> fp32 CUDA-core GEMM           */
-#define NERRF_SAGE_ALGO_UMMA 2   /* fused gather+aggregate -> tcgen05 GEMM, 3-term bf16 split
+#define NERRF_SAGE_ALGO_UMMA 2   /* fused gather+aggregate -> wgmma GEMM, 3-term bf16 split
                                     (6 MMAs per K step; fp32-equivalent accuracy)           */
 #define NERRF_SAGE_ALGO_UMMA2 3  /* same with a 2-term split (3 MMAs; ~1e-5 relative)       */
 
@@ -65,7 +65,8 @@ int nerrf_sage_aggregate(const float* x, const void* rowptr, int rowptr_is64, co
                          int64_t row_end, int F, nerrf_stream_t stream);
 
 /* One fused layer: out[v] = act([x_v || m_v] @ W + b) for v in [row_begin,row_end); out is the
- * FULL [n_nodes, H] array (rows outside the range untouched).  W [2F, H], b [H]; H == 128. */
+ * FULL [n_nodes, H] array (rows outside the range untouched).  W [2F, H], b [H]; H == 128.
+ * x, out, W, b (and node_w below) must be 16-byte aligned. */
 int nerrf_sage_layer_fwd(const float* x, const void* rowptr, int rowptr_is64, const int32_t* col,
                          const float* ew, const float* W, const float* b, float* out,
                          int64_t n_nodes, int64_t row_begin, int64_t row_end, int F, int H,

@@ -94,7 +94,7 @@ def lib():
     if not os.path.exists(path):
         raise NerrfError(
             f"{path} not found: build it with `python -m nerrf_b200.build` "
-            "(nvcc, sm_100a).  There is no CPU fallback.")
+            "(nvcc, sm_90a).  There is no CPU fallback.")
     h = C.CDLL(path)
     for name, (res, args) in SIGNATURES.items():
         fn = getattr(h, name)          # AttributeError if the .so does not export a declared symbol

@@ -1,7 +1,7 @@
 """GraphSAGE-T layers as torch.autograd Functions over the C-ABI kernels (SURVEY.md 8f rank 3: training on the GPU).
 
 Reference surface: the GraphSAGE-T half of ai/train.py "joint GNN+LSTM training script" (README.md:75; ROADMAP.md:62-69 --
-named, never written).  Forward = the fused tcgen05 layer kernel the inference path uses (`nerrf_sage_layer_fwd_ex`),
+named, never written).  Forward = the fused tensor-core (wgmma) layer kernel the inference path uses (`nerrf_sage_layer_fwd_ex`),
 backward = `nerrf_sage_layer_bwd` (csrc/sage_bwd.cu): dP = dy*[y>0], dW = [h||m]^T dP, db, dZ = dP W^T,
 dh = dZ[:, :F] + A^T dZ[:, F:], the last as a gather over the transposed graph.  CUDA tensors only; no CPU fallback
 (ai/train.py keeps its plain-torch restatement for CPU runs and as the thing the gradients are checked against).
@@ -56,7 +56,7 @@ def aggregate(h, tg: TrainGraph):
 
 
 class SageLayerFn(torch.autograd.Function):
-    """y = relu([h || A h] W + b) -- forward on tcgen05 (fused gather + aggregate + GEMM), backward in csrc/sage_bwd.cu."""
+    """y = relu([h || A h] W + b) -- forward on wgmma (fused gather + aggregate + GEMM), backward in csrc/sage_bwd.cu."""
 
     @staticmethod
     def forward(ctx, h, W, b, tg: TrainGraph, model, l: int):

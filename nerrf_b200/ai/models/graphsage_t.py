@@ -1,4 +1,4 @@
-"""ai.models.GraphSAGE_T -- temporal GraphSAGE anomaly scorer (CUDA, sm_100a).
+"""ai.models.GraphSAGE_T -- temporal GraphSAGE anomaly scorer (CUDA, sm_90a).
 
 Reference surface: ai/models/GraphSAGE-T.py `GraphSAGE_T.forward` (README.md:73; ROADMAP.md:67,127
 -- named, never written).  Behaviour: docs/content/docs/architecture.mdx:49-53,157 (edge

@@ -1,4 +1,4 @@
-"""ai.models.lstm -- BiLSTM per-file event-sequence scorer (CUDA, sm_100a).
+"""ai.models.lstm -- BiLSTM per-file event-sequence scorer (CUDA, sm_90a).
 
 Reference surface: ai/models/lstm.py `forward` (README.md:73 -- named, never written).
 Behaviour: "Bidirectional LSTM (256 hidden, 2 layers)", "last 100 events per file"
@@ -94,10 +94,10 @@ Model = LSTMScorer
 
 
 def default_algo() -> str:
-    """Which kernel family nerrf_lstm_forward runs: the tcgen05 path unless NERRF_LSTM_ALGO=ffma selects the fp32
+    """Which kernel family nerrf_lstm_forward runs: the wgmma path unless NERRF_LSTM_ALGO=ffma selects the fp32
     CUDA-core kernel (kept as an independent cross-check)."""
     import os
-    return "ffma" if os.environ.get("NERRF_LSTM_ALGO", "").lower().startswith("f") else "umma (tcgen05)"
+    return "ffma" if os.environ.get("NERRF_LSTM_ALGO", "").lower().startswith("f") else "umma (wgmma)"
 
 _default = None
 

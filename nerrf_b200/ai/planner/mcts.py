@@ -1,4 +1,4 @@
-"""ai.planner.mcts -- MCTS rollback planner (CUDA persistent leaf-parallel kernel, sm_100a).
+"""ai.planner.mcts -- MCTS rollback planner (CUDA persistent leaf-parallel kernel, sm_90a).
 
 Reference surface: ai/planner/mcts.py `search` (README.md:74,115; ROADMAP.md:84 -- named, never
 written).  Behaviour: "500-1000 simulations", "Timeout: 5 min", input "Graph + anomaly scores +

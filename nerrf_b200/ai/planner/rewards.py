@@ -1,4 +1,4 @@
-"""ai.planner.rewards -- rollback reward scorer (CUDA, sm_100a).
+"""ai.planner.rewards -- rollback reward scorer (CUDA, sm_90a).
 
 Reference surface: ai/planner/rewards.py (README.md:74 -- named, never written).
 Behaviour: `Reward = -(data_loss + 0.1 x downtime)` (README.md:115); "restoration gain - side

@@ -6,7 +6,7 @@ docs/content/docs/threat-model.mdx:176-203,277-292.
 
 Training is NOT the north-star hot path (that is inference: GraphSAGE_T.forward, lstm.forward, mcts.search,
 rewards.score -- CUDA only).  With `--device cuda` the GraphSAGE-T half trains through the library's own kernels: the
-fused tcgen05 layer forward and the hand-written backward (`nerrf_sage_layer_bwd`, csrc/sage_bwd.cu) behind a
+fused wgmma layer forward and the hand-written backward (`nerrf_sage_layer_bwd`, csrc/sage_bwd.cu) behind a
 torch.autograd.Function (nerrf_b200.ai.autograd); on the CPU it differentiates a plain-torch statement of the same frozen
 spec (also the thing the CUDA gradients are tested against).  The BiLSTM half is torch.nn.LSTM under autograd on either
 device.  Both update the very nn.Parameters the CUDA inference kernels read (GraphSAGE_T.weights / biases / node_w /
@@ -46,7 +46,7 @@ def sage_node_logits(model: GraphSAGE_T, x, rowptr, col, ew):
 
 
 def node_logits(model: GraphSAGE_T, ex):
-    """Node-head logits of one example with gradients: on a CUDA device through the library's own kernels (fused tcgen05
+    """Node-head logits of one example with gradients: on a CUDA device through the library's own kernels (fused wgmma
     forward + csrc/sage_bwd.cu backward, nerrf_b200.ai.autograd), on the CPU through the plain-torch restatement above."""
     if ex["x"].is_cuda:
         from . import autograd as AG

@@ -1,4 +1,4 @@
-"""Build the C-ABI library in-tree with nvcc for sm_100a (no torch dependency in the .so).
+"""Build the C-ABI library in-tree with nvcc for sm_90a (H100; no torch dependency in the .so).
 
     python -m nerrf_b200.build            # -> nerrf_b200/csrc/libnerrf_b200.so
 """
@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libnerrf_b200.so")
 SOURCES = ["api.cu", "sage.cu", "sage_umma.cu", "sage_bwd.cu", "mcts.cu", "lstm.cu", "lstm_umma.cu", "graph.cu", "ingest.cu", "intern_device.cu"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 

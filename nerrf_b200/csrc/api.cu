@@ -15,12 +15,12 @@ void set_error(const char* fmt, ...) {
 int sm_count() {
     static int cached[64] = {};
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+    if (cudaGetDevice(&dev) != cudaSuccess) return 132;
     int& c = cached[dev & 63];
     if (c == 0) {
         int n = 0;
         if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) c = n;
-        else return 148;
+        else return 132;
     }
     return c;
 }
@@ -47,8 +47,8 @@ extern "C" int nerrf_device_info(int* sm_count, int* cc_major, int* cc_minor) {
     if (sm_count) *sm_count = prop.multiProcessorCount;
     if (cc_major) *cc_major = prop.major;
     if (cc_minor) *cc_minor = prop.minor;
-    if (prop.major != 10) {
-        nerrf::set_error("device is sm_%d%d; this library is built for sm_100a only", prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {
+        nerrf::set_error("device is sm_%d%d; this library is built for sm_90a only", prop.major, prop.minor);
         return NERRF_ERR_NODEVICE;
     }
     return NERRF_OK;

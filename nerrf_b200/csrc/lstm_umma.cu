@@ -1,36 +1,30 @@
-// BiLSTM on 5th-gen tensor cores (tcgen05 / TMEM), sm_100a only -- lstm.forward (SURVEY.md 8a row a4).
+// BiLSTM on Hopper tensor cores (wgmma), sm_90a -- lstm.forward (SURVEY.md 8a row a4).
 //
 // One LSTM layer-direction step is   gates[4H, seqs] = G_x[:, t] + W_hh[4H, H] . h_{t-1}[H, seqs]   followed by the cell
-// update.  Everything that multiplies a weight matrix runs on tcgen05 with the weight slice RESIDENT IN TENSOR MEMORY
-// (A operand, fp32 split into three bf16 terms, six products per K step: fp32-equivalent accuracy, same scheme as
-// sage_umma.cu) and the activations as the B operand, bulk-copied (cp.async.bulk, byte-counting mbarrier) from a
-// global-memory OPERAND IMAGE -- the exact byte layout the UMMA reads (K-major, SWIZZLE_128B, three bf16 planes):
+// update.  Everything that multiplies a weight matrix runs on wgmma: the weight slice is the A operand, register
+// fragments read from L2 and split into three bf16 terms (six products per K step: fp32-equivalent accuracy, same
+// scheme as sage_umma.cu), and the activations are the B operand, bulk-copied (cp.async.bulk, byte-counting mbarrier)
+// from a global-memory OPERAND IMAGE -- the exact byte layout wgmma reads (K-major, SWIZZLE_128B, three bf16 planes):
 //
 //   image of a time-major activation X[t][b][K]:   tile (t, bt = b / 64, khalf):  [plane 3][kblock KB][row 64][128 B]
 //
 //   * lstm_image_kernel     layer-1 input seq [B,T,D] -> image (K padded to 64, one K block)
-//   * lstm_proj_kernel      input projection G_x = X W_ih^T (+ b) for all (t, b): persistent CTAs, each keeps ONE
-//                           (direction, gate slice) of W_ih^T (one K half of 256) in TMEM and streams 64-row tiles of the
-//                           image through a two-stage bulk-copy pipeline; no conversion work, the tensor pipe is the limit
+//   * lstm_proj_kernel      input projection G_x = X W_ih^T (+ b) for all (t, b): persistent CTAs, each owns ONE
+//                           (direction, gate slice) of W_ih^T (one K half of 256) and streams 64-row tiles of the image
+//                           through a two-stage bulk-copy pipeline into one consumer warpgroup
 //   * lstm_rec_kernel       the recurrence.  W_hh (1024 x 256) is cut into 8 slices of 128 gate rows (4 gates x 32 units);
 //                           8 CTAs (one per slice) form a GROUP that advances tiles of 64 sequences of one direction.
-//                           Per step every CTA computes gates^T[128, 64] (+)= W_slice . h_{t-1}^T with the accumulator
-//                           pre-loaded with G_x[:, t]; the epilogue applies the activations, updates c / h in registers,
-//                           splits the new h into its three bf16 terms and stores them INTO THE LAYER'S OUTPUT IMAGE
-//                           (tile (t, bt, khalf = direction)) -- which is at once the next layer's projection operand and
-//                           the h_{t} exchange between the 8 CTAs: after one release-increment of the group's counter every
-//                           CTA bulk-copies the whole 96 KB tile back as its next B operand.
-//                           The step is a latency chain (MMA -> epilogue -> publish -> poll -> 96 KB copy -> MMA), so every
-//                           group works on TWO tiles at once (two operand buffers, two accumulators, two epilogue
-//                           warpgroups): while one tile waits for its exchange the other one's MMAs run.
+//                           Per step every CTA computes gates^T[128, 64] = G_x[:, t] + W_slice . h_{t-1}^T in the
+//                           registers of a warpgroup, applies the activations, updates c / h in registers, splits the
+//                           new h into its three bf16 terms and stores them INTO THE LAYER'S OUTPUT IMAGE (tile (t, bt,
+//                           khalf = direction)) -- which is at once the next layer's projection operand and the h_{t}
+//                           exchange between the 8 CTAs: after one release-increment of the group's counter every CTA
+//                           bulk-copies the whole 96 KB tile back as its next B operand.  The step is a latency chain
+//                           (MMA -> cell update -> publish -> poll -> 96 KB copy -> MMA), so every CTA works on TWO
+//                           tiles at once (two operand buffers, one warpgroup each).
 //
 // Groups are independent (no grid barrier): group g owns direction g & 1.  The 8 CTAs of a group must be co-resident:
 // cooperative launch, one CTA per SM, grid = 8 * G <= #SMs.  Every wait is bounded and ends in a trap, never a hang.
-//
-// History (profiles/r02_lstm.md): v0 FFMA kernel 51.6 ms for B=4096 / T=100; v1 (fp32 exchange, every CTA re-splits h,
-// projections through the GraphSAGE-T kernel as a dense GEMM) 31.7 ms; v2 (bf16x3 image exchange) 30.3 ms -- the
-// recurrence was a 19 us latency chain per step with the tensor pipe idle 85 % of the time, hence the two-tile interleave
-// and the dedicated projection kernel of this version.
 #include <cuda_bf16.h>
 #include <stdlib.h>
 #include "common.cuh"
@@ -40,17 +34,14 @@ namespace nerrf {
 namespace {
 
 constexpr int LH = 256;                 // hidden size
-constexpr int NSEQ = 64;                // sequences per tile = UMMA N
+constexpr int NSEQ = 64;                // sequences per tile = wgmma N
 constexpr int SLICES = 8;               // CTAs per group
-constexpr int UM = 128;                 // gate rows per slice = UMMA M
+constexpr int UM = 128;                 // gate rows per slice = two wgmma M=64 halves
 constexpr int NS = 3;                   // bf16 terms per fp32 value
 constexpr int KB_H = LH / 64;           // 128-byte K blocks of a 256-wide operand
 constexpr int KSTEPS_H = LH / 16;
 constexpr int PLANE_BYTES_H = KB_H * NSEQ * 128;     // 32 KB: one bf16 plane of a [64 rows, 256] tile
 constexpr int TILE_BYTES_H = NS * PLANE_BYTES_H;     // 96 KB
-constexpr int W_PART_COLS = LH / 2;                  // TMEM columns of one W plane (K = 256)
-constexpr int ACC_COL0 = NS * W_PART_COLS;           // 384
-constexpr int TMEM_COLS = 512;
 
 // ---------------------------------------------------------------- PTX wrappers (same forms as sage_umma.cu)
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -89,87 +80,34 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uin
 }
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 __device__ __forceinline__ void named_bar(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                 ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-          "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]),
-          "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]),
-          "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]),
-          "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-// UMMA shared-memory descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B apart (SBO), version 1.
+// wgmma shared-memory matrix descriptor (sm_90): K-major, SWIZZLE_128B, 8-row groups 1024 B apart (SBO)
 __device__ __forceinline__ uint64_t make_b_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-__host__ __device__ constexpr uint32_t make_idesc() {      // D=f32, A=B=bf16 K-major, N = NSEQ, M = 128
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NSEQ >> 3) << 17) | ((uint32_t)(UM >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 x 64] (+)= A[64 x 16] (bf16 register fragment) . B[16 x 64] (bf16, K-major shared memory), fp32 accumulate
+__device__ __forceinline__ void wgmma_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %37, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)
+        : "memory");
 }
 __device__ __forceinline__ void split_pair(float a, float b, uint32_t (&parts)[NS]) {
 #pragma unroll
@@ -183,7 +121,7 @@ __device__ __forceinline__ void split_pair(float a, float b, uint32_t (&parts)[N
     }
 }
 // byte offset of ONE bf16 element (row r of the tile, K index k inside the K block range) inside a plane: K-major
-// SWIZZLE_128B, 128-byte rows of one 64-wide K block, 16-byte chunks XOR-swizzled by the row (what the UMMA reads)
+// SWIZZLE_128B, 128-byte rows of one 64-wide K block, 16-byte chunks XOR-swizzled by the row (what wgmma reads)
 __device__ __forceinline__ uint32_t b_elem_offset(int r, int k) {
     const int kb = k >> 6, col = k & 63;
     return (uint32_t)(kb * (NSEQ * 128) + r * 128 + ((((col >> 3) ^ (r & 7)) << 4) | ((col & 7) << 1)));
@@ -197,49 +135,58 @@ __device__ __forceinline__ unsigned ld_acquire(const unsigned* p) {
 __device__ __forceinline__ float sigmoid_fast(float x) { return __fdividef(1.0f, 1.0f + __expf(-x)); }
 __device__ __forceinline__ float tanh_fast(float x) { return fmaf(2.0f, sigmoid_fast(2.0f * x), -1.0f); }
 
-// W^T slice [K, 128] (fp32, k-major) -> TMEM planes: thread = gate row f (lane of TMEM), 2 bf16 per 32-bit column.
-// K / 2 columns per plane; plane p starts at column p * plane_stride.
-__device__ __forceinline__ void load_w_to_tmem(const float* __restrict__ W, int K, uint32_t tmem_base, int plane_stride, int warp, int lane) {
-    const int f = warp * 32 + lane;
-    const uint32_t lane_addr = tmem_base + ((uint32_t)(warp * 32) << 16);
-    for (int k0 = 0; k0 < K; k0 += 16) {
-        uint32_t parts[NS][8];
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-            const float a = __ldg(W + (size_t)(k0 + 2 * i) * UM + f);
-            const float b = __ldg(W + (size_t)(k0 + 2 * i + 1) * UM + f);
-            uint32_t pp[NS];
-            split_pair(a, b, pp);
-#pragma unroll
-            for (int p = 0; p < NS; ++p) parts[p][i] = pp[p];
-        }
-#pragma unroll
-        for (int p = 0; p < NS; ++p) tmem_st8(lane_addr + (uint32_t)(p * plane_stride + (k0 >> 1)), parts[p]);
-    }
-    tmem_wait_st();
-}
-
-// the six split products of one 64-row tile: D[128, 64] (+)= W[128, K] . X[64, K]^T, W planes in TMEM, X planes in smem
+// Fragment layout shared by both kernels (one warpgroup, thread = (warp w, lane = 4 g + c)): accumulator row m of half h
+// (m = 16 w + i) holds slice column 32 w + 4 (i & 7) + 2 h + (i >> 3), so a thread's four rows are the four CONSECUTIVE
+// slice columns f0 .. f0 + 3 (f0 = 32 w + 4 g) -- with the slice packing of pack_slices_kernel, the gates i, f, g, o of
+// hidden unit 8 w + g.  Its accumulator registers d[h][4 nb + 2 b + e] hold column f0 + 2 h + b, tile row 8 nb + 2 c + e.
+//
+// D[128, 64] (+)= W[128, K] . X[64, K]^T for one 64-row tile: W^T fragments are read from the fp32 slice [K][128] (L2)
+// and split into three bf16 terms per K step (six products: fp32-equivalent), X's three planes are in shared memory.
 template <int KSTEPS>
-__device__ __forceinline__ void issue_tile_mmas(uint32_t d_tmem, uint32_t w_tmem, int plane_stride, uint32_t x_smem, uint32_t plane_bytes,
-                                                bool accumulate_first) {
-    constexpr uint32_t idesc = make_idesc();
-#pragma unroll 2
+__device__ __forceinline__ void mma_tile(float (&d)[2][32], const float* __restrict__ W, uint32_t x_smem, uint32_t plane_bytes,
+                                         bool accumulate_first, int warp, int lane) {
+    const int g = lane >> 2, c = lane & 3;
+    const float* wsrc = W + (size_t)(2 * c) * UM + warp * 32 + 4 * g;
+    auto load_w = [&](int j, float4 (&q)[4]) {
+        const float* p = wsrc + (size_t)(16 * j) * UM;
+        q[0] = __ldg(reinterpret_cast<const float4*>(p));
+        q[1] = __ldg(reinterpret_cast<const float4*>(p + UM));
+        q[2] = __ldg(reinterpret_cast<const float4*>(p + 8 * UM));
+        q[3] = __ldg(reinterpret_cast<const float4*>(p + 9 * UM));
+    };
+    auto comp = [](const float4& v, int i) { return i == 0 ? v.x : (i == 1 ? v.y : (i == 2 ? v.z : v.w)); };
+    float4 q[4];
+    load_w(0, q);
+#pragma unroll 1
     for (int j = 0; j < KSTEPS; ++j) {
+        uint32_t wa[2][NS][4];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {                 // fragment register r: row g + 8 (r & 1), k pair r >> 1
+                const int kq = (r >> 1) * 2;
+                uint32_t pp[NS];
+                split_pair(comp(q[kq], 2 * h + (r & 1)), comp(q[kq + 1], 2 * h + (r & 1)), pp);
+#pragma unroll
+                for (int p = 0; p < NS; ++p) wa[h][p][r] = pp[p];
+            }
+        if (j + 1 < KSTEPS) load_w(j + 1, q);
         const uint32_t boff = (uint32_t)((j >> 2) * (NSEQ * 128) + (j & 3) * 32);
         uint64_t xb[NS];
-        uint32_t wa[NS];
 #pragma unroll
-        for (int p = 0; p < NS; ++p) {
-            xb[p] = make_b_desc(x_smem + (uint32_t)p * plane_bytes + boff);
-            wa[p] = w_tmem + (uint32_t)(p * plane_stride + j * 8);
+        for (int p = 0; p < NS; ++p) xb[p] = make_b_desc(x_smem + (uint32_t)p * plane_bytes + boff);
+        wgmma_fence();
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            wgmma_rs(d[h], wa[h][0], xb[0], (j > 0 || accumulate_first) ? 1u : 0u);
+            wgmma_rs(d[h], wa[h][0], xb[1], 1u);
+            wgmma_rs(d[h], wa[h][1], xb[0], 1u);
+            wgmma_rs(d[h], wa[h][1], xb[1], 1u);
+            wgmma_rs(d[h], wa[h][0], xb[2], 1u);
+            wgmma_rs(d[h], wa[h][2], xb[0], 1u);
         }
-        umma_ts(d_tmem, wa[0], xb[0], idesc, (j > 0 || accumulate_first) ? 1u : 0u);
-        umma_ts(d_tmem, wa[0], xb[1], idesc, 1u);
-        umma_ts(d_tmem, wa[1], xb[0], idesc, 1u);
-        umma_ts(d_tmem, wa[1], xb[1], idesc, 1u);
-        umma_ts(d_tmem, wa[0], xb[2], idesc, 1u);
-        umma_ts(d_tmem, wa[2], xb[0], idesc, 1u);
+        wgmma_commit();
+        wgmma_wait_all();                                  // the fragments are rewritten next step
     }
 }
 
@@ -284,46 +231,32 @@ struct ProjArgs {
     int ctas_per_combo;
 };
 
+constexpr int PROJ_THREADS = 160;                   // warps 0-3: wgmma + epilogue, warp 4: loader
+
 template <int KB>
-__global__ void __launch_bounds__(192, 1) lstm_proj_kernel(ProjArgs P) {
+__global__ void __launch_bounds__(PROJ_THREADS, 1) lstm_proj_kernel(ProjArgs P) {
     constexpr int K = 64 * KB, KSTEPS = K / 16;
     constexpr int PLANE = KB * NSEQ * 128, TILE = NS * PLANE;       // bytes of one (tile, K range)
-    constexpr int WCOLS = K / 2;                                    // TMEM columns per W plane
-    constexpr int ACC0 = NS * WCOLS;
     constexpr int STAGES = 2;
     extern __shared__ unsigned char smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    unsigned char* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
     const uint32_t bar_base = smem_base + STAGES * TILE;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-    auto accf_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + a); };
-    auto acce_bar = [&](int a) { return bar_base + 8u * (2 * STAGES + 2 + a); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * STAGES + 4);
-    volatile uint32_t* tmem_slot_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
 
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;          // warps 0-3 epilogue, 4 MMA, 5 loader
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int combo = blockIdx.x / P.ctas_per_combo, j0 = blockIdx.x % P.ctas_per_combo;
     if (warp == 4) {
         if (lane == 0) {
-            for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-            for (int a = 0; a < 2; ++a) { mbar_init(accf_bar(a), 1); mbar_init(acce_bar(a), 128); }
+            for (int s = 0; s < STAGES; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 4); }
             fence_barrier_init();
         }
         __syncwarp();
-        tmem_alloc(tmem_slot, TMEM_COLS);
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_gen;
-    if (warp < 4) load_w_to_tmem(P.wih + (size_t)combo * K * UM, K, tmem_base, WCOLS, warp, lane);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
 
     const int64_t n_mine = j0 < P.n_tiles ? (P.n_tiles - j0 + P.ctas_per_combo - 1) / P.ctas_per_combo : 0;
-    if (warp == 5) {
+    if (warp == 4) {
         if (lane == 0) {
             for (int64_t i = 0; i < n_mine; ++i) {
                 const int s = (int)(i % STAGES);
@@ -337,58 +270,40 @@ __global__ void __launch_bounds__(192, 1) lstm_proj_kernel(ProjArgs P) {
                     bulk_g2s(smem_base + (uint32_t)(s * TILE + c * CH), src + (size_t)c * CH, (uint32_t)CH, full_bar(s));
             }
         }
-    } else if (warp == 4) {
-        if (lane == 0) {
-            for (int64_t i = 0; i < n_mine; ++i) {
-                const int s = (int)(i % STAGES), a = (int)(i & 1);
-                mbar_wait(acce_bar(a), ((uint32_t)(i >> 1) & 1u) ^ 1u);
-                mbar_wait(full_bar(s), (uint32_t)(i / STAGES) & 1u);
-                tc_fence_after();
-                issue_tile_mmas<KSTEPS>(tmem_base + (uint32_t)(ACC0 + a * NSEQ), tmem_base, WCOLS, smem_base + (uint32_t)(s * TILE),
-                                        (uint32_t)PLANE, false);
-                umma_commit(empty_bar(s));
-                umma_commit(accf_bar(a));
-            }
-        }
     } else {
-        const int gcol = warp * 32 + lane;
-        const float my_bias = P.bias ? __ldg(P.bias + (size_t)combo * UM + gcol) : 0.f;
-        float* g = P.gx + (size_t)combo * P.rows_total * UM + gcol;
+        const int g = lane >> 2, c = lane & 3;
+        const int f0 = warp * 32 + 4 * g;
+        const float4 b4 = P.bias ? *reinterpret_cast<const float4*>(P.bias + (size_t)combo * UM + f0) : make_float4(0.f, 0.f, 0.f, 0.f);
+        float* gout = P.gx + (size_t)combo * P.rows_total * UM + f0;
+        const float* W = P.wih + (size_t)combo * K * UM;
         for (int64_t i = 0; i < n_mine; ++i) {
-            const int a = (int)(i & 1);
-            mbar_wait(accf_bar(a), (uint32_t)(i >> 1) & 1u);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(ACC0 + a * NSEQ);
+            const int s = (int)(i % STAGES);
+            mbar_wait(full_bar(s), (uint32_t)(i / STAGES) & 1u);
+            float d[2][32];
+            mma_tile<KSTEPS>(d, W, smem_base + (uint32_t)(s * TILE), (uint32_t)PLANE, false, warp, lane);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty_bar(s));                    // this warp's MMAs no longer read the stage
             const int64_t row0 = (j0 + i * P.ctas_per_combo) * NSEQ;      // rows of the padded time-major matrix
-            uint32_t v[32], w[32];
-            tmem_ld32(taddr, v);
-            tmem_ld32(taddr + 32, w);
-            tmem_wait_ld();
-            tc_fence_before();
-            mbar_arrive(acce_bar(a));
 #pragma unroll
-            for (int r = 0; r < 32; ++r) g[(size_t)(row0 + r) * UM] = __uint_as_float(v[r]) + my_bias;
+            for (int nb = 0; nb < 8; ++nb)
 #pragma unroll
-            for (int r = 0; r < 32; ++r) g[(size_t)(row0 + 32 + r) * UM] = __uint_as_float(w[r]) + my_bias;
+                for (int e = 0; e < 2; ++e) {
+                    const float4 o = make_float4(d[0][4 * nb + e] + b4.x, d[0][4 * nb + 2 + e] + b4.y,
+                                                 d[1][4 * nb + e] + b4.z, d[1][4 * nb + 2 + e] + b4.w);
+                    *reinterpret_cast<float4*>(gout + (size_t)(row0 + 8 * nb + 2 * c + e) * UM) = o;
+                }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4) { tc_fence_after(); tmem_dealloc(tmem_base, TMEM_COLS); }
 }
 
 // ================================================================================================ recurrence
-// The epilogue is instruction-issue bound (2 warps per scheduler ran at IPC ~0.25 each: 20 k cycles per step,
-// profiles/r02_lstm.md), so every tile slot gets EIGHT epilogue warps: two per TMEM lane quarter, each owning 32 of the
-// tile's 64 sequences.
-constexpr int REC_EPI_WARPS = 16;                    // warps 0-7: tile slot 0, warps 8-15: tile slot 1
-constexpr int REC_MMA_WARP = 16;
-constexpr int REC_INIT_WARP0 = 17;                   // warps 17-20: slot 0, warps 21-24: slot 1 (accumulator init + exchange)
-constexpr int REC_THREADS = (REC_INIT_WARP0 + 8) * 32;               // 800
-constexpr int GATE_BYTES = 2 * 4 * 16 * 32 * 4;      // 16 KB per slot: [half][gate][seq in chunk of 16][unit]
-constexpr size_t REC_SMEM = (size_t)2 * TILE_BYTES_H + 2 * GATE_BYTES + 2 * NSEQ * 4 + 1024 /*align*/ + 128 /*barriers*/;
+// One warpgroup per tile slot (two slots per CTA, so that one tile's MMAs run while the other waits for its exchange).
+// Per step the warpgroup loads G_x[:, t] into its accumulators, adds W_slice . h_{t-1} (wgmma, h_{t-1} bulk-copied into
+// its operand buffer), applies the cell update in registers -- a thread holds the four gates of one hidden unit for 16
+// sequences -- and stores h_t's three bf16 terms into the layer's output image, then publishes the step.
+constexpr int REC_THREADS = 256;
+constexpr size_t REC_SMEM = (size_t)2 * TILE_BYTES_H + 2 * NSEQ * 4 + 1024 /*align*/ + 128 /*barriers*/;
 static_assert(REC_SMEM <= 227 * 1024, "shared memory budget");
-static_assert(ACC_COL0 + 2 * NSEQ <= TMEM_COLS, "TMEM budget");
 
 struct RecArgs {
     const float* gx_a;        // [2 dirs * 8 slices][Rp = T*Bp rows][128]: first K range of the input projection + bias
@@ -407,269 +322,138 @@ __global__ void __launch_bounds__(REC_THREADS, 1) lstm_rec_kernel(RecArgs P) {
     extern __shared__ unsigned char smem_raw[];
     const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     unsigned char* smem_gen = smem_raw + (smem_base - smem_u32(smem_raw));
-    float* gate_s = reinterpret_cast<float*>(smem_gen + 2 * TILE_BYTES_H);                       // [2 slots][4][32][32]
-    int* len_s = reinterpret_cast<int*>(smem_gen + 2 * TILE_BYTES_H + 2 * GATE_BYTES);           // [2 slots][64]
-    const uint32_t bar_base = smem_base + 2 * TILE_BYTES_H + 2 * GATE_BYTES + 2 * NSEQ * 4;
+    int* len_s = reinterpret_cast<int*>(smem_gen + 2 * TILE_BYTES_H);                              // [2 slots][64]
+    const uint32_t bar_base = smem_base + 2 * TILE_BYTES_H + 2 * NSEQ * 4;
     auto opfull_bar = [&](int s) { return bar_base + 8u * s; };
-    auto accinit_bar = [&](int s) { return bar_base + 16u + 8u * s; };
-    auto accf_bar = [&](int s) { return bar_base + 32u + 8u * s; };
-    auto drained_bar = [&](int s) { return bar_base + 48u + 8u * s; };
-    const uint32_t tmem_slot = bar_base + 64u;
-    volatile uint32_t* tmem_slot_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int group = blockIdx.x / SLICES, slice = blockIdx.x % SLICES;
     const int dir = group & 1;
     const int groups_dir = P.groups >> 1;                          // groups per direction
     const int gd = group >> 1;                                     // this group's index inside its direction
-    // tile sequence of (group, slot): bt = gd + (2 * i + slot) * groups_dir, i = 0, 1, ...
-    auto n_items = [&](int slot) -> int64_t {
-        const int64_t first = gd + (int64_t)slot * groups_dir;
-        return first < P.n_bt ? (P.n_bt - first + 2 * groups_dir - 1) / (2 * groups_dir) : 0;
-    };
-    const int64_t Rp = (int64_t)P.T * P.Bp;
-
-    if (warp == REC_MMA_WARP) {
-        if (lane == 0) {
-            for (int s = 0; s < 2; ++s) {
-                mbar_init(opfull_bar(s), 1);                 // one arrive (+ the bulk copies' transaction bytes)
-                mbar_init(accinit_bar(s), 128);              // the slot's accumulator-init warps
-                mbar_init(accf_bar(s), 1);
-                mbar_init(drained_bar(s), 256);              // the slot's epilogue warps
-            }
-            fence_barrier_init();
-        }
-        __syncwarp();
-        tmem_alloc(tmem_slot, TMEM_COLS);
+    if (tid == 0) {
+        for (int s = 0; s < 2; ++s) mbar_init(opfull_bar(s), 1);  // one arrive (+ the bulk copies' transaction bytes)
+        fence_barrier_init();
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_gen;
-    if (warp < 4) load_w_to_tmem(P.whh + (size_t)(dir * SLICES + slice) * LH * UM, LH, tmem_base, W_PART_COLS, warp, lane);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
 
-    const float* gxa = P.gx_a + (size_t)(dir * SLICES + slice) * Rp * UM;
-    const float* gxb = P.gx_b ? P.gx_b + (size_t)(dir * SLICES + slice) * Rp * UM : nullptr;
-
-    if (warp < REC_EPI_WARPS) {
-        // =========================================================== epilogue warps of tile slot `slot`
-        const int slot = warp >> 3;
-        const int half = (warp >> 2) & 1;           // sequences [32 half, 32 half + 32) of the tile
-        const int wq = warp & 3;                    // TMEM lane quarter = gate type (i, f, g, o)
-        const int et = wq * 32 + lane;              // thread index inside the (slot, half) warpgroup (0..127)
-        const int bar_id = 1 + slot * 2 + half;     // named barrier of this warpgroup
-        float* gs = gate_s + slot * (GATE_BYTES / 4) + half * (GATE_BYTES / 8);
-        int* ls = len_s + slot * NSEQ;
-        const uint32_t acc_addr = tmem_base + ((uint32_t)(wq * 32) << 16) + (uint32_t)(ACC_COL0 + slot * NSEQ + half * 32);
-        const int ucol = slice * 32 + lane;         // hidden unit of this thread in the cell-update phase
-        unsigned* counter = P.counter + (size_t)group * 2 + slot;
-        uint32_t q = 0;                             // global step index of this (group, slot)
-        const int64_t items = n_items(slot);
-        const bool prof_on = blockIdx.x == 0 && tid == 0;           // diagnostics: cycles of CTA 0's slot-0 epilogue thread 0
-        long long pf[4] = {0, 0, 0, 0}, tc = prof_on ? clock64() : 0;
-        for (int64_t it = 0; it < items; ++it) {
-            const int64_t bt = gd + (2 * it + slot) * groups_dir;
-            const int64_t b0 = bt * NSEQ;
-            if (et < 32) { const int64_t b = b0 + half * 32 + et; ls[half * 32 + et] = b < P.B ? P.len[b] : 0; }
-            named_bar(bar_id, 128);
-            float c_reg[8], h_reg[8];
+    const int slot = warp >> 2, wq = warp & 3;
+    const int et = wq * 32 + lane;                                 // thread index inside the slot's warpgroup
+    const int g = lane >> 2, c = lane & 3;
+    const int unit = wq * 8 + g;                                   // hidden unit (inside the slice) of this thread
+    const int ucol = slice * 32 + unit;
+    const int f0 = wq * 32 + 4 * g;                                // its gate columns i, f, g, o in the packed slice
+    const int bar_id = 1 + slot;
+    const int64_t Rp = (int64_t)P.T * P.Bp;
+    const float* gxa = P.gx_a + (size_t)(dir * SLICES + slice) * Rp * UM + f0;
+    const float* gxb = P.gx_b ? P.gx_b + (size_t)(dir * SLICES + slice) * Rp * UM + f0 : nullptr;
+    const float* whh = P.whh + (size_t)(dir * SLICES + slice) * LH * UM;
+    int* ls = len_s + slot * NSEQ;
+    unsigned* counter = P.counter + (size_t)group * 2 + slot;
+    const uint32_t op_u32 = smem_base + (uint32_t)(slot * TILE_BYTES_H);
+    // tile sequence of (group, slot): bt = gd + (2 * i + slot) * groups_dir, i = 0, 1, ...
+    const int64_t first = gd + (int64_t)slot * groups_dir;
+    const int64_t items = first < P.n_bt ? (P.n_bt - first + 2 * groups_dir - 1) / (2 * groups_dir) : 0;
+    uint32_t q = 0, fetched = 0;                                   // steps published / operand fetches waited for
+    for (int64_t it = 0; it < items; ++it) {
+        const int64_t bt = gd + (2 * it + slot) * groups_dir;
+        const int64_t b0 = bt * NSEQ;
+        named_bar(bar_id, 128);                                    // the previous tile's last reads of ls are done
+        if (et < NSEQ) { const int64_t b = b0 + et; ls[et] = b < P.B ? P.len[b] : 0; }
+        named_bar(bar_id, 128);
+        float c_reg[16], h_reg[16];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) { c_reg[j] = 0.f; h_reg[j] = 0.f; }
-            for (int step = 0; step < P.T; ++step, ++q) {
-                const int t = dir ? (P.T - 1 - step) : step;
-                unsigned char* tile = P.out_img + ((size_t)t * P.n_bt + bt) * (2 * TILE_BYTES_H) + (size_t)dir * TILE_BYTES_H;
-                mbar_wait(accf_bar(slot), q & 1u);
-                tc_fence_after();
-                if (prof_on) { const long long c_ = clock64(); pf[0] += c_ - tc; tc = c_; }      // waiting for the MMAs
-                uint32_t v0[16], v1[16];
-                tmem_ld16(acc_addr, v0);
-                tmem_ld16(acc_addr + 16, v1);
-                tmem_wait_ld();
-                tc_fence_before();
-                mbar_arrive(drained_bar(slot));                     // this thread has read all of its accumulator columns
+        for (int j = 0; j < 16; ++j) { c_reg[j] = 0.f; h_reg[j] = 0.f; }
+        for (int step = 0; step < P.T; ++step, ++q) {
+            const int t = dir ? (P.T - 1 - step) : step;
+            // ---- accumulator <- G_x[:, t] (rows of the padded time-major matrix: always in range)
+            float d[2][32];
+            const size_t rbase = (size_t)((int64_t)t * P.Bp + b0) * UM;
 #pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                    // phase A: activated gates of this thread's gate row for 16 sequences -> shared [gate][seq][unit]
+            for (int nb = 0; nb < 8; ++nb)
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) {
-                        const float x = __uint_as_float(c == 0 ? v0[j] : v1[j]);
-                        gs[(wq * 16 + j) * 32 + lane] = (wq == 2) ? tanh_fast(x) : sigmoid_fast(x);
+                for (int e = 0; e < 2; ++e) {
+                    const size_t off = rbase + (size_t)(8 * nb + 2 * c + e) * UM;
+                    float4 v = __ldg(reinterpret_cast<const float4*>(gxa + off));
+                    if (gxb) {
+                        const float4 w = __ldg(reinterpret_cast<const float4*>(gxb + off));
+                        v.x += w.x; v.y += w.y; v.z += w.z; v.w += w.w;
                     }
-                    named_bar(bar_id, 128);
-                    // phase B: cell update, thread = (unit lane, sequences wq*4 .. wq*4+3 of the chunk)
-#pragma unroll
-                    for (int jj = 0; jj < 4; ++jj) {
-                        const int j = wq * 4 + jj;                 // sequence inside the chunk
-                        const int n = half * 32 + c * 16 + j;      // sequence inside the tile
-                        const float ig = gs[(0 * 16 + j) * 32 + lane], fg = gs[(1 * 16 + j) * 32 + lane];
-                        const float gg = gs[(2 * 16 + j) * 32 + lane], og = gs[(3 * 16 + j) * 32 + lane];
-                        float& cr = c_reg[c * 4 + jj];
-                        float& hr = h_reg[c * 4 + jj];
-                        if (t < ls[n]) {
-                            cr = fmaf(fg, cr, ig * gg);
-                            hr = og * tanh_fast(cr);
-                        }
-                        // h (state, kept when masked) -> three bf16 terms -> output image = exchange; even lanes store the
-                        // pair.  Masked positions of the layer output are never read by the next layer (its own steps
-                        // are masked there), so the kept state is as good as the zero packed sequences would hold.
-                        float r = hr;
-                        uint32_t term[NS];
-#pragma unroll
-                        for (int p = 0; p < NS; ++p) {
-                            const __nv_bfloat16 hb = __float2bfloat16_rn(r);
-                            term[p] = (uint32_t)__bfloat16_as_ushort(hb);
-                            r -= __bfloat162float(hb);
-                        }
-                        unsigned char* dstp = tile + b_elem_offset(n, ucol);
-#pragma unroll
-                        for (int p = 0; p < NS; ++p) {
-                            const uint32_t nb = __shfl_down_sync(0xffffffffu, term[p], 1);
-                            if (!(lane & 1)) *reinterpret_cast<uint32_t*>(dstp + p * PLANE_BYTES_H) = term[p] | (nb << 16);
-                        }
-                    }
-                    named_bar(bar_id, 128);                         // the gate buffer is reused by the next chunk
+                    d[0][4 * nb + e] = v.x; d[0][4 * nb + 2 + e] = v.y; d[1][4 * nb + e] = v.z; d[1][4 * nb + 2 + e] = v.w;
                 }
-                if (prof_on) { const long long c_ = clock64(); pf[1] += c_ - tc; tc = c_; }      // activations + cell update + stores
-                fence_proxy_async_all();                            // generic stores above are read by bulk (async-proxy) copies
-                named_bar(5 + slot, 256);                           // both halves of the slot have written their h
-                if (half == 0 && et == 0) {
-                    __threadfence();
-                    atomicAdd(counter, 1u);                          // release: this CTA's h_t slice is published
-                }
-                if (prof_on) { const long long c_ = clock64(); pf[2] += c_ - tc; tc = c_; }      // fences + publish
+            // ---- + W_slice . h_{t-1} (h_{-1} = 0: the first step is G_x alone)
+            if (step > 0) {
+                mbar_wait(opfull_bar(slot), fetched & 1u);
+                ++fetched;
+                mma_tile<KSTEPS_H>(d, whh, op_u32, (uint32_t)PLANE_BYTES_H, true, wq, lane);
             }
-            // final state of the tile
+            // ---- cell update in registers; h (state, kept when masked) -> three bf16 terms -> output image = exchange.
+            // Masked positions of the layer output are never read by the next layer (its own steps are masked there).
+            unsigned char* tile = P.out_img + ((size_t)t * P.n_bt + bt) * (2 * TILE_BYTES_H) + (size_t)dir * TILE_BYTES_H;
 #pragma unroll
-            for (int c = 0; c < 2; ++c)
+            for (int nb = 0; nb < 8; ++nb)
 #pragma unroll
-                for (int jj = 0; jj < 4; ++jj) {
-                    const int64_t b = b0 + half * 32 + c * 16 + wq * 4 + jj;
-                    if (b < P.B) P.hfin[b * (2 * LH) + dir * LH + ucol] = h_reg[c * 4 + jj];
-                }
-        }
-        if (prof_on) for (int i = 0; i < 3; ++i) P.counter[128 + i] = (unsigned)(pf[i] >> 6);
-    } else if (warp == REC_MMA_WARP) {
-        // =========================================================== MMA issuer (one thread), slots interleaved
-        if (lane == 0) {
-            const uint32_t total[2] = {(uint32_t)(n_items(0) * P.T), (uint32_t)(n_items(1) * P.T)};
-            uint32_t q[2] = {0, 0};
-            uint32_t idle = 0;
-            while (q[0] < total[0] || q[1] < total[1]) {
-                bool issued = false;
-#pragma unroll
-                for (int s = 0; s < 2; ++s) {
-                    // whichever tile is ready goes next: accumulator holds G_x[:, t] AND the B operand holds h_{t-1}
-                    if (q[s] >= total[s] || !mbar_try(accinit_bar(s), q[s] & 1u) || !mbar_try(opfull_bar(s), q[s] & 1u)) continue;
-                    tc_fence_after();
-                    issue_tile_mmas<KSTEPS_H>(tmem_base + (uint32_t)(ACC_COL0 + s * NSEQ), tmem_base, W_PART_COLS,
-                                              smem_base + (uint32_t)(s * TILE_BYTES_H), (uint32_t)PLANE_BYTES_H, true);
-                    umma_commit(accf_bar(s));
-                    ++q[s];
-                    issued = true;
-                }
-                if (issued) idle = 0;
-                else if (++idle > (1u << 24)) __trap();                  // bounded: a protocol bug ends in a launch error
-            }
-        }
-    } else {
-        // =========================================================== accumulator-init warps + the slot's exchange thread
-        const int slot = (warp - REC_INIT_WARP0) >> 2;
-        const int wq = warp & 3;                       // TMEM lane quarter this warp may touch (warp % 4)
-        const int pt = ((warp - REC_INIT_WARP0) & 3) * 32 + lane;     // 0..127 inside the slot's init warpgroup
-        const int gcol = wq * 32 + lane;               // gate row inside the slice = column of the G_x slab
-        const uint32_t acc_addr = tmem_base + ((uint32_t)(wq * 32) << 16) + (uint32_t)(ACC_COL0 + slot * NSEQ);
-        unsigned* counter = P.counter + (size_t)group * 2 + slot;
-        unsigned char* op_gen = smem_gen + (size_t)slot * TILE_BYTES_H;
-        const uint32_t op_u32 = smem_base + (uint32_t)(slot * TILE_BYTES_H);
-        uint32_t q = 0;
-        const int64_t items = n_items(slot);
-        const bool prof_on = blockIdx.x == 0 && slot == 0 && pt == 0;
-        long long pf[4] = {0, 0, 0, 0}, tc = prof_on ? clock64() : 0;
-        for (int64_t it = 0; it < items; ++it) {
-            const int64_t bt = gd + (2 * it + slot) * groups_dir;
-            const int64_t b0 = bt * NSEQ;
-            for (int step = 0; step < P.T; ++step, ++q) {
-                const int t = dir ? (P.T - 1 - step) : step;
-                if (prof_on) tc = clock64();
-                // ---- accumulator <- G_x[:, t] (rows of the padded time-major matrix: always in range)
-                const float* ra = gxa + (size_t)((int64_t)t * P.Bp + b0) * UM + gcol;
-                const float* rb = gxb ? gxb + (size_t)((int64_t)t * P.Bp + b0) * UM + gcol : nullptr;
-#pragma unroll 1
-                for (int c = 0; c < 4; ++c) {
-                    float ga[16];
-#pragma unroll
-                    for (int j = 0; j < 16; ++j) ga[j] = __ldg(ra + (size_t)(c * 16 + j) * UM);
-                    if (rb) {
-                        float gb[16];
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) gb[j] = __ldg(rb + (size_t)(c * 16 + j) * UM);
-#pragma unroll
-                        for (int j = 0; j < 16; ++j) ga[j] += gb[j];
+                for (int e = 0; e < 2; ++e) {
+                    const int n = 8 * nb + 2 * c + e;                  // sequence inside the tile
+                    const int j = 2 * nb + e;
+                    if (t < ls[n]) {
+                        const float ig = sigmoid_fast(d[0][4 * nb + e]), fg = sigmoid_fast(d[0][4 * nb + 2 + e]);
+                        const float gg = tanh_fast(d[1][4 * nb + e]), og = sigmoid_fast(d[1][4 * nb + 2 + e]);
+                        c_reg[j] = fmaf(fg, c_reg[j], ig * gg);
+                        h_reg[j] = og * tanh_fast(c_reg[j]);
                     }
-                    if (c == 0 && q > 0) {                           // the epilogue of step q-1 has drained the accumulator
-                        if (prof_on) { const long long c_ = clock64(); pf[0] += c_ - tc; tc = c_; }   // G_x loads issued + landed
-                        mbar_wait(drained_bar(slot), (q - 1) & 1u);
-                        tc_fence_after();
-                        if (prof_on) { const long long c_ = clock64(); pf[1] += c_ - tc; tc = c_; }   // waiting for the drain
-                    }
-                    uint32_t v[16];
+                    float r = h_reg[j];
+                    uint32_t term[NS];
 #pragma unroll
-                    for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(ga[j]);
-                    tmem_st16(acc_addr + (uint32_t)(c * 16), v);
+                    for (int p = 0; p < NS; ++p) {
+                        const __nv_bfloat16 hb = __float2bfloat16_rn(r);
+                        term[p] = (uint32_t)__bfloat16_as_ushort(hb);
+                        r -= __bfloat162float(hb);
+                    }
+                    unsigned char* dstp = tile + b_elem_offset(n, ucol);
+#pragma unroll
+                    for (int p = 0; p < NS; ++p) {                      // units (even, odd) = lanes (l, l + 4): one 4-byte store
+                        const uint32_t nbv = __shfl_down_sync(0xffffffffu, term[p], 4);
+                        if (!(g & 1)) *reinterpret_cast<uint32_t*>(dstp + p * PLANE_BYTES_H) = term[p] | (nbv << 16);
+                    }
                 }
-                tmem_wait_st();
-                tc_fence_before();
-                mbar_arrive(accinit_bar(slot));
-
-                // ---- B operand <- h_{t-1}
-                if (step == 0) {
-                    // (the MMAs of the previous tile's last step have retired: its epilogue ran, and this warpgroup waited
-                    // for that epilogue's drained barrier above)
-                    named_bar(7 + slot, 128);
-                    const uint4 z = make_uint4(0u, 0u, 0u, 0u);
-                    for (int i = pt; i < TILE_BYTES_H / 16; i += 128) reinterpret_cast<uint4*>(op_gen)[i] = z;
-                    fence_proxy_async();
-                    named_bar(7 + slot, 128);
-                    if (pt == 0) mbar_arrive(opfull_bar(slot));
-                } else if (pt == 0) {
-                    // every CTA of the group has published step q-1 of this slot (so this CTA's MMA of step q-1, which
-                    // read the operand buffer, has retired as well)
-                    const unsigned want = (unsigned)SLICES * q;
-                    if (prof_on) { const long long c_ = clock64(); pf[2] += c_ - tc; tc = c_; }       // second chunk + tmem st
+            fence_proxy_async_all();                                  // generic stores above are read by bulk (async-proxy) copies
+            named_bar(bar_id, 128);                                   // the whole slice of h_t is written, every MMA has retired
+            if (et == 0) {
+                __threadfence();
+                atomicAdd(counter, 1u);                               // release: this CTA's h_t slice is published
+                if (step + 1 < P.T) {
+                    // every CTA of the group has published this step: fetch the whole h_t tile as the next B operand
+                    const unsigned want = (unsigned)SLICES * (q + 1);
                     for (uint32_t spin = 0; ld_acquire(counter) < want; ++spin) {
                         if (spin > 64) __nanosleep(32);
                         if (spin > (1u << 25)) __trap();
                     }
-                    if (prof_on) { const long long c_ = clock64(); pf[3] += c_ - tc; tc = c_; }       // polling the group's counter
-                    fence_proxy_async_all();                         // acquired generic writes -> async-proxy reads
-                    const int tp = dir ? t + 1 : t - 1;              // the step that produced h_{t-1}
-                    const unsigned char* src = P.out_img + ((size_t)tp * P.n_bt + bt) * (2 * TILE_BYTES_H) + (size_t)dir * TILE_BYTES_H;
+                    fence_proxy_async_all();                          // acquired generic writes -> async-proxy reads
                     mbar_arrive_expect_tx(opfull_bar(slot), (uint32_t)TILE_BYTES_H);
 #pragma unroll 1
                     for (int i = 0; i < TILE_BYTES_H / 16384; ++i)
-                        bulk_g2s(op_u32 + (uint32_t)(i * 16384), src + (size_t)i * 16384, 16384u, opfull_bar(slot));
+                        bulk_g2s(op_u32 + (uint32_t)(i * 16384), tile + (size_t)i * 16384, 16384u, opfull_bar(slot));
                 }
             }
         }
-        if (prof_on) for (int i = 0; i < 4; ++i) P.counter[136 + i] = (unsigned)(pf[i] >> 6);
+        // final state of the tile
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+            const int64_t b = b0 + 8 * (j >> 1) + 2 * c + (j & 1);
+            if (b < P.B) P.hfin[b * (2 * LH) + dir * LH + ucol] = h_reg[j];
+        }
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == REC_MMA_WARP) { tc_fence_after(); tmem_dealloc(tmem_base, TMEM_COLS); }
 }
 
 // ---------------------------------------------------------------- packing kernels
-// Wt [K_src, 1024] (k-major, gate g = w*256 + unit) -> [8 slices][K_dst][128]:
-// dst[s][k][w*32+u] = (k < k_real) ? Wt[(k_lo + k) * 1024 + w*256 + s*32 + u] : 0
+// Wt [K_src, 1024] (k-major, gate row = w*256 + unit) -> [8 slices][K_dst][128], slice column = 4 u + w (the four gates
+// of one unit side by side):  dst[s][k][4u+w] = (k < k_real) ? Wt[(k_lo + k) * 1024 + w*256 + s*32 + u] : 0
 __global__ void pack_slices_kernel(const float* __restrict__ Wt, int k_lo, int k_real, int K_dst, float* __restrict__ dst) {
     const int total = SLICES * K_dst * UM;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
         const int j = i % UM, k = (i / UM) % K_dst, s = i / (UM * K_dst);
-        const int g = (j >> 5) * LH + s * 32 + (j & 31);
+        const int g = (j & 3) * LH + s * 32 + (j >> 2);
         dst[i] = k < k_real ? Wt[(size_t)(k_lo + k) * (4 * LH) + g] : 0.f;
     }
 }
@@ -677,7 +461,7 @@ __global__ void pack_bias_kernel(const float* __restrict__ bias, float* __restri
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < SLICES * UM) {
         const int j = i % UM, s = i / UM;
-        dst[i] = bias[(j >> 5) * LH + s * 32 + (j & 31)];
+        dst[i] = bias[(j & 3) * LH + s * 32 + (j >> 2)];
     }
 }
 
@@ -719,7 +503,7 @@ int launch_proj(const ProjArgs& a, cudaStream_t st) {
         NERRF_CHECK_CUDA(cudaFuncSetAttribute(lstm_proj_kernel<KB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set_dev[dev_ & 63] = true;
     }
-    lstm_proj_kernel<KB><<<16 * a.ctas_per_combo, 192, smem, st>>>(a);
+    lstm_proj_kernel<KB><<<16 * a.ctas_per_combo, PROJ_THREADS, smem, st>>>(a);
     return launch_status("lstm_proj_kernel");
 }
 
@@ -791,15 +575,6 @@ int lstm_layers_umma(const float* seq, const int32_t* len, int64_t B, int T, int
         void* args[] = {&r};
         NERRF_CHECK_CUDA(cudaLaunchCooperativeKernel((const void*)lstm_rec_kernel, dim3(groups * SLICES), dim3(REC_THREADS), args,
                                                      REC_SMEM, st));
-        if (getenv("NERRF_LSTM_PROF")) {           // diagnostics: phase cycle counts of CTA 0 (see lstm_rec_kernel)
-            unsigned h[16];
-            NERRF_CHECK_CUDA(cudaStreamSynchronize(st));
-            NERRF_CHECK_CUDA(cudaMemcpy(h, counter + 128, sizeof(h), cudaMemcpyDeviceToHost));
-            const double steps = (double)T * ((n_bt + (groups / 2) * 2 - 1) / ((groups / 2) * 2));
-            fprintf(stderr, "[lstm prof] layer %d, cycles per step of CTA 0 / slot 0: epilogue wait-MMA %.0f, compute %.0f, fence+publish %.0f | "
-                            "init: G_x loads %.0f, wait-drain %.0f, st+arrive %.0f, poll %.0f\n", l, h[0] * 64.0 / steps, h[1] * 64.0 / steps,
-                    h[2] * 64.0 / steps, h[8] * 64.0 / steps, h[9] * 64.0 / steps, h[10] * 64.0 / steps, h[11] * 64.0 / steps);
-        }
     }
     return launch_status("lstm_rec_kernel");
 }

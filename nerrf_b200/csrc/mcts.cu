@@ -26,7 +26,7 @@
 namespace nerrf {
 
 constexpr int MAXD = 256;
-constexpr int MCTS_THREADS = 896;     // 28 warps: one CTA per SM covers 4096 rollouts in a single pass (148 x 28)
+constexpr int MCTS_THREADS = 896;     // 28 warps, one CTA per SM (72 registers: 896 threads fill the register file)
 constexpr int MCTS_WARPS = MCTS_THREADS / 32;
 constexpr int MAXR = 8192;
 
@@ -382,8 +382,7 @@ __global__ void __launch_bounds__(MCTS_THREADS) mcts_search_kernel(MctsArgs P) {
 
         // ------------------------------------------------------------------ rollouts (warp per rollout)
         // (8 lanes per rollout / 4 rollouts per warp was tried: the per-step chain of dependent collectives got LONGER --
-        // the n-th-set-bit search has to run inside one lane -- and with 7 instead of 28 warps per SM nothing hid it:
-        // 54 k instead of 30 k cycles for the phase, profiles/r02_mcts.md)
+        // the n-th-set-bit search has to run inside one lane -- and with 7 instead of 28 warps per SM nothing hid it)
         // RANK-SPACE rollouts (round 2): a rollout applies "the j_k-th still-legal action" left times.  Instead of updating
         // the warp-distributed bitset at every step (ballot -> ffs -> 2 shfl -> popc -> ballot -> ffs: a chain of dependent
         // collectives, ~35 instructions), the picks are kept as a SORTED list of ranks among the leaf's legal actions, one

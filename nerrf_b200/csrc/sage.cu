@@ -4,7 +4,7 @@
 //   K2  [x_v || m_v] @ W + b, ReLU            -- fused with K1: the aggregate tile is written
 //       straight into the shared-memory A operand and never round-trips HBM.
 // This file holds the fp32 CUDA-core (FFMA) fused kernel, the standalone K1, the heads, the
-// whole-forward driver and the host-buffer session.  The tcgen05 fused kernel is sage_umma.cu.
+// whole-forward driver and the host-buffer session.  The tensor-core (wgmma) fused kernel is sage_umma.cu.
 #include "common.cuh"
 #include "sage_gather.cuh"
 
@@ -290,8 +290,8 @@ static int layer_fwd_impl(const float* x, const void* rowptr, int rowptr_is64, c
     if (rc) return rc;
     NERRF_REQUIRE(W && b && out, "null weight/output pointer");
     NERRF_REQUIRE(H == HH, "hidden width must be 128 (got %d)", H);
-    NERRF_REQUIRE(((uintptr_t)out & 15) == 0 && ((uintptr_t)W & 15) == 0 && ((uintptr_t)b & 15) == 0,
-                  "out/W/b must be 16-byte aligned");
+    NERRF_REQUIRE(((uintptr_t)out & 15) == 0 && ((uintptr_t)W & 15) == 0 && ((uintptr_t)b & 15) == 0 &&
+                  ((uintptr_t)node_w & 15) == 0, "out/W/b/node_w must be 16-byte aligned");
     NERRF_REQUIRE(x != out, "in-place layer is not supported");
     NERRF_REQUIRE(!node_w || score, "score output required with node_w");
     cudaStream_t st = (cudaStream_t)stream;
@@ -302,7 +302,7 @@ static int layer_fwd_impl(const float* x, const void* rowptr, int rowptr_is64, c
         return sage_layer_umma(x, rowptr, rowptr_is64, col, ew, W, b, out, n_nodes, row_begin, row_end, F, relu,
                                algo == NERRF_SAGE_ALGO_UMMA ? 3 : 2, node_w, node_b, score, long_ws, long_ws_bytes,
                                reuse_scan, peer_out, n_peers, peer_need, st);
-    NERRF_REQUIRE(n_peers == 0, "the fused peer exchange needs the tcgen05 layer (algo umma)");
+    NERRF_REQUIRE(n_peers == 0, "the fused peer exchange needs the tensor-core layer (algo umma)");
     NERRF_REQUIRE(algo == NERRF_SAGE_ALGO_FFMA, "unknown algo %d", algo);
     rc = rowptr_is64
              ? layer_dispatch<int64_t>(x, (const int64_t*)rowptr, col, ew, W, b, out, row_begin, row_end, F, relu, st)

@@ -1,5 +1,5 @@
 // K1 inner loop: weighted-mean gather of one CSR row by one warp (SURVEY.md 8a row a2).  Used by the fp32
-// cross-check layer, the standalone aggregate and the hub-row chunk pre-pass; the tcgen05 layer has its own
+// cross-check layer, the standalone aggregate and the hub-row chunk pre-pass; the tensor-core (wgmma) layer has its own
 // cp.async ring pipeline (sage_umma.cu).
 //
 // A source row is F floats = F/4 float4.  LPR = F/4 lanes cover one source row with one 16-byte

@@ -1,36 +1,38 @@
-// Fused GraphSAGE-T layer on 5th-gen tensor cores (tcgen05 / TMEM), sm_100a only.
+// Fused GraphSAGE-T layer on Hopper tensor cores (wgmma), sm_90a.
 //
 //   out[v, :] = act( [x_v || m_v] @ W + b ),   m_v = weighted mean of gathered source rows
 //
-// computed TRANSPOSED so that the small, reused operand lives in tensor memory:
+// computed TRANSPOSED so that the gathered tile is the shared-memory operand and the weights travel in registers:
 //
-//   D^T[H=128 features, rows] = W^T[128, K=2F] . X^T[K, rows]
-//     A operand = W^T, resident in TMEM for the whole (persistent) kernel, bf16 hi and lo halves
-//                 (lane = feature, two K elements per 32-bit column)
-//     B operand = the gathered tile X[rows, K] exactly as the gather warps produce it: row-major,
-//                 K contiguous == the UMMA "K-major" canonical layout (128-byte swizzle), bf16 hi/lo
-//     D         = fp32 accumulator in TMEM, [128 lanes x 64 columns] per tile, double buffered
+//   D^T[H=128 features, rows] = W^T[128, K=2F] . X^T[K, rows]      (one m64n32k16 wgmma half per consumer warpgroup)
+//     A operand = W^T, register fragments split into bf16 terms once per launch (split_w_kernel) and read from L2 by the
+//                 consumer warpgroups: the split W^T of an F=128 layer (192 KB) does not fit in shared memory next to
+//                 the gather rings and operand stages, and Hopper has no tensor memory to hold it
+//     B operand = the gathered tile X[rows, K] exactly as the gather warps produce it: row-major, K contiguous ==
+//                 the wgmma "K-major" canonical layout (128-byte swizzle), bf16 terms
+//     D         = fp32 accumulators in the consumer warpgroups' registers
 //
-// fp32-level accuracy from bf16 tensor cores (the north star's 1e-4 bound rules out plain
-// TF32/bf16): every fp32 value v is split v = hi + lo (hi = bf16(v), lo = bf16(v - hi)) and
-// three MMAs accumulate x_hi.w_hi + x_lo.w_hi + x_hi.w_lo in fp32 (error ~1e-5 relative).
+// fp32-level accuracy from bf16 tensor cores (the 1e-4 bound rules out plain TF32/bf16): every fp32 value v is split
+// v = hi + lo (hi = bf16(v), lo = bf16(v - hi)) and the products x_hi.w_hi + x_lo.w_hi + x_hi.w_lo are accumulated in
+// fp32 (error ~1e-5 relative); NS = 3 terms with six products is fp32-equivalent.
 //
-// The aggregate never round-trips HBM: gather warps write hi/lo bf16 straight into the shared
-// memory B operand.  Warp roles in one CTA per SM (512 threads):
-//   warps 0-3   epilogue: tcgen05.ld accumulator (lane = feature), + bias, ReLU, 128 B/warp stores
-//   warp  4     TMEM allocator + single-thread MMA issuer (tcgen05.mma, commit -> mbarriers)
-//   warp  5     edge-block loader: stages each tile's rowptr words and its col / ew slices into shared memory --
+// The aggregate never round-trips HBM: gather warps write hi/lo bf16 straight into the shared memory B operand.
+// Warp roles in one CTA per SM:
+//   warps 0-7   two consumer warpgroups (output features 0-63 and 64-127): wgmma (A in registers, B from shared
+//               memory), then the epilogue from the accumulator registers: + bias, ReLU, row stores, fused node head
+//   warp  8     edge-block loader: stages each tile's rowptr words and its col / ew slices into shared memory --
 //               the slices as two BULK async copies (cp.async.bulk, byte count on the stage's mbarrier) --
 //               running up to IDX_STAGES tiles ahead; the next tile's rowptr words are prefetched before it
 //               waits for a free stage
-//   warps 6-..  gather: one CSR row per warp at a time, rows round-robin; every source row (512 B at F=128,
-//               128 B at F=32) is ONE bulk async copy into the warp's shared-memory ring, completion counted in
-//               bytes on the ring slot's mbarrier (the "TMA-staged edge block" of the north star); indices come
-//               from shared memory, so the only global latency a row exposes is its x rows
-// Pipelines: idx stages full/empty (loader <-> gather), smem operand stages full/empty (gather <-> MMA),
-// TMEM accumulators full/empty (MMA <-> epilogue).
+//   warps 9-..  gather: one CSR row per warp at a time, rows round-robin; source rows are copied into the warp's
+//               shared-memory ring with cp.async (16 B per lane) or, as an option, one bulk async copy per row;
+//               indices come from shared memory, so the only global latency a row exposes is its x rows
+// Pipelines: idx stages full/empty (loader <-> gather), smem operand stages full/empty (gather <-> consumer).
 #include <cuda_bf16.h>
 #include <stdlib.h>
+#include <map>
+#include <mutex>
+#include <utility>
 #include "common.cuh"
 #include "sage_gather.cuh"
 
@@ -38,12 +40,11 @@ namespace nerrf {
 
 namespace {
 
-constexpr int TN = 32;                 // destination rows per tile (UMMA N)
-constexpr int UM = 128;                // UMMA M = hidden width
-constexpr int EPI_WARPS = 4;
-constexpr int MMA_WARP = 4;
-constexpr int LOADER_WARP = 5;
-constexpr int GATHER_WARP0 = 6;
+constexpr int TN = 32;                 // destination rows per tile (wgmma N)
+constexpr int UM = 128;                // hidden width = two wgmma M=64 halves
+constexpr int EPI_WARPS = 8;           // two consumer warpgroups, one per 64-feature half of the output
+constexpr int LOADER_WARP = 8;
+constexpr int GATHER_WARP0 = 9;
 constexpr int EMAX = 512;              // staged edges per tile (4 KB); the rest of a heavier tile is read from global
 constexpr int EPAD = EMAX + 4;         // a slice is copied as its 16-byte aligned superset: up to 3 leading + 3 trailing elements
 constexpr int IDX_STAGE_BYTES = EPAD * 8 + 512;      // col[EPAD] | ew[EPAD] | rp[TN+1] (relative) | e_lo (int64) | col_off, ew_off
@@ -56,15 +57,12 @@ constexpr int NQ = 4;                  // sub-batch slots in a warp's ring; NQ-1
 // terms below 2^-24: fp32-equivalent.  NS = 2 with three products is ~1e-5 relative.
 template <int F, int NS>
 struct UmmaCfg {
-#ifdef NERRF_EXP_GW128                                            // experiment knob (scripts/exp_gather_warps.sh): fewer gather warps at F=128
-    static constexpr int GATHER_WARPS = (F == 32) ? 18 : (F == 128 ? NERRF_EXP_GW128 : 14);
-#else
-    static constexpr int GATHER_WARPS = (F == 32) ? 18 : 14;  // F=32 leaves room for more rings (and needs more TLP)
-#endif
+    static constexpr int GATHER_WARPS = (F == 32) ? 16 : 14;  // F=32 leaves room for more rings (and needs more TLP);
+                                                                // 25 warps keep 80 registers per thread
     static constexpr int THREADS = (GATHER_WARP0 + GATHER_WARPS) * 32;
     // F = 32 (quad-mode gather): a warp runs up to 3 units = ~7 tiles ahead of what it has consumed and holds a tile's edge
     // block from issue to completion, so the look-ahead is bounded by the number of edge-block stages, not by the rings
-    // (ncu r2g: with 4 stages 77 % of the issue-side polls found the next tile not staged)
+    // (with 4 stages most issue-side polls find the next tile not yet staged)
     static constexpr int IDX_STAGES = (F == 32) ? 9 : 3;
     static constexpr int K = 2 * F;
     static constexpr int KB = K / 64;                        // 128-byte K blocks
@@ -74,14 +72,10 @@ struct UmmaCfg {
     static constexpr int QS = qs_for<F>();                    // 4 (F=128), 8 (F=64), 16 (F=32): always 2 KB per sub-batch
     static constexpr int RING_BYTES = NQ * QS * F * 4;       // per gather warp: NQ sub-batches x QS source rows
     static constexpr int STAGES = (F == 128) ? 2 : (F == 32 ? 3 : 4);
-    static constexpr int W_PART_COLS = K / 2;                // W^T term p lives in TMEM columns [p*K/2, (p+1)*K/2)
-    static constexpr int ACC_COL0 = NS * W_PART_COLS;
-    static constexpr int TMEM_COLS = (ACC_COL0 + 2 * TN <= 256) ? 256 : 512;
     static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + IDX_STAGES * IDX_STAGE_BYTES +
-                                   (size_t)GATHER_WARPS * RING_BYTES + 1024 /*head reduce*/ + 1024 /*align*/ + 1024 /*barriers*/;
+                                   (size_t)GATHER_WARPS * RING_BYTES + 2048 /*head reduce*/ + 1024 /*align*/ + 1024 /*barriers*/;
     static_assert(SMEM <= 227 * 1024, "shared memory budget");
     static_assert(STAGES >= 2, "need at least two smem stages");
-    static_assert(ACC_COL0 + 2 * TN <= 512, "TMEM overflow");
 };
 
 // ---------------------------------------------------------------- PTX wrappers
@@ -117,7 +111,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
             : "memory");
     } while (!done);
 }
-// for the roles that have slack (epilogue, MMA issuer, loader): poll with a sleep so they do not burn
+// for the roles that have slack (consumer warpgroups, loader): poll with a sleep so they do not burn
 // the issue slots the gather warps need (a tile period is ~10 us)
 __device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity) {
     uint32_t done;
@@ -150,61 +144,33 @@ template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[tmem] . B[smem desc]^T   (kind::f16: bf16 inputs, fp32 accumulate)
-__device__ __forceinline__ void umma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-                 ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-
-// UMMA shared-memory descriptor: K-major, SWIZZLE_128B, 8-row groups 1024 B apart (SBO), version 1.
+// wgmma shared-memory matrix descriptor (sm_90): K-major, SWIZZLE_128B, 8-row groups 1024 B apart (SBO); the leading
+// byte offset is unused for swizzled K-major operands.  A K step inside the 128-byte swizzle atom advances the start
+// address by 32 bytes (the atom itself is 1024-byte aligned).
 __device__ __forceinline__ uint64_t make_b_desc(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);          // start address
-    d |= (uint64_t)1 << 16;                               // LBO (unused for swizzled K-major)
+    d |= (uint64_t)1 << 16;                               // LBO (unused)
     d |= (uint64_t)(1024 >> 4) << 32;                     // SBO = 1024 B
-    d |= (uint64_t)1 << 46;                               // descriptor version (sm_100)
-    d |= (uint64_t)2 << 61;                               // SWIZZLE_128B
+    d |= (uint64_t)1 << 62;                               // SWIZZLE_128B
     return d;
 }
-// Instruction descriptor: D=f32, A=B=bf16, both K-major, N = TN, M = 128.
-__host__ __device__ constexpr uint32_t make_idesc() {
-    return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(UM >> 4) << 24);
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 x 32] (+)= A[64 x 16] (bf16 register fragment) . B[16 x 32] (bf16, K-major shared memory), fp32 accumulate
+__device__ __forceinline__ void wgmma_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "{%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)
+        : "memory");
 }
 
 // split fp32 values into NS bf16 terms of the running residual; pairs packed (first element low)
@@ -229,22 +195,6 @@ __device__ __forceinline__ void split4(const float4 v, uint2 (&parts)[NS]) {
     for (int p = 0; p < NS; ++p) parts[p] = make_uint2(lo[p], hi[p]);
 }
 
-// v[j] (j = 0..31) per lane  ->  sum over the 32 lanes of v[lane]: a 32x32 transpose-reduce in 31 shuffles
-__device__ __forceinline__ float warp_transpose_reduce32(float (&v)[32], int lane) {
-#pragma unroll
-    for (int s = 0; s < 5; ++s) {
-        const int n = 16 >> s;                                  // also the xor offset
-        const bool up = (lane & n) != 0;
-#pragma unroll
-        for (int i = 0; i < n; ++i) {
-            const float send = up ? v[i] : v[i + n];
-            const float keep = up ? v[i + n] : v[i];
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, n);
-        }
-    }
-    return v[0];
-}
-
 // byte offset of element (row r, k) inside one hi/lo part of a stage (k multiple of 4)
 __device__ __forceinline__ uint32_t b_offset(int r, int k) {
     const int kb = k >> 6, col = k & 63;
@@ -265,30 +215,18 @@ struct Peers {
     float* mc;            // NVSwitch multicast address of the same buffer on ALL ranks (incl. this one), or nullptr:
                           // one multimem.st per element, replicated by the switch (egress 1x instead of (G-1)x)
 };
-__device__ __forceinline__ void multimem_st4(float* addr, const float4 v) {
-    asm volatile("multimem.st.relaxed.sys.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)
-                 : "memory");
+__device__ __forceinline__ void multimem_st2(float* addr, const float2 v) {
+    asm volatile("multimem.st.relaxed.sys.global.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(v.x), "f"(v.y) : "memory");
 }
-// 4x4 transpose across the 4 lanes of a quad: in: lane i holds a[0..3]; out: lane i holds (a[i] of lanes 0,1,2,3).
-__device__ __forceinline__ void quad_transpose(float& a0, float& a1, float& a2, float& a3, int lane) {
-    const bool b0 = lane & 1, b1 = lane & 2;
-    float t;
-    t = b0 ? a0 : a1; t = __shfl_xor_sync(0xffffffffu, t, 1); if (b0) a0 = t; else a1 = t;
-    t = b0 ? a2 : a3; t = __shfl_xor_sync(0xffffffffu, t, 1); if (b0) a2 = t; else a3 = t;
-    t = b1 ? a0 : a2; t = __shfl_xor_sync(0xffffffffu, t, 2); if (b1) a0 = t; else a2 = t;
-    t = b1 ? a1 : a3; t = __shfl_xor_sync(0xffffffffu, t, 2); if (b1) a1 = t; else a3 = t;
-}
-
 // ---------------------------------------------------------------- long rows (hub destinations)
 // A destination row with more than LONG_T in-edges would be gathered by ONE warp.  A deterministic pre-pass
 // cuts every such row into fixed chunks of LONG_CH edges; one CTA per chunk computes the unnormalised
 // weighted sum + weight sum (fixed order: 8 warps x 64 edges, then warp 0 adds the 8 warp partials in order)
 // into a side buffer.  The main kernel then sees the row as the items [self, partial_0 .. partial_{nc-1}]
 // (weight 1 each, weight-sum from pw[]).  The workspace is capacity driven: rows that do not fit stay inline.
-// Threshold: a 300-edge row gathered by one warp (512 B per edge at ~6 GB/s per warp) takes ~25 us while the other 31 rows
-// of its tile are done in 2 -- and a trace graph has exactly such a row every 64 nodes (the process node of each
-// component, in-degree = events of its files).  Measured on the trace-structured bench graph: 2.07 ms per F=128 layer with
-// the r1 threshold of 512, see profiles/r02_bench_n2.json vs r02 final.
+// Threshold: a row of a few hundred edges gathered by one warp takes many times as long as the other 31 rows of its tile,
+// and a trace graph has exactly such a row every 64 nodes (the process node of each component, in-degree = events of
+// its files).
 constexpr int LONG_T = 128;
 constexpr int LONG_CH = 256;
 
@@ -399,20 +337,19 @@ __global__ void __launch_bounds__(256) long_chunk_kernel(const float* __restrict
 
 // LONG: compiled with the hub-row (pre-aggregated partial items) paths; the plain variant is used when the
 // launch has no hub-row scratch, so graphs without hub rows pay nothing for the feature.
-// BULK: source rows travel as one bulk async copy each (cp.async.bulk, SASS UBLKCP) instead of 32 lanes x 16-byte
-// cp.async (LDGSTS).  Measured on B200 (profiles/r02_gather_transport.md): the TMA unit retires ~one bulk request per
-// 20-30 cycles per SM, so at one request per 128..512-byte row it -- not HBM, not issue slots -- becomes the limiter
-// (F=128 layer 1.24 ms vs 1.01 ms).  The LDGSTS transport is therefore the default; the edge-block slices (col / ew,
-// kilobytes per request) use bulk copies in both variants.
+// BULK: source rows travel as one bulk async copy each (cp.async.bulk) instead of 32 lanes x 16-byte cp.async
+// (LDGSTS).  At one bulk request per 128..512-byte row the copy engine's request rate, not HBM, becomes the limiter,
+// so the LDGSTS transport is the default; the edge-block slices (col / ew, kilobytes per request) use bulk copies in
+// both variants.
 template <int F, int NS, typename RP, bool LONG, bool BULK>
 __global__ void __launch_bounds__((UmmaCfg<F, NS>::THREADS), 1)
 sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowptr, const int32_t* __restrict__ col,
                        const float* __restrict__ ew, const float* __restrict__ W, const float* __restrict__ bias,
                        float* __restrict__ out, int64_t row_begin, int64_t row_end, int relu,
                        const float* __restrict__ node_w, float node_b, float* __restrict__ score, const LongWs lw,
-                       const Peers peers, unsigned* __restrict__ tile_ctr) {
+                       const Peers peers, unsigned* __restrict__ tile_ctr, const uint4* __restrict__ wsplit) {
     using C = UmmaCfg<F, NS>;
-    constexpr int K = C::K, LPR = F / 4;
+    constexpr int LPR = F / 4;
     constexpr int GATHER_WARPS = C::GATHER_WARPS, IDX_STAGES = C::IDX_STAGES;
     extern __shared__ unsigned char smem_dyn[];
     const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;          // SWIZZLE_128B needs 1024-B alignment
@@ -421,11 +358,9 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
     const uint32_t bar_base = idx_base + IDX_STAGES * IDX_STAGE_BYTES;     // 256 B of barriers, then the gather rings
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
-    auto accf_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + a); };
-    auto acce_bar = [&](int a) { return bar_base + 8u * (2 * C::STAGES + 2 + a); };
-    auto idxf_bar = [&](int q) { return bar_base + 8u * (2 * C::STAGES + 4 + q); };
-    auto idxe_bar = [&](int q) { return bar_base + 8u * (2 * C::STAGES + 4 + IDX_STAGES + q); };
-    const uint32_t tmem_slot = bar_base + 8u * (2 * C::STAGES + 4 + 2 * IDX_STAGES);
+    auto idxf_bar = [&](int q) { return bar_base + 8u * (2 * C::STAGES + q); };
+    auto idxe_bar = [&](int q) { return bar_base + 8u * (2 * C::STAGES + IDX_STAGES + q); };
+    static_assert(8 * (2 * C::STAGES + 2 * IDX_STAGES) <= 256, "barrier area");
     // per gather warp: NQ ring-slot barriers (bulk-copy byte counts), private to the warp
     auto ring_bar = [&](int g, int q) { return bar_base + 256u + 8u * (uint32_t)(g * NQ + q); };
     static_assert(256 + GATHER_WARPS * NQ * 8 <= 1024 - 64, "barrier area");
@@ -433,30 +368,29 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
     // the id of the CTA's tl-th tile in this ring (-1 = end of stream) before it releases the tile's edge block; every
     // role reads it after the mbarrier wait that orders it behind that release.  Rows are not equally expensive (hub
     // destinations: a 32-row tile can hold 50x the edges of an average one), a static round-robin left whole SMs idle.
-    constexpr int TILE_RING = 16;                  // > IDX_STAGES + STAGES + 2 accumulators: an entry outlives its tile
+    constexpr int TILE_RING = 16;                  // > IDX_STAGES + STAGES: an entry outlives its tile
     volatile int* tile_ids = reinterpret_cast<volatile int*>(smem_gen + (bar_base + 1024 - 64 - smem_base));
     // QUAD mode (F = 32): a gather warp works on FOUR rows at a time, one per 8-lane group (a 128-byte source row is 8 lanes
     // x 16 B), so the per-row overhead -- row setup, the cross-group combine, the bf16 split, the operand stores, the barrier
-    // arrivals -- is paid once per four rows and by all 32 lanes (r1/r2 ncu: the F=32 layer was issue-bound at ~500
-    // instructions per row, most of them this overhead).  Units of 4 rows are dealt round-robin to the warps; a warp need not
+    // arrivals -- is paid once per four rows and by all 32 lanes (one row per warp leaves the F=32 layer issue-bound on
+    // this overhead).  Units of 4 rows are dealt round-robin to the warps; a warp need not
     // own a unit in every tile, so the end of the tile stream is also published in `end_tl` (the closing tile's index).
     constexpr bool QUAD = (F == 32) && !BULK;
     volatile int* end_tl = reinterpret_cast<volatile int*>(smem_gen + (bar_base + 1024 - 64 - 8 - smem_base));
     static_assert(256 + GATHER_WARPS * NQ * 8 <= 1024 - 64 - 8, "barrier area");
     unsigned char* idx_gen = smem_gen + (idx_base - smem_base);
     const uint32_t ring_base = bar_base + 1024;
-    float* head_red = reinterpret_cast<float*>(smem_gen + (ring_base - smem_base) + (size_t)GATHER_WARPS * C::RING_BYTES);   // [2][4][32]
-    volatile uint32_t* tmem_slot_gen = reinterpret_cast<volatile uint32_t*>(smem_gen + (tmem_slot - smem_base));
+    float* head_red = reinterpret_cast<float*>(smem_gen + (ring_base - smem_base) + (size_t)GATHER_WARPS * C::RING_BYTES);   // [2][8][32]
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int64_t rows = row_end - row_begin;
     const int64_t n_tiles = (rows + TN - 1) / TN;
 
-    if (warp == MMA_WARP) {
+    if (warp == LOADER_WARP) {
         if (lane == 0) {
-            for (int s = 0; s < C::STAGES; ++s) { mbar_init(full_bar(s), QUAD ? TN / 4 : TN); mbar_init(empty_bar(s), 1); }
+            // operand stage full: one arrival per row (per 4-row unit in QUAD mode); empty: one per consumer warp
+            for (int s = 0; s < C::STAGES; ++s) { mbar_init(full_bar(s), QUAD ? TN / 4 : TN); mbar_init(empty_bar(s), EPI_WARPS); }
             *end_tl = 0x7fffffff;
-            for (int a = 0; a < 2; ++a) { mbar_init(accf_bar(a), 1); mbar_init(acce_bar(a), EPI_WARPS * 32); }
             // idx full: ONE arrive.expect_tx by the loader (publishes the rowptr words, counts the bytes of the two bulk
             // copies); empty: one per gather warp.  ring slots: one arrive.expect_tx by the issuing lane per use
             for (int q = 0; q < IDX_STAGES; ++q) { mbar_init(idxf_bar(q), 1); mbar_init(idxe_bar(q), QUAD ? TN / 4 : GATHER_WARPS); }
@@ -465,38 +399,8 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
             fence_barrier_init();
         }
         __syncwarp();
-        tmem_alloc(tmem_slot, C::TMEM_COLS);
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot_gen;
-
-    // ---- W^T -> TMEM (hi | lo), done once per CTA by the four epilogue warps: thread = feature
-    float my_bias = 0.f;
-    if (warp < EPI_WARPS) {
-        const int f = warp * 32 + lane;
-        my_bias = __ldg(bias + f);
-        const uint32_t lane_addr = tmem_base + ((uint32_t)(warp * 32) << 16);
-        for (int k0 = 0; k0 < K; k0 += 16) {
-            uint32_t parts[NS][8];
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const float a = __ldg(W + (size_t)(k0 + 2 * i) * UM + f);
-                const float b = __ldg(W + (size_t)(k0 + 2 * i + 1) * UM + f);
-                uint32_t pp[NS];
-                split_pair<NS>(a, b, pp);
-#pragma unroll
-                for (int p = 0; p < NS; ++p) parts[p][i] = pp[p];
-            }
-#pragma unroll
-            for (int p = 0; p < NS; ++p) tmem_st8(lane_addr + (uint32_t)(p * C::W_PART_COLS + (k0 >> 1)), parts[p]);
-        }
-        tmem_wait_st();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
 
     if (warp >= GATHER_WARP0) {
       if constexpr (QUAD) {
@@ -947,7 +851,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
             cslot = (cslot + 1) % NQ;
             if (++cb < cnb) continue;
 
-            // ---- row complete: normalise, split to bf16 terms, write the UMMA B operand, signal
+            // ---- row complete: normalise, split to bf16 terms, write the wgmma B operand, signal
             const int tl = ctl;
             const int r = ci % TN;
             const int s = tl % C::STAGES;
@@ -980,7 +884,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
 #pragma unroll
                     for (int p = 0; p < NS; ++p) *reinterpret_cast<uint2*>(st + p * C::PART_BYTES + off) = parts[p];
                 }
-                fence_proxy_async();                                     // generic-proxy writes -> async proxy (UMMA)
+                fence_proxy_async();                                     // generic-proxy writes -> async proxy (wgmma)
                 acc = make_float4(0.f, 0.f, 0.f, 0.f); self = acc; wsum = 0.f;
             }
             __syncwarp();
@@ -1007,8 +911,8 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
         };
         // Software pipeline, two tiles deep and free of register copies (the loop body is instantiated twice with the roles of
         // the two rowptr register sets swapped): the atomic that claims tile t+2 and the rowptr loads of tile t+1 are issued
-        // in iteration t and first needed one iteration later, so neither latency (~1 us each) sits on the per-tile path --
-        // at F=32 a tile period is < 2 us and the r1/r2 loader (claim -> dependent loads -> use, serial) was as slow as that.
+        // in iteration t and first needed one iteration later, so neither latency sits on the per-tile path -- at F=32 a
+        // tile period is short enough that a serial loader (claim -> dependent loads -> use) would set the pace.
         unsigned craw = 0;                                               // lane 0: raw result of the claim in flight
         auto claim_issue = [&]() { if (lane == 0) craw = atomicAdd(tile_ctr, 1u); };
         auto claim_take = [&]() -> int64_t { return (int64_t)__shfl_sync(0xffffffffu, craw, 0); };
@@ -1071,125 +975,145 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
             if (body(tl, tile_a, rp_a, tile_b, rp_b)) break;
             if (body(tl + 1, tile_b, rp_b, tile_a, rp_a)) break;
         }
-    } else if (warp == MMA_WARP) {
-        // =========================================================== MMA issuer (one thread)
-        if (lane == 0) {
-            constexpr uint32_t idesc = make_idesc();
-            for (int64_t tl = 0;; ++tl) {
-                const int s = (int)(tl % C::STAGES);
-                const uint32_t n = (uint32_t)(tl / C::STAGES);
-                const int a = (int)(tl & 1);
-                const uint32_t m = (uint32_t)(tl >> 1);
-                mbar_wait_relaxed(acce_bar(a), (m & 1u) ^ 1u);           // epilogue drained this accumulator
-                mbar_wait_relaxed(full_bar(s), n & 1u);                  // gather filled this stage
-                tc_fence_after();
-                if (tile_ids[tl % TILE_RING] < 0) {                      // closing entry: hand the end of stream to the epilogue
-                    umma_commit(accf_bar(a));
-                    break;
-                }
-                const uint32_t d_tmem = tmem_base + (uint32_t)(C::ACC_COL0 + a * TN);
-                const uint32_t st0 = smem_base + (uint32_t)(s * C::STAGE_BYTES);
-#pragma unroll 2
-                for (int j = 0; j < C::KSTEPS; ++j) {
-                    const uint32_t boff = (uint32_t)((j >> 2) * (TN * 128) + (j & 3) * 32);
-                    uint64_t xb[NS];
-                    uint32_t wa[NS];
+    } else if (warp < EPI_WARPS) {
+        // =========================================================== consumer warpgroups: wgmma + epilogue
+        // Warpgroup h computes output features [64 h, 64 h + 64).  Its accumulator row m = 16 wq + i (warp wq of the
+        // warpgroup, i < 16) is feature 64 h + 16 wq + 2 (i & 7) + (i >> 3): a thread's two rows are two CONSECUTIVE
+        // features f0, f0 + 1, so its outputs are 8-byte stores and a warp writes 64 contiguous bytes of a row.  The
+        // accumulator register d[4 nb + 2 b + e] of thread (wq, lane = 4 g + c) holds feature f0 + b of tile row
+        // 8 nb + 2 c + e.  The A fragments (W^T terms) come pre-split from `wsplit` (split_w_kernel), 16 bytes per
+        // thread, term and K step, from L2.  They are the same for every tile, so their loads run two K steps ahead of
+        // the MMAs across tile boundaries: an L2 round trip under the gather's load is longer than one K step.
+        const int h = warp >> 2, wq = warp & 3, et = tid & 127;
+        const int g = lane >> 2, c = lane & 3;
+        const int f0 = 64 * h + 16 * wq + 2 * g;
+        const float2 b2 = *reinterpret_cast<const float2*>(bias + f0);
+        const float2 nw2 = node_w ? *reinterpret_cast<const float2*>(node_w + f0) : make_float2(0.f, 0.f);
+        const uint4* wfr = reinterpret_cast<const uint4*>(wsplit) + (size_t)h * NS * 128 + et;   // + (2 j NS + p) * 128
+        auto load_a = [&](int j, uint32_t (&a)[NS][4]) {
 #pragma unroll
-                    for (int p = 0; p < NS; ++p) {
-                        xb[p] = make_b_desc(st0 + (uint32_t)(p * C::PART_BYTES) + boff);     // x term p (smem)
-                        wa[p] = tmem_base + (uint32_t)(p * C::W_PART_COLS + j * 8);          // W^T term p (TMEM)
-                    }
-                    umma_ts(d_tmem, wa[0], xb[0], idesc, j > 0 ? 1u : 0u);
-                    umma_ts(d_tmem, wa[0], xb[1], idesc, 1u);
-                    umma_ts(d_tmem, wa[1], xb[0], idesc, 1u);
-                    if constexpr (NS == 3) {
-                        umma_ts(d_tmem, wa[1], xb[1], idesc, 1u);
-                        umma_ts(d_tmem, wa[0], xb[2], idesc, 1u);
-                        umma_ts(d_tmem, wa[2], xb[0], idesc, 1u);
-                    }
-                }
-                umma_commit(empty_bar(s));                               // smem stage reusable once the MMAs retire
-                umma_commit(accf_bar(a));                                // accumulator ready for the epilogue
+            for (int p = 0; p < NS; ++p) {
+                const uint4 v = __ldg(wfr + (size_t)(2 * j * NS + p) * 128);
+                a[p][0] = v.x; a[p][1] = v.y; a[p][2] = v.z; a[p][3] = v.w;
             }
-        }
-    } else {
-        // =========================================================== epilogue warps
-        const int f = warp * 32 + lane;
-        const float my_nw = node_w ? __ldg(node_w + f) : 0.f;
+        };
+        auto copy_a = [](uint32_t (&dst)[NS][4], const uint32_t (&src)[NS][4]) {
+#pragma unroll
+            for (int p = 0; p < NS; ++p)
+#pragma unroll
+                for (int r = 0; r < 4; ++r) dst[p][r] = src[p][r];
+        };
+        uint32_t a_n1[NS][4], a_n2[NS][4];                                    // fragments of the next two K steps
+        load_a(0, a_n1);
+        load_a(1, a_n2);
         for (int64_t tl = 0;; ++tl) {
-            const int a = (int)(tl & 1);
-            const uint32_t m = (uint32_t)(tl >> 1);
-            mbar_wait_relaxed(accf_bar(a), m & 1u);
-            tc_fence_after();
+            const int s = (int)(tl % C::STAGES);
+            mbar_wait_relaxed(full_bar(s), (uint32_t)(tl / C::STAGES) & 1u);   // gather filled this stage
             const int64_t tile = tile_ids[tl % TILE_RING];
-            if (tile < 0) break;
-            const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(C::ACC_COL0 + a * TN);
-            const int64_t row0 = row_begin + tile * TN;
-            uint32_t v[32];
-            tmem_ld32(taddr, v);
-            tmem_wait_ld();
-            tc_fence_before();
-            mbar_arrive(acce_bar(a));                                    // accumulator drained: the MMA may reuse it
-            float hv[32], ov[32];
+            if (tile < 0) break;                                              // closing entry: end of stream
+            const uint32_t st0 = smem_base + (uint32_t)(s * C::STAGE_BYTES);
+            float d[16];
+            auto mma_step = [&](int j, const uint32_t (&a)[NS][4]) {
+                const uint32_t boff = (uint32_t)((j >> 2) * (TN * 128) + (j & 3) * 32);
+                uint64_t xb[NS];
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-                float o = __uint_as_float(v[j]) + my_bias;
-                if (relu) o = fmaxf(o, 0.f);
-                ov[j] = o;
-                hv[j] = o * my_nw;
+                for (int p = 0; p < NS; ++p) xb[p] = make_b_desc(st0 + (uint32_t)(p * C::PART_BYTES) + boff);   // x term p
+                wgmma_fence();
+                wgmma_rs(d, a[0], xb[0], j > 0 ? 1u : 0u);
+                wgmma_rs(d, a[0], xb[1], 1u);
+                wgmma_rs(d, a[1], xb[0], 1u);
+                if constexpr (NS == 3) {
+                    wgmma_rs(d, a[1], xb[1], 1u);
+                    wgmma_rs(d, a[0], xb[2], 1u);
+                    wgmma_rs(d, a[2], xb[0], 1u);
+                }
+                wgmma_commit();
+            };
+            // (registers a running wgmma reads must not be written before it retires, and ptxas serializes the MMAs of a
+            // step when any wgmma input is written while one is in flight: the next fragments are loaded before the step)
+#pragma unroll 1
+            for (int j = 0; j < C::KSTEPS; ++j) {
+                uint32_t a_cur[NS][4];
+                copy_a(a_cur, a_n1);
+                copy_a(a_n1, a_n2);
+                load_a(j + 2 < C::KSTEPS ? j + 2 : j + 2 - C::KSTEPS, a_n2);  // K >= 64: at least four K steps
+                mma_step(j, a_cur);
+                wgmma_wait_all();
             }
-            if (peers.n == 0 && !peers.mc) {
-                // single GPU: thread = feature, 32 row stores of 128 B per warp (no extra shuffles: the epilogue
-                // shares issue slots with the gather warps)
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty_bar(s));                         // this warp's MMAs no longer read the stage
+
+            // ---- epilogue: + bias, ReLU, one 8-byte store per (row, thread)
+            const int64_t row0 = row_begin + tile * TN;
+            float part[8];
 #pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    if (row0 + j < row_end) out[(row0 + j) * UM + f] = ov[j];
-            } else {
-                // fused exchange: transpose 4x4 inside each lane quad so that a lane owns 4 consecutive features of
-                // one row (16-byte stores; a warp instruction writes four full 128-byte row segments) -- locally and
-                // to every peer's buffer over NVLink, or once through the NVSwitch multicast address.
-                const int qi = lane & 3;                                  // row within the block of 4
-                const int fq = warp * 32 + (lane & ~3);                   // first of this lane's 4 features
+            for (int nb = 0; nb < 4; ++nb) {
 #pragma unroll
-                for (int r = 0; r < 8; ++r) {
-                    float a0 = ov[4 * r], a1 = ov[4 * r + 1], a2 = ov[4 * r + 2], a3 = ov[4 * r + 3];
-                    quad_transpose(a0, a1, a2, a3, lane);
-                    const int64_t row = row0 + 4 * r + qi;
+                for (int e = 0; e < 2; ++e) {
+                    float2 o = make_float2(d[4 * nb + e] + b2.x, d[4 * nb + 2 + e] + b2.y);
+                    if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+                    part[2 * nb + e] = o.x * nw2.x + o.y * nw2.y;
+                    const int64_t row = row0 + 8 * nb + 2 * c + e;
                     if (row < row_end) {
-                        const int64_t off = row * UM + fq;
-                        const float4 val = make_float4(a0, a1, a2, a3);
-                        if (peers.mc) {
-                            multimem_st4(peers.mc + off, val);
+                        const int64_t off = row * UM + f0;
+                        if (peers.mc) {                                       // NVSwitch multicast: every rank's buffer at once
+                            multimem_st2(peers.mc + off, o);
                         } else {
-                            *reinterpret_cast<float4*>(out + off) = val;
-                            const unsigned need = peers.need ? (unsigned)__ldg(peers.need + row) : 0xFFu;
+                            *reinterpret_cast<float2*>(out + off) = o;
+                            if (peers.n) {                                    // fused exchange over NVLink
+                                const unsigned need = peers.need ? (unsigned)__ldg(peers.need + row) : 0xFFu;
 #pragma unroll
-                            for (int pr = 0; pr < MAX_PEERS; ++pr)
-                                if (pr < peers.n && ((need >> pr) & 1u)) *reinterpret_cast<float4*>(peers.out[pr] + off) = val;
+                                for (int pr = 0; pr < MAX_PEERS; ++pr)
+                                    if (pr < peers.n && ((need >> pr) & 1u)) *reinterpret_cast<float2*>(peers.out[pr] + off) = o;
+                            }
                         }
                     }
                 }
             }
             if (node_w) {
-                // fused node head: score[row] = sigmoid(h[row,:] . node_w + node_b)
-                const float part = warp_transpose_reduce32(hv, lane);    // lane l: this warp's 32 features of row l
-                head_red[(a * EPI_WARPS + warp) * 32 + lane] = part;
-                asm volatile("bar.sync 1, 128;" ::: "memory");          // the four epilogue warps
+                // fused node head: score[row] = sigmoid(h[row,:] . node_w + node_b); a warp's 16 features summed over g
+#pragma unroll
+                for (int i = 0; i < 8; ++i) {
+                    part[i] += __shfl_xor_sync(0xffffffffu, part[i], 4);
+                    part[i] += __shfl_xor_sync(0xffffffffu, part[i], 8);
+                    part[i] += __shfl_xor_sync(0xffffffffu, part[i], 16);
+                }
+                float* hb = head_red + ((int)(tl & 1) * EPI_WARPS + warp) * 32;
+                if (g == 0) {
+#pragma unroll
+                    for (int nb = 0; nb < 4; ++nb) { hb[8 * nb + 2 * c] = part[2 * nb]; hb[8 * nb + 2 * c + 1] = part[2 * nb + 1]; }
+                }
+                asm volatile("bar.sync 1, 256;" ::: "memory");          // the eight consumer warps
                 if (warp == 0) {
-                    const float* hr = head_red + a * EPI_WARPS * 32 + lane;
-                    const float dot = (hr[0] + hr[32]) + (hr[64] + hr[96]);
+                    const float* hr = head_red + (int)(tl & 1) * EPI_WARPS * 32 + lane;
+                    const float dot = ((hr[0] + hr[32]) + (hr[64] + hr[96])) + ((hr[128] + hr[160]) + (hr[192] + hr[224]));
                     if (row0 + lane < row_end) score[row0 + lane] = 1.f / (1.f + expf(-(dot + node_b)));
                 }
             }
         }
     }
+}
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == MMA_WARP) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, C::TMEM_COLS);
+// W [K][128] fp32 -> the consumer warpgroups' A fragments, split into NS bf16 terms:
+// wsplit[((2 j + h) NS + p) 128 + t] = uint4 of term p of thread t of warpgroup h at K step j (see the consumer role)
+template <int NS>
+__global__ void __launch_bounds__(256) split_w_kernel(const float* __restrict__ W, int ksteps, uint4* __restrict__ wsplit) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;               // (j, h, t)
+    if (i >= ksteps * 2 * 128) return;
+    const int t = i & 127, h = (i >> 7) & 1, j = i >> 8;
+    const int wq = t >> 5, g = (t & 31) >> 2, c = t & 3;
+    const int f0 = 64 * h + 16 * wq + 2 * g;
+    uint32_t a[NS][4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {                                     // register r: row g + 8 (r & 1), K pair r >> 1
+        const int k = 16 * j + 2 * c + 8 * (r >> 1), f = f0 + (r & 1);
+        uint32_t pp[NS];
+        split_pair<NS>(W[(size_t)k * UM + f], W[(size_t)(k + 1) * UM + f], pp);
+#pragma unroll
+        for (int p = 0; p < NS; ++p) a[p][r] = pp[p];
     }
+#pragma unroll
+    for (int p = 0; p < NS; ++p) wsplit[(size_t)((2 * j + h) * NS + p) * 128 + t] = make_uint4(a[p][0], a[p][1], a[p][2], a[p][3]);
 }
 
 // the per-row bulk-copy transport is an experiment knob (NERRF_SAGE_ROW_COPY=bulk), compiled for the headline shapes only
@@ -1212,6 +1136,21 @@ inline unsigned* tile_counter_slot(cudaStream_t st) {
     unsigned* slot = ring[dev_] + (__atomic_fetch_add(&next[dev_], 1u, __ATOMIC_RELAXED) & 255u);
     if (cudaMemsetAsync(slot, 0, sizeof(unsigned), st) != cudaSuccess) return nullptr;
     return slot;
+}
+
+// Scratch for the split W^T of one launch (192 KB at F=128, three terms), one buffer per (device, stream), allocated on
+// the stream's first launch and kept: launches on one stream run in order, so each one re-splits its weights into the
+// buffer the previous one has finished with, and the layer launches themselves allocate nothing.
+constexpr size_t WSPLIT_MAX_BYTES = (size_t)(2 * 128 / 16) * 2 * 3 * 128 * sizeof(uint4);
+inline uint4* wsplit_buffer(cudaStream_t st) {
+    static std::mutex mu;
+    static std::map<std::pair<int, cudaStream_t>, uint4*> bufs;
+    int dev_ = 0;
+    if (cudaGetDevice(&dev_) != cudaSuccess) return nullptr;
+    std::lock_guard<std::mutex> lock(mu);
+    uint4*& buf = bufs[std::make_pair(dev_, st)];
+    if (!buf && cudaMalloc((void**)&buf, WSPLIT_MAX_BYTES) != cudaSuccess) buf = nullptr;
+    return buf;
 }
 
 template <int F, int NS, typename RP>
@@ -1250,15 +1189,20 @@ int launch_umma(const float* x, const RP* rowptr, const int32_t* col, const floa
     const int64_t grid = tiles < sm_count() ? tiles : sm_count();
     unsigned* tile_ctr = tile_counter_slot(st);
     if (!tile_ctr) { set_error("could not allocate the tile counter"); return NERRF_ERR_CUDA; }
+    // W^T split into bf16 terms in fragment order, once per launch (the weights may have changed in place since the last one)
+    static_assert((size_t)C::KSTEPS * 2 * NS * 128 * sizeof(uint4) <= WSPLIT_MAX_BYTES, "split W scratch");
+    uint4* wsplit = wsplit_buffer(st);
+    if (!wsplit) { set_error("could not allocate the split-weight scratch"); return NERRF_ERR_CUDA; }
+    split_w_kernel<NS><<<(C::KSTEPS * 2 * 128 + 255) / 256, 256, 0, st>>>(W, C::KSTEPS, wsplit);
     // the per-row bulk-copy transport needs 16-byte aligned rows; every transport stages col / ew with bulk copies,
     // which only need 4-byte aligned slices (the aligned superset is copied)
     if (lw.cap > 0)
-        sage_layer_umma_kernel<F, NS, RP, true, false><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr);
+        sage_layer_umma_kernel<F, NS, RP, true, false><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit);
     else if (kBulkVariant<F, NS, RP> && bulk_rows_requested() && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
         if constexpr (kBulkVariant<F, NS, RP>)
-            sage_layer_umma_kernel<F, NS, RP, false, true><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr);
+            sage_layer_umma_kernel<F, NS, RP, false, true><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit);
     } else
-        sage_layer_umma_kernel<F, NS, RP, false, false><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr);
+        sage_layer_umma_kernel<F, NS, RP, false, false><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit);
     return launch_status("sage_layer_umma_kernel");
 }
 
@@ -1297,7 +1241,7 @@ int sage_layer_umma(const float* x, const void* rowptr, int is64, const int32_t*
         }
     }
 #undef GO
-    set_error("UMMA layer: unsupported feature width F=%d / split %d (supported: F in 32, 64, 128; split 2 or 3)", F, nsplit);
+    set_error("tensor-core layer: unsupported feature width F=%d / split %d (supported: F in 32, 64, 128; split 2 or 3)", F, nsplit);
     return NERRF_ERR_INVALID;
 }
 

@@ -7,12 +7,13 @@ Two uses, both on the checker side of the fence:
 Never imported by the product (nerrf_b200/).
 
 Built on demand with gcc -O3 -march=native into oracle/_build/.  The file name carries a hash of this host's CPU
-flags, so a library built in the authoring container is not reused on a GPU box with a different CPU (it is
-rebuilt there in about a second; gcc is part of the image)."""
+flags, so a library built on one host is not reused on a host with a different CPU (it is rebuilt there in about a
+second, into a temporary directory when the tree is read-only)."""
 import ctypes as C
 import hashlib
 import os
 import subprocess
+import tempfile
 
 import numpy as np
 
@@ -38,9 +39,16 @@ def lib_path():
 
 
 def build(force=False):
-    os.makedirs(OUT_DIR, exist_ok=True)
     out = lib_path()
     if force or not os.path.exists(out) or os.path.getmtime(out) < os.path.getmtime(SRC):
+        try:
+            os.makedirs(OUT_DIR, exist_ok=True)
+            writable = os.access(OUT_DIR, os.W_OK)
+        except OSError:
+            writable = False
+        if not writable:                                        # a read-only tree built on another host: build aside
+            out = os.path.join(tempfile.gettempdir(), f"nerrf_oracle_{os.getuid()}", os.path.basename(out))
+            os.makedirs(os.path.dirname(out), exist_ok=True)
         base = ["gcc", "-O3", "-fopenmp", "-fno-fast-math", "-shared", "-fPIC", SRC, "-lm"]
         tmp = out + f".{os.getpid()}.tmp"
         r = subprocess.run(base + ["-march=native", "-o", tmp], capture_output=True, text=True)

@@ -11,7 +11,7 @@ from oracle import lstm_ref  # noqa: E402
 
 
 def run(model, seq, ln, algo):
-    os.environ["NERRF_LSTM_ALGO"] = algo          # "ffma" = the fp32 CUDA-core cross-check kernel; anything else = tcgen05
+    os.environ["NERRF_LSTM_ALGO"] = algo          # "ffma" = the fp32 CUDA-core cross-check kernel; anything else = wgmma
     out = model(seq, ln)
     torch.cuda.synchronize()
     return out

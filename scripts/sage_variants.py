@@ -1,5 +1,5 @@
 """Per-layer timing of the fused GraphSAGE-T layer on the three cfg-2-size graph families + a quick cross-check of the
-tcgen05 path against the fp32 CUDA-core path.  usage: sage_variants.py [reps]"""
+tensor-core path against the fp32 CUDA-core path.  usage: sage_variants.py [reps]"""
 import sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

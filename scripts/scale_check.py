@@ -1,4 +1,4 @@
-"""Config-4 size on ONE GPU (10M nodes / 100M edges): size-independent properties of the tcgen05 layer.
+"""Config-4 size on ONE GPU (10M nodes / 100M edges): size-independent properties of the tensor-core layer.
   (1) W = [0; I], b = 0, x = const  ->  out == const on every non-isolated row, 0 on isolated rows
   (2) random x: 64 sampled rows of out = relu(mean) against an fp64 host evaluation
   (3) full 3-layer forward: finite, deterministic; timing"""

@@ -1,4 +1,4 @@
-"""Diagnose the tcgen05 fused layer against closed-form inputs (run on the GPU box)."""
+"""Diagnose the tensor-core fused layer against closed-form inputs (run on the GPU box)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

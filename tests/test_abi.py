@@ -46,6 +46,11 @@ def test_invalid_arguments_return_error_not_crash(lib_built):
     assert h.nerrf_mcts_workspace_bytes(10, 4, 48, ctypes.byref(n)) == -1      # R not a power of two
     assert h.nerrf_mcts_workspace_bytes(10, 4, 64, ctypes.byref(n)) == 0 and n.value > 0
     assert h.nerrf_lstm_workspace_bytes(4, 100, 128, ctypes.byref(n)) == -1     # H != 256
+    # the layer reads node_w 8 bytes at a time: a misaligned head vector is refused before anything is touched
+    p = lambda a: ctypes.c_void_p(a)
+    args = [p(1 << 20), p(2 << 20), 0, p(3 << 20), p(4 << 20), p(5 << 20), p(6 << 20), p(7 << 20), 10, 0, 10, 32, 128, 1, 0]
+    assert h.nerrf_sage_layer_head_fwd(*args, p((8 << 20) + 4), 0.0, p(9 << 20), None) == -1
+    assert b"node_w" in h.nerrf_last_error()
 
 
 def test_product_never_imports_oracle():

@@ -1,6 +1,7 @@
 """Golden fixtures (tests/golden/, made by make_golden.py): the oracle must keep reproducing them, and the
 graph derived from the reference's own LockBit traces must label exactly the files the reference lists as
-encrypted (benchmarks/m{0,1}/results/file_list.txt)."""
+encrypted (its benchmarks/m{0,1}/results/file_list.txt, stored as tests/golden/m{0,1}_file_list.txt next to the
+traces m{0,1}_trace.jsonl)."""
 import os
 
 import numpy as np
@@ -51,9 +52,8 @@ def test_reference_trace_graph_labels_match_file_list():
         assert int((tr[f"{name}_kind"] == 1).sum()) == 1     # one ransomware process node
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/benchmarks"), reason="reference checkout not present")
 def test_golden_graph_is_current_with_reference():
     from nerrf_b200 import graph as G
     tr = np.load(os.path.join(GOLD, "golden_m1_graph.npz"))
-    g = G.graph_from_jsonl("/root/reference/benchmarks/m1/results/m1_trace.jsonl")
+    g = G.graph_from_jsonl(os.path.join(GOLD, "m1_trace.jsonl"))
     assert np.array_equal(g.rowptr, tr["m1_rowptr"]) and np.array_equal(g.col, tr["m1_col"]) and np.allclose(g.x, tr["m1_x"])

@@ -1,4 +1,4 @@
-"""CUDA path against the committed golden fixtures, through the reference-named Python surface (needs a B200)."""
+"""CUDA path against the committed golden fixtures, through the reference-named Python surface (needs an H100)."""
 import os
 
 import numpy as np

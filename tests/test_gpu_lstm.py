@@ -1,4 +1,4 @@
-"""lstm.forward CUDA path vs the oracle (needs a B200).  The tcgen05 path (csrc/lstm_umma.cu) is the default; the fp32
+"""lstm.forward CUDA path vs the oracle (needs an H100).  The wgmma path (csrc/lstm_umma.cu) is the default; the fp32
 CUDA-core kernel (csrc/lstm.cu, NERRF_LSTM_ALGO=ffma) stays as an independent cross-check of it."""
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""Multi-GPU checks (need >= 2 B200s on the box; skipped on a single-GPU box): the sharded forward with every
+"""Multi-GPU checks (need >= 2 H100s on the box; skipped on a single-GPU box): the sharded forward with every
 exchange mode -- NCCL collectives and the fused P2P / multicast epilogue -- is bit-identical to the single-GPU forward."""
 import os
 import subprocess

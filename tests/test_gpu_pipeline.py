@@ -1,4 +1,4 @@
-"""End-to-end pipeline (trace -> graph -> GNN -> LSTM -> MCTS plan) on a simulator-schema LockBit trace (needs a B200)."""
+"""End-to-end pipeline (trace -> graph -> GNN -> LSTM -> MCTS plan) on a simulator-schema LockBit trace (needs an H100)."""
 import numpy as np
 import pytest
 import torch

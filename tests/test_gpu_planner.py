@@ -1,4 +1,4 @@
-"""rewards.score and mcts.search CUDA path vs the oracle: BIT-EXACT (needs a B200)."""
+"""rewards.score and mcts.search CUDA path vs the oracle: BIT-EXACT (needs an H100)."""
 import numpy as np
 import pytest
 

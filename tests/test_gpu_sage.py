@@ -1,4 +1,4 @@
-"""GraphSAGE-T CUDA path vs the oracle, through the C-ABI (needs a B200)."""
+"""GraphSAGE-T CUDA path vs the oracle, through the C-ABI (needs an H100)."""
 import numpy as np
 import pytest
 import torch

@@ -1,4 +1,4 @@
-"""BASELINE config 5 in miniature (needs a B200): a fleet trace streamed tick by tick through the sliding window, the
+"""BASELINE config 5 in miniature (needs an H100): a fleet trace streamed tick by tick through the sliding window, the
 GPU graph constructor, GraphSAGE_T, the LSTM on the top-A candidates and the MCTS planner with process-kill candidates
 (planner spec v1) -- the running undo plan must end up reverting the encrypted files and killing their writers."""
 import numpy as np

@@ -1,5 +1,5 @@
 """Weights trained by ai.train (autograd, CPU) drive the CUDA inference path: same scores, same AUC, and the
-pipeline plans from MODEL confidence alone (needs a B200)."""
+pipeline plans from MODEL confidence alone (needs an H100)."""
 import numpy as np
 import pytest
 import torch
@@ -49,7 +49,7 @@ def _grad_close(got, want, what, rtol=2e-4, atol_rms=2e-5):
 @pytest.mark.parametrize("N,E,L,F,seed", [(3000, 30000, 3, 32, 1), (257, 1500, 2, 64, 2), (1000, 20000, 2, 128, 3),
                                           (33, 20, 1, 32, 4), (5000, 400000, 2, 32, 5)])
 def test_backward_kernels_match_the_oracle(N, E, L, F, seed):
-    """d(loss)/d(every parameter) and d(loss)/dx from the CUDA path (fused tcgen05 forward + sage_bwd.cu backward) against
+    """d(loss)/d(every parameter) and d(loss)/dx from the CUDA path (fused wgmma forward + sage_bwd.cu backward) against
     the hand-written fp64 backward oracle (itself pinned to autograd, tests/test_oracle_sage_bwd.py)."""
     from nerrf_b200 import graph as G
     from nerrf_b200.ai import autograd as AG

@@ -1,4 +1,4 @@
-"""`python -m nerrf_b200.undo`: EventBatch wire file in, undo plan out (needs a B200)."""
+"""`python -m nerrf_b200.undo`: EventBatch wire file in, undo plan out (needs an H100)."""
 import json
 
 import pytest
