@@ -1,4 +1,7 @@
 // ABI version, error string, device info.
+#include <map>
+#include <mutex>
+#include <utility>
 #include "common.cuh"
 
 namespace nerrf {
@@ -23,6 +26,19 @@ int sm_count() {
         else return 132;
     }
     return c;
+}
+
+int set_max_dynamic_smem(const void* kernel, size_t bytes) {
+    static std::mutex mu;
+    static std::map<std::pair<int, const void*>, size_t> set;      // function attributes are per device
+    int dev = 0;
+    NERRF_CHECK_CUDA(cudaGetDevice(&dev));
+    std::lock_guard<std::mutex> lock(mu);
+    size_t& cur = set[std::make_pair(dev, kernel)];
+    if (cur >= bytes) return NERRF_OK;
+    NERRF_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    cur = bytes;
+    return NERRF_OK;
 }
 
 }  // namespace nerrf

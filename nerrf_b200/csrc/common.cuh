@@ -39,6 +39,10 @@ inline int launch_status(const char* what) {
 
 int sm_count();   // cached per process (current device at first call)
 
+// Raise `kernel`'s dynamic shared-memory limit on the current device to at least `bytes`.  The attribute is set once per
+// (device, kernel) and again only when a larger size is asked for.  Returns NERRF_OK or NERRF_ERR_CUDA.
+int set_max_dynamic_smem(const void* kernel, size_t bytes);
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -7,7 +7,6 @@
 // registers, h lives in shared memory).  Weights are pre-transposed ([K, 4H]) so the 256
 // threads read 1 KB contiguous per (k, gate); they stream from L2 every step (8.2 MB of
 // weights is L2-resident, too big for one SM's shared memory).
-#include <stdlib.h>
 #include "common.cuh"
 
 namespace nerrf {
@@ -151,7 +150,8 @@ static int launch_lstm_layer(const float* in, int sb, int stt, int D, const int3
                              const float* Whh_b, const float* bias_b, float* out, float* hfin, cudaStream_t st) {
     const size_t smem = (size_t)(2 * LH * BS + (size_t)D * BS) * sizeof(float);
     NERRF_REQUIRE(smem <= 200 * 1024, "LSTM input width %d too large for shared memory", D);
-    NERRF_CHECK_CUDA(cudaFuncSetAttribute(lstm_layer_kernel<BS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const int rc = set_max_dynamic_smem((const void*)lstm_layer_kernel<BS>, smem);
+    if (rc) return rc;
     dim3 grid((unsigned)((B + BS - 1) / BS), 2);
     lstm_layer_kernel<BS><<<grid, LH, smem, st>>>(in, sb, stt, D, len, B, T, Wih_f, Whh_f, bias_f, Wih_b, Whh_b, bias_b, out, hfin);
     return launch_status("lstm_layer_kernel");
@@ -200,17 +200,10 @@ extern "C" int nerrf_lstm_forward(const float* seq, const int32_t* len, int64_t 
     float* hfin = buf1 + (size_t)B * T * 2 * H;
     const float* in = seq;
     int sb = T * D_in, stt = D_in, D = D_in;
-    // NERRF_LSTM_BS=8|16 overrides the batch-tile heuristic (tuning aid)
-    const char* bs_env = getenv("NERRF_LSTM_BS");
-    const bool big = bs_env ? atoi(bs_env) == 16 : false;   // BS=8 (2 CTAs/SM) by default
     for (int l = 0; l < num_layers; ++l) {
         float* o = (l == num_layers - 1) ? nullptr : ((l & 1) ? buf1 : buf0);
-        if (big)
-            rc = launch_lstm_layer<16>(in, sb, stt, D, len, B, T, Wih_t[2 * l], Whh_t[2 * l], bias[2 * l], Wih_t[2 * l + 1],
-                                       Whh_t[2 * l + 1], bias[2 * l + 1], o, hfin, st);
-        else
-            rc = launch_lstm_layer<8>(in, sb, stt, D, len, B, T, Wih_t[2 * l], Whh_t[2 * l], bias[2 * l], Wih_t[2 * l + 1],
-                                      Whh_t[2 * l + 1], bias[2 * l + 1], o, hfin, st);
+        rc = launch_lstm_layer<8>(in, sb, stt, D, len, B, T, Wih_t[2 * l], Whh_t[2 * l], bias[2 * l], Wih_t[2 * l + 1],
+                                  Whh_t[2 * l + 1], bias[2 * l + 1], o, hfin, st);
         if (rc) return rc;
         in = o; sb = T * 2 * H; stt = 2 * H; D = 2 * H;
     }

@@ -28,6 +28,7 @@
 #include <cuda_bf16.h>
 #include <stdlib.h>
 #include "common.cuh"
+#include "ptx.cuh"
 
 namespace nerrf {
 
@@ -43,89 +44,6 @@ constexpr int KSTEPS_H = LH / 16;
 constexpr int PLANE_BYTES_H = KB_H * NSEQ * 128;     // 32 KB: one bf16 plane of a [64 rows, 256] tile
 constexpr int TILE_BYTES_H = NS * PLANE_BYTES_H;     // 96 KB
 
-// ---------------------------------------------------------------- PTX wrappers (same forms as sage_umma.cu)
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try(uint32_t bar, uint32_t parity) {
-    uint32_t done;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    return done != 0;
-}
-// every wait in this file is bounded: a protocol bug must end in a trap (launch error), never in a hung GPU
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    for (uint32_t spin = 0; !mbar_try(bar, parity); ++spin) {
-        if (spin > (1u << 16)) __nanosleep(64);
-        if (spin > (1u << 26)) __trap();
-    }
-}
-// global -> shared bulk async copy (async proxy, SASS UBLKCP); completes `bytes` transactions on the mbarrier
-__device__ __forceinline__ void bulk_g2s(uint32_t dst_smem, const void* src, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(dst_smem), "l"(src), "r"(bytes), "r"(bar)
-                 : "memory");
-}
-__device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void named_bar(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
-// wgmma shared-memory matrix descriptor (sm_90): K-major, SWIZZLE_128B, 8-row groups 1024 B apart (SBO)
-__device__ __forceinline__ uint64_t make_b_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 62;
-    return d;
-}
-__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// D[64 x 64] (+)= A[64 x 16] (bf16 register fragment) . B[16 x 64] (bf16, K-major shared memory), fp32 accumulate
-__device__ __forceinline__ void wgmma_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %37, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-        "{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
-          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
-          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void split_pair(float a, float b, uint32_t (&parts)[NS]) {
-#pragma unroll
-    for (int p = 0; p < NS; ++p) {
-        const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-        parts[p] = *reinterpret_cast<const uint32_t*>(&h);
-        if (p + 1 < NS) {
-            const float2 f = __bfloat1622float2(h);
-            a -= f.x; b -= f.y;
-        }
-    }
-}
-// byte offset of ONE bf16 element (row r of the tile, K index k inside the K block range) inside a plane: K-major
-// SWIZZLE_128B, 128-byte rows of one 64-wide K block, 16-byte chunks XOR-swizzled by the row (what wgmma reads)
-__device__ __forceinline__ uint32_t b_elem_offset(int r, int k) {
-    const int kb = k >> 6, col = k & 63;
-    return (uint32_t)(kb * (NSEQ * 128) + r * 128 + ((((col >> 3) ^ (r & 7)) << 4) | ((col & 7) << 1)));
-}
 __device__ __forceinline__ unsigned ld_acquire(const unsigned* p) {
     unsigned v;
     asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
@@ -260,7 +178,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, 1) lstm_proj_kernel(ProjArgs P) 
         if (lane == 0) {
             for (int64_t i = 0; i < n_mine; ++i) {
                 const int s = (int)(i % STAGES);
-                mbar_wait(empty_bar(s), ((uint32_t)(i / STAGES) & 1u) ^ 1u);
+                mbar_wait_bounded(empty_bar(s), ((uint32_t)(i / STAGES) & 1u) ^ 1u);
                 const unsigned char* src = P.img + (size_t)(j0 + i * P.ctas_per_combo) * P.tile_stride + P.k_off;
                 mbar_arrive_expect_tx(full_bar(s), (uint32_t)TILE);
                 constexpr int CH = 8192;                                 // divides both tile sizes (24 KB, 96 KB)
@@ -278,7 +196,7 @@ __global__ void __launch_bounds__(PROJ_THREADS, 1) lstm_proj_kernel(ProjArgs P) 
         const float* W = P.wih + (size_t)combo * K * UM;
         for (int64_t i = 0; i < n_mine; ++i) {
             const int s = (int)(i % STAGES);
-            mbar_wait(full_bar(s), (uint32_t)(i / STAGES) & 1u);
+            mbar_wait_bounded(full_bar(s), (uint32_t)(i / STAGES) & 1u);
             float d[2][32];
             mma_tile<KSTEPS>(d, W, smem_base + (uint32_t)(s * TILE), (uint32_t)PLANE, false, warp, lane);
             __syncwarp();
@@ -383,7 +301,7 @@ __global__ void __launch_bounds__(REC_THREADS, 1) lstm_rec_kernel(RecArgs P) {
                 }
             // ---- + W_slice . h_{t-1} (h_{-1} = 0: the first step is G_x alone)
             if (step > 0) {
-                mbar_wait(opfull_bar(slot), fetched & 1u);
+                mbar_wait_bounded(opfull_bar(slot), fetched & 1u);
                 ++fetched;
                 mma_tile<KSTEPS_H>(d, whh, op_u32, (uint32_t)PLANE_BYTES_H, true, wq, lane);
             }
@@ -410,7 +328,7 @@ __global__ void __launch_bounds__(REC_THREADS, 1) lstm_rec_kernel(RecArgs P) {
                         term[p] = (uint32_t)__bfloat16_as_ushort(hb);
                         r -= __bfloat162float(hb);
                     }
-                    unsigned char* dstp = tile + b_elem_offset(n, ucol);
+                    unsigned char* dstp = tile + sw128_offset<NSEQ>(n, ucol);
 #pragma unroll
                     for (int p = 0; p < NS; ++p) {                      // units (even, odd) = lanes (l, l + 4): one 4-byte store
                         const uint32_t nbv = __shfl_down_sync(0xffffffffu, term[p], 4);
@@ -496,13 +414,8 @@ int groups_for_device() {
 template <int KB>
 int launch_proj(const ProjArgs& a, cudaStream_t st) {
     constexpr size_t smem = (size_t)2 * NS * KB * NSEQ * 128 + 1024 + 128;
-    static bool attr_set_dev[64] = {};
-    int dev_ = 0;
-    cudaGetDevice(&dev_);
-    if (!attr_set_dev[dev_ & 63]) {
-        NERRF_CHECK_CUDA(cudaFuncSetAttribute(lstm_proj_kernel<KB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set_dev[dev_ & 63] = true;
-    }
+    const int rc = set_max_dynamic_smem((const void*)lstm_proj_kernel<KB>, smem);
+    if (rc) return rc;
     lstm_proj_kernel<KB><<<16 * a.ctas_per_combo, PROJ_THREADS, smem, st>>>(a);
     return launch_status("lstm_proj_kernel");
 }
@@ -537,13 +450,8 @@ int lstm_layers_umma(const float* seq, const int32_t* len, int64_t B, int T, int
     const int blk = sm_count() * 4;
     const int ctas_per_combo = sm_count() / 16 > 0 ? sm_count() / 16 : 1;
     lstm_image_kernel<<<blk, 256, 0, st>>>(seq, D_in, B, T, n_bt, img0);
-    static bool attr_set_dev[64] = {};
-    int dev_ = 0;
-    cudaGetDevice(&dev_);
-    if (!attr_set_dev[dev_ & 63]) {
-        NERRF_CHECK_CUDA(cudaFuncSetAttribute(lstm_rec_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)REC_SMEM));
-        attr_set_dev[dev_ & 63] = true;
-    }
+    int rc = set_max_dynamic_smem((const void*)lstm_rec_kernel, REC_SMEM);
+    if (rc) return rc;
     for (int l = 0; l < num_layers; ++l) {
         // ---- input projection: one launch per K range, 16 (direction, slice) combos each
         const unsigned char* in_img = l == 0 ? img0 : img[(l - 1) & 1];
@@ -561,7 +469,7 @@ int lstm_layers_umma(const float* seq, const int32_t* len, int64_t B, int T, int
             a.k_off = l == 0 ? 0 : (size_t)kr * TILE_BYTES_H;
             a.wih = wih; a.bias = kr == 0 ? bp : nullptr; a.gx = kr == 0 ? gxa : gxb;
             a.n_tiles = n_tiles; a.rows_total = (int64_t)T * Bp; a.ctas_per_combo = ctas_per_combo;
-            const int rc = l == 0 ? launch_proj<1>(a, st) : launch_proj<KB_H>(a, st);
+            rc = l == 0 ? launch_proj<1>(a, st) : launch_proj<KB_H>(a, st);
             if (rc) return rc;
         }
         for (int d = 0; d < 2; ++d)

@@ -766,16 +766,11 @@ static MctsLayout mcts_layout(int A, int T, int R) {
 template <int NW>
 static int launch_mcts(MctsArgs& args, int grid, cudaStream_t st) {
     const size_t smem = mcts_smem_bytes<NW>();
-    static bool attr_set_dev[64] = {};
-    int dev_ = 0;
-    cudaGetDevice(&dev_);
-    if (!attr_set_dev[dev_ & 63]) {
-        NERRF_CHECK_CUDA(cudaFuncSetAttribute(mcts_search_kernel<NW>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int per_sm = 0;
-        NERRF_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, mcts_search_kernel<NW>, MCTS_THREADS, smem));
-        NERRF_REQUIRE(per_sm >= 1, "mcts kernel does not fit on an SM");
-        attr_set_dev[dev_ & 63] = true;
-    }
+    const int rc = set_max_dynamic_smem((const void*)mcts_search_kernel<NW>, smem);
+    if (rc) return rc;
+    int per_sm = 0;
+    NERRF_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, mcts_search_kernel<NW>, MCTS_THREADS, smem));
+    NERRF_REQUIRE(per_sm >= 1, "mcts kernel does not fit on an SM");
     void* kargs[] = {(void*)&args};
     NERRF_CHECK_CUDA(cudaLaunchCooperativeKernel((void*)mcts_search_kernel<NW>, dim3(grid), dim3(MCTS_THREADS), kargs, smem, st));
     return NERRF_OK;
@@ -798,10 +793,12 @@ extern "C" int nerrf_reward_score(const uint32_t* states, int64_t B, const float
     cudaStream_t st = (cudaStream_t)stream;
     if (NW == 1) reward_score_kernel<1><<<(unsigned)g, 256, terms_smem_bytes<1>(), st>>>(states, B, p, size, cost, guard, A, out);
     else if (NW == 2) {                                                   // 50 / 100 KB of staged terms: above the 48 KB default
-        NERRF_CHECK_CUDA(cudaFuncSetAttribute(reward_score_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)terms_smem_bytes<2>()));
+        const int rc = set_max_dynamic_smem((const void*)reward_score_kernel<2>, terms_smem_bytes<2>());
+        if (rc) return rc;
         reward_score_kernel<2><<<(unsigned)g, 256, terms_smem_bytes<2>(), st>>>(states, B, p, size, cost, guard, A, out);
     } else {
-        NERRF_CHECK_CUDA(cudaFuncSetAttribute(reward_score_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)terms_smem_bytes<4>()));
+        const int rc = set_max_dynamic_smem((const void*)reward_score_kernel<4>, terms_smem_bytes<4>());
+        if (rc) return rc;
         reward_score_kernel<4><<<(unsigned)g, 256, terms_smem_bytes<4>(), st>>>(states, B, p, size, cost, guard, A, out);
     }
     return launch_status("reward_score_kernel");
@@ -965,7 +962,8 @@ extern "C" int nerrf_plan_commit(const float* p, const float* size, const float*
     if (grid > sm_count()) grid = sm_count();
     void* kargs[] = {(void*)&a};
     auto go = [&](auto kern, size_t smem) -> int {
-        NERRF_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        const int rc = set_max_dynamic_smem((const void*)kern, smem);
+        if (rc) return rc;
         NERRF_CHECK_CUDA(cudaLaunchCooperativeKernel((void*)kern, dim3(grid), dim3(256), kargs, smem, st));
         return NERRF_OK;
     };

@@ -6,6 +6,7 @@
 // This file holds the fp32 CUDA-core (FFMA) fused kernel, the standalone K1, the heads, the
 // whole-forward driver and the host-buffer session.  The tensor-core (wgmma) fused kernel is sage_umma.cu.
 #include "common.cuh"
+#include "ptx.cuh"
 #include "sage_gather.cuh"
 
 namespace nerrf {
@@ -15,7 +16,6 @@ int sage_layer_umma(const float* x, const void* rowptr, int is64, const int32_t*
                     int64_t row_end, int F, int relu, int nsplit, const float* node_w, float node_b, float* score,
                     void* long_ws, size_t long_ws_bytes, bool reuse_scan, float* const* peer_out, int n_peers,
                     const uint8_t* peer_need, cudaStream_t st);   // sage_umma.cu (node_w != NULL: node head fused into the epilogue)
-bool sage_umma_available();
 
 // ------------------------------------------------------------------------------------------
 // K1 standalone: one warp per destination row.
@@ -48,14 +48,6 @@ struct FfmaCfg {
     static constexpr size_t smem = (size_t)(BM * LDA + 2 * KC * HH) * sizeof(float);
 };
 
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
-    unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;\n" ::"r"(s), "l"(gmem));
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;\n" ::); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
-
 template <int F, typename RP>
 __global__ void __launch_bounds__(256, 2)
 sage_layer_ffma_kernel(const float* __restrict__ x, const RP* __restrict__ rowptr, const int32_t* __restrict__ col,
@@ -77,7 +69,7 @@ sage_layer_ffma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
 #pragma unroll
         for (int i = 0; i < (KC * HH / 4) / 256; ++i) {
             int idx = tid + i * 256;
-            cp_async16(dst + idx * 4, src + idx * 4);
+            cp_async16(smem_u32(dst + idx * 4), src + idx * 4);
         }
         cp_async_commit();
     };
@@ -212,15 +204,8 @@ template <int F, typename RP>
 static int launch_ffma(const float* x, const RP* rowptr, const int32_t* col, const float* ew, const float* W,
                        const float* b, float* out, int64_t row_begin, int64_t row_end, int relu, cudaStream_t st) {
     using C = FfmaCfg<F>;
-    static bool attr_set_dev[64] = {};
-    int dev_ = 0;
-    cudaGetDevice(&dev_);
-    bool& attr_set = attr_set_dev[dev_ & 63];          // function attributes are per device
-    if (!attr_set) {
-        NERRF_CHECK_CUDA(cudaFuncSetAttribute(sage_layer_ffma_kernel<F, RP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              (int)C::smem));
-        attr_set = true;
-    }
+    const int rc = set_max_dynamic_smem((const void*)sage_layer_ffma_kernel<F, RP>, C::smem);
+    if (rc) return rc;
     const int64_t rows = row_end - row_begin;
     const int64_t tiles = (rows + BM - 1) / BM;
     if (tiles == 0) return NERRF_OK;
@@ -297,7 +282,7 @@ static int layer_fwd_impl(const float* x, const void* rowptr, int rowptr_is64, c
     cudaStream_t st = (cudaStream_t)stream;
     const bool reuse_scan = (algo & NERRF_SAGE_FLAG_REUSE_LONG_SCAN) != 0;
     algo &= 0xFF;
-    if (algo == NERRF_SAGE_ALGO_AUTO) algo = sage_umma_available() ? NERRF_SAGE_ALGO_UMMA : NERRF_SAGE_ALGO_FFMA;
+    if (algo == NERRF_SAGE_ALGO_AUTO) algo = NERRF_SAGE_ALGO_UMMA;
     if (algo == NERRF_SAGE_ALGO_UMMA || algo == NERRF_SAGE_ALGO_UMMA2)
         return sage_layer_umma(x, rowptr, rowptr_is64, col, ew, W, b, out, n_nodes, row_begin, row_end, F, relu,
                                algo == NERRF_SAGE_ALGO_UMMA ? 3 : 2, node_w, node_b, score, long_ws, long_ws_bytes,

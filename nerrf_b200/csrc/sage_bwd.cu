@@ -226,13 +226,8 @@ int launch_bwd(const float* h, const float* m, const float* y, const float* dy, 
     float* dz = ws;
     float* part = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(ws) + p.dz_bytes);
     float* dbpart = part + (size_t)p.chunks * 2 * F * HB;
-    static bool attr_set[64] = {};
-    int dev_ = 0;
-    cudaGetDevice(&dev_);
-    if (!attr_set[dev_ & 63]) {
-        NERRF_CHECK_CUDA(cudaFuncSetAttribute(sage_bwd_dz_kernel<F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)DZ_SMEM));
-        attr_set[dev_ & 63] = true;
-    }
+    const int rc = set_max_dynamic_smem((const void*)sage_bwd_dz_kernel<F>, DZ_SMEM);
+    if (rc) return rc;
     if (dW) {
         sage_bwd_dw_kernel<F><<<dim3((unsigned)p.chunks, 2 * F / DW_KS), 256, 0, st>>>(h, m, dy, y, part, dbpart, n, p.rows_per_chunk, relu);
         sage_bwd_reduce_kernel<<<(2 * F * HB + 255) / 256, 256, 0, st>>>(part, dW, 2 * F * HB, p.chunks);

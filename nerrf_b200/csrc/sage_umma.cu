@@ -21,19 +21,18 @@
 //   warps 0-7   two consumer warpgroups (output features 0-63 and 64-127): wgmma (A in registers, B from shared
 //               memory), then the epilogue from the accumulator registers: + bias, ReLU, row stores, fused node head
 //   warp  8     edge-block loader: stages each tile's rowptr words and its col / ew slices into shared memory --
-//               the slices as two BULK async copies (cp.async.bulk, byte count on the stage's mbarrier) --
+//               the slices as two bulk async copies (cp.async.bulk, byte count on the stage's mbarrier) --
 //               running up to IDX_STAGES tiles ahead; the next tile's rowptr words are prefetched before it
 //               waits for a free stage
-//   warps 9-..  gather: one CSR row per warp at a time, rows round-robin; source rows are copied into the warp's
-//               shared-memory ring with cp.async (16 B per lane) or, as an option, one bulk async copy per row;
+//   warps 9-..  gather: one CSR row per warp at a time (four at F=32), rows round-robin; source rows are copied into the
+//               warp's shared-memory ring with cp.async (LDGSTS, 16 B per lane), NQ-1 sub-batches in flight;
 //               indices come from shared memory, so the only global latency a row exposes is its x rows
 // Pipelines: idx stages full/empty (loader <-> gather), smem operand stages full/empty (gather <-> consumer).
-#include <cuda_bf16.h>
-#include <stdlib.h>
 #include <map>
 #include <mutex>
 #include <utility>
 #include "common.cuh"
+#include "ptx.cuh"
 #include "sage_gather.cuh"
 
 namespace nerrf {
@@ -78,114 +77,6 @@ struct UmmaCfg {
     static_assert(STAGES >= 2, "need at least two smem stages");
 };
 
-// ---------------------------------------------------------------- PTX wrappers
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(bar) : "memory");
-}
-// arrive (count 1) and add `bytes` to the phase's pending transaction count: the phase completes when the
-// arrival count AND the byte count are both satisfied
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(bar), "r"(bytes) : "memory");
-}
-// bulk async copy global -> shared (the non-tensor TMA path, SASS UBLKCP): `bytes` (multiple of 16) from a 16-byte
-// aligned global address to a 16-byte aligned shared address; completion is signalled on `bar` as complete_tx(bytes)
-__device__ __forceinline__ void bulk_g2s(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_dst), "l"(gsrc), "r"(bytes), "r"(bar)
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    uint32_t done;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(bar), "r"(parity)
-            : "memory");
-    } while (!done);
-}
-// for the roles that have slack (consumer warpgroups, loader): poll with a sleep so they do not burn
-// the issue slots the gather warps need (a tile period is ~10 us)
-__device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity) {
-    uint32_t done;
-    while (true) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(bar), "r"(parity)
-            : "memory");
-        if (done) break;
-        __nanosleep(400);
-    }
-}
-// predicated 16-byte async copy (no branch)
-__device__ __forceinline__ void cp_async16_pred(uint32_t smem_dst, const void* gsrc, bool pred) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %2, 0;\n\t"
-        "@p cp.async.cg.shared.global [%0], [%1], 16;\n\t}"
-        ::"r"(smem_dst), "l"(gsrc), "r"((uint32_t)pred)
-        : "memory");
-}
-__device__ __forceinline__ void cp_async16(uint32_t smem_dst, const void* gsrc) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_dst), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-// wgmma shared-memory matrix descriptor (sm_90): K-major, SWIZZLE_128B, 8-row groups 1024 B apart (SBO); the leading
-// byte offset is unused for swizzled K-major operands.  A K step inside the 128-byte swizzle atom advances the start
-// address by 32 bytes (the atom itself is 1024-byte aligned).
-__device__ __forceinline__ uint64_t make_b_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);          // start address
-    d |= (uint64_t)1 << 16;                               // LBO (unused)
-    d |= (uint64_t)(1024 >> 4) << 32;                     // SBO = 1024 B
-    d |= (uint64_t)1 << 62;                               // SWIZZLE_128B
-    return d;
-}
-__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// D[64 x 32] (+)= A[64 x 16] (bf16 register fragment) . B[16 x 32] (bf16, K-major shared memory), fp32 accumulate
-__device__ __forceinline__ void wgmma_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %21, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-        "{%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
-          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)
-        : "memory");
-}
-
-// split fp32 values into NS bf16 terms of the running residual; pairs packed (first element low)
-template <int NS>
-__device__ __forceinline__ void split_pair(float a, float b, uint32_t (&parts)[NS]) {
-#pragma unroll
-    for (int p = 0; p < NS; ++p) {
-        const __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-        parts[p] = *reinterpret_cast<const uint32_t*>(&h);
-        if (p + 1 < NS) {
-            const float2 f = __bfloat1622float2(h);
-            a -= f.x; b -= f.y;                        // exact: the residual is representable in fp32
-        }
-    }
-}
 template <int NS>
 __device__ __forceinline__ void split4(const float4 v, uint2 (&parts)[NS]) {
     uint32_t lo[NS], hi[NS];
@@ -193,13 +84,6 @@ __device__ __forceinline__ void split4(const float4 v, uint2 (&parts)[NS]) {
     split_pair<NS>(v.z, v.w, hi);
 #pragma unroll
     for (int p = 0; p < NS; ++p) parts[p] = make_uint2(lo[p], hi[p]);
-}
-
-// byte offset of element (row r, k) inside one hi/lo part of a stage (k multiple of 4)
-__device__ __forceinline__ uint32_t b_offset(int r, int k) {
-    const int kb = k >> 6, col = k & 63;
-    const int chunk = col >> 3;                            // 16-byte chunk in the 128-byte row
-    return (uint32_t)(kb * (TN * 128) + r * 128 + (((chunk ^ (r & 7)) << 4) | ((col & 7) << 1)));
 }
 
 // ---------------------------------------------------------------- fused exchange (multi-GPU)
@@ -234,7 +118,7 @@ struct LongWs {
     int* hdr;              // [0] = number of chunk items claimed (may exceed cap), [1] = cap
     int* hash_key;         // row + 1, 0 = empty
     int* hash_val;         // first item of the row
-    int2* queue;           // (row - row_begin? no: absolute row as two ints) -> see pack/unpack
+    int2* queue;           // per chunk item: (absolute row, chunk index within the row)
     float* partial;        // [cap][128]
     float* pw;             // [cap]
     int cap;
@@ -337,11 +221,7 @@ __global__ void __launch_bounds__(256) long_chunk_kernel(const float* __restrict
 
 // LONG: compiled with the hub-row (pre-aggregated partial items) paths; the plain variant is used when the
 // launch has no hub-row scratch, so graphs without hub rows pay nothing for the feature.
-// BULK: source rows travel as one bulk async copy each (cp.async.bulk) instead of 32 lanes x 16-byte cp.async
-// (LDGSTS).  At one bulk request per 128..512-byte row the copy engine's request rate, not HBM, becomes the limiter,
-// so the LDGSTS transport is the default; the edge-block slices (col / ew, kilobytes per request) use bulk copies in
-// both variants.
-template <int F, int NS, typename RP, bool LONG, bool BULK>
+template <int F, int NS, typename RP, bool LONG>
 __global__ void __launch_bounds__((UmmaCfg<F, NS>::THREADS), 1)
 sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowptr, const int32_t* __restrict__ col,
                        const float* __restrict__ ew, const float* __restrict__ W, const float* __restrict__ bias,
@@ -355,15 +235,14 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
     const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;          // SWIZZLE_128B needs 1024-B alignment
     unsigned char* smem_gen = smem_dyn + (smem_base - smem_u32(smem_dyn));
     const uint32_t idx_base = smem_base + C::STAGES * C::STAGE_BYTES;
-    const uint32_t bar_base = idx_base + IDX_STAGES * IDX_STAGE_BYTES;     // 256 B of barriers, then the gather rings
+    // 1 KB barrier area, then the gather rings: the stage mbarriers in the first 256 B, end_tl and the tile-id ring in
+    // the last 72 B, the bytes in between unused
+    const uint32_t bar_base = idx_base + IDX_STAGES * IDX_STAGE_BYTES;
     auto full_bar = [&](int s) { return bar_base + 8u * s; };
     auto empty_bar = [&](int s) { return bar_base + 8u * (C::STAGES + s); };
     auto idxf_bar = [&](int q) { return bar_base + 8u * (2 * C::STAGES + q); };
     auto idxe_bar = [&](int q) { return bar_base + 8u * (2 * C::STAGES + IDX_STAGES + q); };
     static_assert(8 * (2 * C::STAGES + 2 * IDX_STAGES) <= 256, "barrier area");
-    // per gather warp: NQ ring-slot barriers (bulk-copy byte counts), private to the warp
-    auto ring_bar = [&](int g, int q) { return bar_base + 256u + 8u * (uint32_t)(g * NQ + q); };
-    static_assert(256 + GATHER_WARPS * NQ * 8 <= 1024 - 64, "barrier area");
     // DYNAMIC TILE SCHEDULE: the loader warp claims tiles from a global counter (tile_ctr, zero at launch) and publishes
     // the id of the CTA's tl-th tile in this ring (-1 = end of stream) before it releases the tile's edge block; every
     // role reads it after the mbarrier wait that orders it behind that release.  Rows are not equally expensive (hub
@@ -375,9 +254,8 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
     // arrivals -- is paid once per four rows and by all 32 lanes (one row per warp leaves the F=32 layer issue-bound on
     // this overhead).  Units of 4 rows are dealt round-robin to the warps; a warp need not
     // own a unit in every tile, so the end of the tile stream is also published in `end_tl` (the closing tile's index).
-    constexpr bool QUAD = (F == 32) && !BULK;
+    constexpr bool QUAD = F == 32;
     volatile int* end_tl = reinterpret_cast<volatile int*>(smem_gen + (bar_base + 1024 - 64 - 8 - smem_base));
-    static_assert(256 + GATHER_WARPS * NQ * 8 <= 1024 - 64 - 8, "barrier area");
     unsigned char* idx_gen = smem_gen + (idx_base - smem_base);
     const uint32_t ring_base = bar_base + 1024;
     float* head_red = reinterpret_cast<float*>(smem_gen + (ring_base - smem_base) + (size_t)GATHER_WARPS * C::RING_BYTES);   // [2][8][32]
@@ -392,10 +270,8 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
             for (int s = 0; s < C::STAGES; ++s) { mbar_init(full_bar(s), QUAD ? TN / 4 : TN); mbar_init(empty_bar(s), EPI_WARPS); }
             *end_tl = 0x7fffffff;
             // idx full: ONE arrive.expect_tx by the loader (publishes the rowptr words, counts the bytes of the two bulk
-            // copies); empty: one per gather warp.  ring slots: one arrive.expect_tx by the issuing lane per use
+            // copies); empty: one per gather warp (per 4-row unit in QUAD mode)
             for (int q = 0; q < IDX_STAGES; ++q) { mbar_init(idxf_bar(q), 1); mbar_init(idxe_bar(q), QUAD ? TN / 4 : GATHER_WARPS); }
-            for (int g = 0; g < GATHER_WARPS; ++g)
-                for (int q = 0; q < NQ; ++q) mbar_init(ring_bar(g, q), 1);
             fence_barrier_init();
         }
         __syncwarp();
@@ -607,11 +483,11 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                 unsigned char* st = smem_gen + (size_t)s * C::STAGE_BYTES;
                 uint2 parts[NS];
                 split4<NS>(self, parts);
-                uint32_t off = b_offset(r, 4 * sub);
+                uint32_t off = sw128_offset<TN>(r, 4 * sub);
 #pragma unroll
                 for (int p = 0; p < NS; ++p) *reinterpret_cast<uint2*>(st + p * C::PART_BYTES + off) = parts[p];
                 split4<NS>(mean, parts);
-                off = b_offset(r, F + 4 * sub);
+                off = sw128_offset<TN>(r, F + 4 * sub);
 #pragma unroll
                 for (int p = 0; p < NS; ++p) *reinterpret_cast<uint2*>(st + p * C::PART_BYTES + off) = parts[p];
             }
@@ -629,19 +505,17 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
       } else {
         // =========================================================== gather warps (producers of the B operand)
         // Row stream of this warp: i = g, g+G, g+2G, ... over the CTA's tiles.  A row is the item list
-        // [self, edge_0 .. edge_{deg-1}], cut into sub-batches of QS items.  Every item is ONE bulk async copy of a
-        // whole source row (F*4 bytes) into a slot of this warp's shared-memory ring, issued by the lane that owns
-        // the item; the slot's mbarrier counts the bytes.  NQ-1 sub-batches stay in flight while the oldest is
-        // consumed (LDS + FFMA), so memory-level parallelism is bounded by the ring, not by registers, no load ever
-        // stalls a scoreboard, and a source row costs one copy instruction instead of one per 16 bytes.
+        // [self, edge_0 .. edge_{deg-1}], cut into sub-batches of QS items.  A sub-batch is one cp.async group into a
+        // slot of this warp's shared-memory ring: each warp-wide 16-byte cp.async (LDGSTS) copies G whole source rows.
+        // NQ-1 sub-batches stay in flight while the oldest is consumed (LDS + FFMA), so memory-level parallelism is
+        // bounded by the ring, not by registers, and no load ever stalls a scoreboard.
         constexpr int G = 32 / LPR;                                     // items consumed by one warp-wide LDS.128
         constexpr int QS = C::QS;
         constexpr int SLOT_FLOATS = QS * F;
-        constexpr uint32_t ROW_BYTES = F * 4;
         const int g = warp - GATHER_WARP0;
         const int grp = lane / LPR, sub = lane % LPR;
-        // LDGSTS transport: lane (grp, sub) moves bytes [16 sub, 16 sub + 16) of item t + grp; bulk: whole rows
-        const uint32_t ring_u32 = ring_base + (uint32_t)(g * C::RING_BYTES) + (BULK ? 0u : (uint32_t)((grp * F + 4 * sub) * 4));
+        // lane (grp, sub) moves bytes [16 sub, 16 sub + 16) of item t + grp
+        const uint32_t ring_u32 = ring_base + (uint32_t)(g * C::RING_BYTES) + (uint32_t)((grp * F + 4 * sub) * 4);
         const float* xs = x + 4 * sub;
         const float* ring_gen = reinterpret_cast<const float*>(smem_gen + (ring_base - smem_base) + (size_t)g * C::RING_BYTES) + grp * F + 4 * sub;
         int stream_end = 0x7fffff00;                                     // rows of this CTA's tile stream; known once the
@@ -705,8 +579,8 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                 cnb = (citems + QS - 1) / QS;
             }
         };
-        // LDGSTS transport: one cp.async group = sub-batch `ib` of the issue row, into ring slot `slot`
-        auto issue_ldgsts = [&](int slot) {
+        // one cp.async group = sub-batch `ib` of the issue row, into ring slot `slot`
+        auto issue = [&](int slot) {
             if (ii < stream_end) {
                 if (ideg >= 0) {
                     const int first = ib * QS;
@@ -751,36 +625,6 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
             }
             cp_async_commit();                                            // (possibly empty) group keeps the count in step
         };
-        // sub-batch `ib` of the issue row -> ring slot `slot`: lane j < nitems copies item j (one bulk copy per source row)
-        auto issue_bulk = [&](int slot) {
-            const uint32_t bar = ring_bar(g, slot);
-            uint32_t tx = 0;
-            if (ii < stream_end) {
-                if (ideg >= 0) {
-                    const int first = ib * QS;
-                    int nitems = iitems - first;                         // items left in the row (>= 1)
-                    nitems = nitems < QS ? nitems : QS;
-                    tx = (uint32_t)nitems * ROW_BYTES;
-                    if (lane == 0) mbar_arrive_expect_tx(bar, tx);
-                    if (lane < nitems) {
-                        const int it = first + lane;                     // item number inside the row; 0 = the self row
-                        const int k = ie0 + it - 1;                      // its edge, relative to the staged slice
-                        const float* srcp;
-                        if (it == 0) srcp = x + (size_t)irow * F;
-                        else if (LONG && ilong >= 0) srcp = lw.partial + (size_t)(ilong + it - 1) * 128;   // pre-aggregated chunk
-                        else srcp = x + (size_t)(uint32_t)((k < EMAX) ? icol[k] : __ldg(col + ielo + k)) * F;
-                        bulk_g2s(ring_u32 + (uint32_t)((slot * QS + lane) * (int)ROW_BYTES), srcp, ROW_BYTES, bar);
-                    }
-                }
-                if (++ib >= inb) {
-                    ii += GATHER_WARPS;
-                    if (ii < stream_end) setup_issue_row();
-                }
-            }
-            if (tx == 0 && lane == 0) mbar_arrive(bar);                   // empty sub-batch: keeps the slot's phase in step
-        };
-
-        auto issue = [&](int slot) { if constexpr (BULK) issue_bulk(slot); else issue_ldgsts(slot); };
 
         if (ii < stream_end) { setup_issue_row(); }
         if (ci < stream_end) { setup_consume_row(); }
@@ -790,16 +634,10 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
         float4 acc = make_float4(0.f, 0.f, 0.f, 0.f), self = acc;
         float wsum = 0.f;
         int last_tl = -1;
-        uint32_t ring_phase = 0;                                          // bit q = parity to wait for on ring slot q
         while (ci < stream_end) {
-            if constexpr (BULK) {
-                mbar_wait(ring_bar(g, cslot), (ring_phase >> cslot) & 1u);    // oldest sub-batch landed (all its bytes)
-                ring_phase ^= 1u << cslot;
-            } else {
-                cp_async_wait<NQ - 2>();                                  // oldest group landed (this lane's part) ...
-            }
-            __syncwarp();                                                 // ... and everyone else's;                                                 // all lanes are done reading the slot consumed
-                                                                          // last iteration
+            cp_async_wait<NQ - 2>();                                      // oldest group landed (this lane's part) ...
+            __syncwarp();                                                 // ... and everyone else's; all lanes are done
+                                                                          // reading the slot consumed last iteration
             issue(islot);                                                 // refill that slot
             islot = (islot + 1) % NQ;
             if (cdeg >= 0) {
@@ -876,11 +714,11 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                     unsigned char* st = smem_gen + (size_t)s * C::STAGE_BYTES;
                     uint2 parts[NS];
                     split4<NS>(self, parts);
-                    uint32_t off = b_offset(r, 4 * lane);
+                    uint32_t off = sw128_offset<TN>(r, 4 * lane);
 #pragma unroll
                     for (int p = 0; p < NS; ++p) *reinterpret_cast<uint2*>(st + p * C::PART_BYTES + off) = parts[p];
                     split4<NS>(mean, parts);
-                    off = b_offset(r, F + 4 * lane);
+                    off = sw128_offset<TN>(r, F + 4 * lane);
 #pragma unroll
                     for (int p = 0; p < NS; ++p) *reinterpret_cast<uint2*>(st + p * C::PART_BYTES + off) = parts[p];
                 }
@@ -895,7 +733,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
             ci += GATHER_WARPS;
             if (ci < stream_end) setup_consume_row();
         }
-        if constexpr (!BULK) cp_async_wait<0>();
+        cp_async_wait<0>();
       }
     } else if (warp == LOADER_WARP) {
         // =========================================================== edge-block loader
@@ -1083,7 +921,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
 #pragma unroll
                     for (int nb = 0; nb < 4; ++nb) { hb[8 * nb + 2 * c] = part[2 * nb]; hb[8 * nb + 2 * c + 1] = part[2 * nb + 1]; }
                 }
-                asm volatile("bar.sync 1, 256;" ::: "memory");          // the eight consumer warps
+                named_bar(1, 256);                                       // the eight consumer warps
                 if (warp == 0) {
                     const float* hr = head_red + (int)(tl & 1) * EPI_WARPS * 32 + lane;
                     const float dot = ((hr[0] + hr[32]) + (hr[64] + hr[96])) + ((hr[128] + hr[160]) + (hr[192] + hr[224]));
@@ -1114,14 +952,6 @@ __global__ void __launch_bounds__(256) split_w_kernel(const float* __restrict__ 
     }
 #pragma unroll
     for (int p = 0; p < NS; ++p) wsplit[(size_t)((2 * j + h) * NS + p) * 128 + t] = make_uint4(a[p][0], a[p][1], a[p][2], a[p][3]);
-}
-
-// the per-row bulk-copy transport is an experiment knob (NERRF_SAGE_ROW_COPY=bulk), compiled for the headline shapes only
-template <int F, int NS, typename RP>
-constexpr bool kBulkVariant = (NS == 3) && (F == 32 || F == 128) && (sizeof(RP) == 4);
-inline bool bulk_rows_requested() {
-    static const bool v = [] { const char* e = getenv("NERRF_SAGE_ROW_COPY"); return e && e[0] == 'b'; }();
-    return v;
 }
 
 // per-device ring of launch-private tile counters (1 KB, allocated on first use and kept): a launch zeroes its slot on its
@@ -1158,17 +988,9 @@ int launch_umma(const float* x, const RP* rowptr, const int32_t* col, const floa
                 float* out, int64_t row_begin, int64_t row_end, int relu, const float* node_w, float node_b, float* score,
                 void* long_ws, size_t long_ws_bytes, bool reuse_scan, const Peers& peers, cudaStream_t st) {
     using C = UmmaCfg<F, NS>;
-    static bool attr_set_dev[64] = {};
-    int dev_ = 0;
-    cudaGetDevice(&dev_);
-    bool& attr_set = attr_set_dev[dev_ & 63];          // function attributes are per device
-    if (!attr_set) {
-        NERRF_CHECK_CUDA(cudaFuncSetAttribute(sage_layer_umma_kernel<F, NS, RP, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
-        NERRF_CHECK_CUDA(cudaFuncSetAttribute(sage_layer_umma_kernel<F, NS, RP, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
-        if constexpr (kBulkVariant<F, NS, RP>)
-            NERRF_CHECK_CUDA(cudaFuncSetAttribute(sage_layer_umma_kernel<F, NS, RP, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::SMEM));
-        attr_set = true;
-    }
+    int rc = set_max_dynamic_smem((const void*)sage_layer_umma_kernel<F, NS, RP, false>, C::SMEM);
+    if (!rc) rc = set_max_dynamic_smem((const void*)sage_layer_umma_kernel<F, NS, RP, true>, C::SMEM);
+    if (rc) return rc;
     const int64_t rows = row_end - row_begin;
     const int64_t tiles = (rows + TN - 1) / TN;
     if (tiles == 0) return NERRF_OK;
@@ -1183,7 +1005,7 @@ int launch_umma(const float* x, const RP* rowptr, const int32_t* col, const floa
             long_scan_kernel<RP><<<sms * 4, 256, 0, st>>>(rowptr, row_begin, row_end, lw);
         }
         long_chunk_kernel<F, RP><<<sms * 4, 256, 0, st>>>(x, rowptr, col, ew, lw);
-        int rc = launch_status("long-row pre-pass");
+        rc = launch_status("long-row pre-pass");
         if (rc) return rc;
     }
     const int64_t grid = tiles < sm_count() ? tiles : sm_count();
@@ -1194,21 +1016,15 @@ int launch_umma(const float* x, const RP* rowptr, const int32_t* col, const floa
     uint4* wsplit = wsplit_buffer(st);
     if (!wsplit) { set_error("could not allocate the split-weight scratch"); return NERRF_ERR_CUDA; }
     split_w_kernel<NS><<<(C::KSTEPS * 2 * 128 + 255) / 256, 256, 0, st>>>(W, C::KSTEPS, wsplit);
-    // the per-row bulk-copy transport needs 16-byte aligned rows; every transport stages col / ew with bulk copies,
-    // which only need 4-byte aligned slices (the aligned superset is copied)
+    // the col / ew slices are staged with bulk copies, which only need 4-byte aligned slices (the aligned superset is copied)
     if (lw.cap > 0)
-        sage_layer_umma_kernel<F, NS, RP, true, false><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit);
-    else if (kBulkVariant<F, NS, RP> && bulk_rows_requested() && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
-        if constexpr (kBulkVariant<F, NS, RP>)
-            sage_layer_umma_kernel<F, NS, RP, false, true><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit);
-    } else
-        sage_layer_umma_kernel<F, NS, RP, false, false><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit);
+        sage_layer_umma_kernel<F, NS, RP, true><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit);
+    else
+        sage_layer_umma_kernel<F, NS, RP, false><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit);
     return launch_status("sage_layer_umma_kernel");
 }
 
 }  // namespace
-
-bool sage_umma_available() { return true; }
 
 int sage_layer_umma(const float* x, const void* rowptr, int is64, const int32_t* col, const float* ew, const float* W,
                     const float* b, float* out, int64_t n_nodes, int64_t row_begin, int64_t row_end, int F, int relu,
