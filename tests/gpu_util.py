@@ -1,6 +1,10 @@
 import numpy as np
 import torch
 
+# atol_rms of assert_close_fp32 per GraphSAGE-T layer algo.  "umma2" (2-term bf16 split) is ~1e-5 relative to the tensor
+# scale: within the north star's 1e-4 bound but not within the strict absolute floor used for the fp32-equivalent paths.
+ATOL_RMS = {"ffma": 1e-5, "umma": 1e-5, "umma2": 1e-4, "auto": 1e-5}
+
 
 def dev_graph(g, device="cuda", rowptr64=False):
     rp = torch.from_numpy(g.rowptr.astype(np.int64 if rowptr64 else g.rowptr.dtype)).to(device)
