@@ -56,6 +56,10 @@ __device__ __forceinline__ void bulk_g2s(uint32_t smem_dst, const void* gsrc, ui
                  ::"r"(smem_dst), "l"(gsrc), "r"(bytes), "r"(bar)
                  : "memory");
 }
+// bulk prefetch of `bytes` (multiple of 16) from a 16-byte aligned global address into L2, no completion signal
+__device__ __forceinline__ void bulk_prefetch_l2(const void* gsrc, uint32_t bytes) {
+    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gsrc), "r"(bytes) : "memory");
+}
 __device__ __forceinline__ void cp_async16(uint32_t smem_dst, const void* gsrc) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_dst), "l"(gsrc) : "memory");
 }

@@ -5,9 +5,13 @@
 // computed TRANSPOSED so that the gathered tile is the shared-memory operand and the weights travel in registers:
 //
 //   D^T[H=128 features, rows] = W^T[128, K=2F] . X^T[K, rows]      (one m64n32k16 wgmma half per consumer warpgroup)
-//     A operand = W^T, register fragments split into bf16 terms once per launch (split_w_kernel) and read from L2 by the
-//                 consumer warpgroups: the split W^T of an F=128 layer (192 KB) does not fit in shared memory next to
-//                 the gather rings and operand stages, and Hopper has no tensor memory to hold it
+//     A operand = W^T, register fragments split into bf16 terms once per launch and read from L2 by the consumer
+//                 warpgroups: the split W^T of an F=128 layer (192 KB) does not fit in shared memory next to the gather
+//                 rings and operand stages, and Hopper has no tensor memory to hold it
+//     F = 64 / 128: the self half x_v . W[0:F] needs no gather; a prep kernel (sage_self_prep_kernel) computes it over
+//                 contiguous rows of x with W resident in registers and stores the raw accumulators in out, and the
+//                 layer kernel starts from them and runs only the mean half (K = F), which halves its weight traffic.
+//                 F = 32 keeps K = 2F in the layer kernel (split_w_kernel).
 //     B operand = the gathered tile X[rows, K] exactly as the gather warps produce it: row-major, K contiguous ==
 //                 the wgmma "K-major" canonical layout (128-byte swizzle), bf16 terms
 //     D         = fp32 accumulators in the consumer warpgroups' registers
@@ -63,14 +67,18 @@ struct UmmaCfg {
     // block from issue to completion, so the look-ahead is bounded by the number of edge-block stages, not by the rings
     // (with 4 stages most issue-side polls find the next tile not yet staged)
     static constexpr int IDX_STAGES = (F == 32) ? 9 : 3;
-    static constexpr int K = 2 * F;
+    // F = 64 / 128: the self half x_v . W[0:F] is computed by the prep kernel (sage_self_prep_kernel) and the layer kernel
+    // starts its accumulators from it, so a tile carries only the mean columns (K = F).  At F = 32 a mean-only row
+    // (64 B) would be less than one 128-byte swizzle block, so the tile keeps [x_v || m_v] (K = 2F).
+    static constexpr bool SELF_SPLIT = F != 32;
+    static constexpr int K = SELF_SPLIT ? F : 2 * F;
     static constexpr int KB = K / 64;                        // 128-byte K blocks
     static constexpr int KSTEPS = K / 16;                    // MMAs (K=16) per product
     static constexpr int PART_BYTES = KB * TN * 128;         // one bf16 term of one stage
     static constexpr int STAGE_BYTES = NS * PART_BYTES;
     static constexpr int QS = qs_for<F>();                    // 4 (F=128), 8 (F=64), 16 (F=32): always 2 KB per sub-batch
     static constexpr int RING_BYTES = NQ * QS * F * 4;       // per gather warp: NQ sub-batches x QS source rows
-    static constexpr int STAGES = (F == 128) ? 2 : (F == 32 ? 3 : 4);
+    static constexpr int STAGES = (F == 32) ? 3 : 4;
     static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + IDX_STAGES * IDX_STAGE_BYTES +
                                    (size_t)GATHER_WARPS * RING_BYTES + 2048 /*head reduce*/ + 1024 /*align*/ + 1024 /*barriers*/;
     static_assert(SMEM <= 227 * 1024, "shared memory budget");
@@ -106,8 +114,8 @@ __device__ __forceinline__ void multimem_st2(float* addr, const float2 v) {
 // A destination row with more than LONG_T in-edges would be gathered by ONE warp.  A deterministic pre-pass
 // cuts every such row into fixed chunks of LONG_CH edges; one CTA per chunk computes the unnormalised
 // weighted sum + weight sum (fixed order: 8 warps x 64 edges, then warp 0 adds the 8 warp partials in order)
-// into a side buffer.  The main kernel then sees the row as the items [self, partial_0 .. partial_{nc-1}]
-// (weight 1 each, weight-sum from pw[]).  The workspace is capacity driven: rows that do not fit stay inline.
+// into a side buffer.  The main kernel then sees the row as the items [partial_0 .. partial_{nc-1}] (F=32:
+// [self, partial_0 ..]; weight 1 each, weight-sum from pw[]).  The workspace is capacity driven: rows that do not fit stay inline.
 // Threshold: a row of a few hundred edges gathered by one warp takes many times as long as the other 31 rows of its tile,
 // and a trace graph has exactly such a row every 64 nodes (the process node of each component, in-degree = events of
 // its files).
@@ -269,6 +277,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
             // operand stage full: one arrival per row (per 4-row unit in QUAD mode); empty: one per consumer warp
             for (int s = 0; s < C::STAGES; ++s) { mbar_init(full_bar(s), QUAD ? TN / 4 : TN); mbar_init(empty_bar(s), EPI_WARPS); }
             *end_tl = 0x7fffffff;
+            for (int i = 0; i < TILE_RING; ++i) tile_ids[i] = -1;        // (the consumers peek at entries ahead)
             // idx full: ONE arrive.expect_tx by the loader (publishes the rowptr words, counts the bytes of the two bulk
             // copies); empty: one per gather warp (per 4-row unit in QUAD mode)
             for (int q = 0; q < IDX_STAGES; ++q) { mbar_init(idxf_bar(q), 1); mbar_init(idxe_bar(q), QUAD ? TN / 4 : GATHER_WARPS); }
@@ -505,10 +514,12 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
       } else {
         // =========================================================== gather warps (producers of the B operand)
         // Row stream of this warp: i = g, g+G, g+2G, ... over the CTA's tiles.  A row is the item list
-        // [self, edge_0 .. edge_{deg-1}], cut into sub-batches of QS items.  A sub-batch is one cp.async group into a
+        // [edge_0 .. edge_{deg-1}] (the self row is the prep kernel's), cut into sub-batches of QS items; a row without
+        // items travels as one empty sub-batch and writes a zero mean.  A sub-batch is one cp.async group into a
         // slot of this warp's shared-memory ring: each warp-wide 16-byte cp.async (LDGSTS) copies G whole source rows.
         // NQ-1 sub-batches stay in flight while the oldest is consumed (LDS + FFMA), so memory-level parallelism is
         // bounded by the ring, not by registers, and no load ever stalls a scoreboard.
+        static_assert(C::SELF_SPLIT, "the row-per-warp gather writes only the mean columns");
         constexpr int G = 32 / LPR;                                     // items consumed by one warp-wide LDS.128
         constexpr int QS = C::QS;
         constexpr int SLOT_FLOATS = QS * F;
@@ -523,7 +534,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
         int itile = 0, ctile = 0;
 
         // ---- per-row state, issue side (i*) and consume side (c*)
-        int ii = g, ib = 0, inb = 1, ie0 = 0, ideg = -1, itl = -1, ilong = -1, iitems = 0;  uint32_t irow = 0;
+        int ii = g, ib = 0, inb = 1, ie0 = 0, ideg = -1, itl = -1, ilong = -1, iitems = 0;
         const int32_t* icol = nullptr; int64_t ielo = 0;
         int ci = g, cb = 0, cnb = 1, ce0 = 0, cdeg = -1, ctl = -1, clong = -1, citems = 0;
         const float* cew = nullptr; int64_t celo = 0;
@@ -545,16 +556,15 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
             const int64_t row = row_begin + (int64_t)itile * TN + r;
             ib = 0; inb = 1; ideg = -1;
             if (itile >= 0 && row < row_end) {
-                irow = (uint32_t)row;
                 ie0 = rp_s[r];
                 ideg = rp_s[r + 1] - ie0;
-                iitems = ideg + 1;                                       // [self, edges...]
+                iitems = ideg;
                 ilong = -1;
-                if (LONG && ideg > LONG_T && lw.cap > 0) {               // hub row: [self, chunk partials...] if pre-aggregated
+                if (LONG && ideg > LONG_T && lw.cap > 0) {               // hub row: [chunk partials...] if pre-aggregated
                     ilong = long_lookup(lw, row);
-                    if (ilong >= 0) iitems = 1 + (ideg + LONG_CH - 1) / LONG_CH;
+                    if (ilong >= 0) iitems = (ideg + LONG_CH - 1) / LONG_CH;
                 }
-                inb = (iitems + QS - 1) / QS;
+                inb = iitems > 0 ? (iitems + QS - 1) / QS : 1;
             }
         };
         auto setup_consume_row = [&]() {                                // ci < stream_end, tile already staged
@@ -570,13 +580,13 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
             if (ctile >= 0 && row < row_end) {
                 ce0 = rp_s[r];
                 cdeg = rp_s[r + 1] - ce0;
-                citems = cdeg + 1;
+                citems = cdeg;
                 clong = -1;
                 if (LONG && cdeg > LONG_T && lw.cap > 0) {
                     clong = long_lookup(lw, row);
-                    if (clong >= 0) citems = 1 + (cdeg + LONG_CH - 1) / LONG_CH;
+                    if (clong >= 0) citems = (cdeg + LONG_CH - 1) / LONG_CH;
                 }
-                cnb = (citems + QS - 1) / QS;
+                cnb = citems > 0 ? (citems + QS - 1) / QS : 1;
             }
         };
         // one cp.async group = sub-batch `ib` of the issue row, into ring slot `slot`
@@ -584,14 +594,13 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
             if (ii < stream_end) {
                 if (ideg >= 0) {
                     const int first = ib * QS;
-                    const int nitems = iitems - first;                   // items left in the row (>= 1)
+                    const int nitems = iitems - first;                   // items left in the row (0: a row without items)
                     const uint32_t dst = ring_u32 + (uint32_t)(slot * SLOT_FLOATS * 4);
-                    const int kbase = ie0 + first - 1;                   // item `it` of this sub-batch is edge kbase + it
+                    const int kbase = ie0 + first;                       // item `it` of this sub-batch is edge kbase + it
                     if (!(LONG && ilong >= 0) && ie0 + ideg <= EMAX) {   // whole row staged (the common case): branch free
                         uint32_t src[QS / G];
 #pragma unroll
                         for (int t = 0; t < QS; t += G) src[t / G] = (uint32_t)icol[kbase + t + grp];   // slack reads stay in smem
-                        if (first == 0 && grp == 0) src[0] = irow;       // item 0 of the row is the self row
 #pragma unroll
                         for (int t = 0; t < QS; t += G)
                             cp_async16_pred(dst + (uint32_t)(t * F * 4), xs + (size_t)src[t / G] * F, t + grp < nitems);
@@ -599,11 +608,8 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
 #pragma unroll
                         for (int t = 0; t < QS; t += G) {
                             const int it = t + grp;
-                            if (it < nitems) {
-                                const float* srcp = (first + it == 0) ? xs + (size_t)irow * F
-                                                                      : lw.partial + (size_t)(ilong + first + it - 1) * 128 + 4 * sub;
-                                cp_async16(dst + (uint32_t)(t * F * 4), srcp);
-                            }
+                            if (it < nitems)
+                                cp_async16(dst + (uint32_t)(t * F * 4), lw.partial + (size_t)(ilong + first + it) * 128 + 4 * sub);
                         }
                     } else {
 #pragma unroll
@@ -611,8 +617,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                             const int it = t + grp;
                             if (it < nitems) {
                                 const int k = kbase + it;
-                                uint32_t src = irow;
-                                if (first + it > 0) src = (uint32_t)((k < EMAX) ? icol[k] : __ldg(col + ielo + k));
+                                const uint32_t src = (uint32_t)((k < EMAX) ? icol[k] : __ldg(col + ielo + k));
                                 cp_async16(dst + (uint32_t)(t * F * 4), xs + (size_t)src * F);
                             }
                         }
@@ -631,7 +636,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
         int islot = 0, cslot = 0;
 #pragma unroll
         for (int d = 0; d < NQ - 1; ++d) { issue(islot); islot = (islot + 1) % NQ; }   // prologue: NQ-1 groups in flight
-        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f), self = acc;
+        float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
         float wsum = 0.f;
         int last_tl = -1;
         while (ci < stream_end) {
@@ -644,7 +649,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                 const int first = cb * QS;
                 const int nitems = citems - first;
                 const float* rs = ring_gen + cslot * SLOT_FLOATS;
-                const int kbase = ce0 + first - 1;
+                const int kbase = ce0 + first;
                 if (!(LONG && clong >= 0) && ce0 + cdeg <= EMAX) {       // whole row staged: batched LDS, predicated math
                     float4 v[QS / G];
                     float w[QS / G];
@@ -653,7 +658,6 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                         v[t / G] = *reinterpret_cast<const float4*>(rs + t * F);
                         w[t / G] = cew[kbase + t + grp];
                     }
-                    if (first == 0 && grp == 0) { self = v[0]; w[0] = 0.f; v[0] = make_float4(0.f, 0.f, 0.f, 0.f); }
 #pragma unroll
                     for (int t = 0; t < QS; t += G) {
                         if (t + grp < nitems) {
@@ -670,10 +674,8 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                         const int it = t + grp;
                         if (it < nitems) {
                             const float4 v = *reinterpret_cast<const float4*>(rs + t * F);
-                            if (t == 0 && first + it == 0) {
-                                self = v;
-                            } else if (LONG && clong >= 0) {             // chunk partial: already weighted
-                                wsum += lw.pw[clong + first + it - 1];
+                            if (LONG && clong >= 0) {                    // chunk partial: already weighted
+                                wsum += lw.pw[clong + first + it];
                                 acc.x += v.x; acc.y += v.y; acc.z += v.z; acc.w += v.w;
                             } else {
                                 const int k = kbase + it;
@@ -699,31 +701,25 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                     acc.x += __shfl_xor_sync(0xffffffffu, acc.x, o); acc.y += __shfl_xor_sync(0xffffffffu, acc.y, o);
                     acc.z += __shfl_xor_sync(0xffffffffu, acc.z, o); acc.w += __shfl_xor_sync(0xffffffffu, acc.w, o);
                     wsum += __shfl_xor_sync(0xffffffffu, wsum, o);
-                    self.x += __shfl_xor_sync(0xffffffffu, self.x, o); self.y += __shfl_xor_sync(0xffffffffu, self.y, o);
-                    self.z += __shfl_xor_sync(0xffffffffu, self.z, o); self.w += __shfl_xor_sync(0xffffffffu, self.w, o);
                 }
             }
             if (tl != last_tl) {                                         // first write of this warp into the stage
                 mbar_wait(empty_bar(s), ((uint32_t)(tl / C::STAGES) & 1u) ^ 1u);
                 last_tl = tl;
             }
-            if (cdeg >= 0) {
+            if (cdeg >= 0) {                                             // (no items: acc = wsum = 0, a zero mean)
                 const float inv = 1.0f / fmaxf(wsum, 1e-12f);
                 const float4 mean = make_float4(acc.x * inv, acc.y * inv, acc.z * inv, acc.w * inv);
                 if (lane < LPR) {
                     unsigned char* st = smem_gen + (size_t)s * C::STAGE_BYTES;
                     uint2 parts[NS];
-                    split4<NS>(self, parts);
-                    uint32_t off = sw128_offset<TN>(r, 4 * lane);
-#pragma unroll
-                    for (int p = 0; p < NS; ++p) *reinterpret_cast<uint2*>(st + p * C::PART_BYTES + off) = parts[p];
                     split4<NS>(mean, parts);
-                    off = sw128_offset<TN>(r, F + 4 * lane);
+                    const uint32_t off = sw128_offset<TN>(r, 4 * lane);
 #pragma unroll
                     for (int p = 0; p < NS; ++p) *reinterpret_cast<uint2*>(st + p * C::PART_BYTES + off) = parts[p];
                 }
                 fence_proxy_async();                                     // generic-proxy writes -> async proxy (wgmma)
-                acc = make_float4(0.f, 0.f, 0.f, 0.f); self = acc; wsum = 0.f;
+                acc = make_float4(0.f, 0.f, 0.f, 0.f); wsum = 0.f;
             }
             __syncwarp();
             if (lane == 0) {
@@ -792,6 +788,11 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
             if (lane == 0) {
                 *reinterpret_cast<int64_t*>(ib + EPAD * 8 + 384) = e_lo;
                 rp_s[96 + 2] = (int32_t)c_off; rp_s[96 + 3] = (int32_t)w_off;
+                if constexpr (C::SELF_SPLIT) {                           // the tile's self terms, read by the consumers
+                    const int64_t row0 = row_begin + tile * TN;
+                    const int64_t nr = row_end - row0 < TN ? row_end - row0 : TN;
+                    bulk_prefetch_l2(out + row0 * UM, (uint32_t)(nr * UM * 4));
+                }
             }
             __syncwarp();                                                // every lane's rowptr words are written ...
             if (lane == 0) {
@@ -819,7 +820,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
         // warpgroup, i < 16) is feature 64 h + 16 wq + 2 (i & 7) + (i >> 3): a thread's two rows are two CONSECUTIVE
         // features f0, f0 + 1, so its outputs are 8-byte stores and a warp writes 64 contiguous bytes of a row.  The
         // accumulator register d[4 nb + 2 b + e] of thread (wq, lane = 4 g + c) holds feature f0 + b of tile row
-        // 8 nb + 2 c + e.  The A fragments (W^T terms) come pre-split from `wsplit` (split_w_kernel), 16 bytes per
+        // 8 nb + 2 c + e.  The A fragments (W^T terms) come pre-split from `wsplit` (the prep kernel), 16 bytes per
         // thread, term and K step, from L2.  They are the same for every tile, so their loads run two K steps ahead of
         // the MMAs across tile boundaries: an L2 round trip under the gather's load is longer than one K step.
         const int h = warp >> 2, wq = warp & 3, et = tid & 127;
@@ -844,20 +845,41 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
         uint32_t a_n1[NS][4], a_n2[NS][4];                                    // fragments of the next two K steps
         load_a(0, a_n1);
         load_a(1, a_n2);
+        // F = 64 / 128: the accumulators start from the prep kernel's self terms (the first F/16 K steps), stored raw in
+        // out -- the local buffer: peers and the multicast address never hold this rank's self terms.  The epilogue of
+        // a tile already loads the next tile's into d when the loader has published that tile's id: the ids of a CTA's
+        // tiles increase, so a ring entry greater than the current tile is the next tile's, not a stale one.
+        float d[16];
+        int64_t s_tile = -1;                                                  // tile whose self terms d holds
+        auto self_terms = [&](int64_t t, int nb, int e) -> float2 {           // (row 8 nb + 2 c + e of tile t, f0)
+            const int64_t row = row_begin + t * TN + 8 * nb + 2 * c + e;
+            return row < row_end ? *reinterpret_cast<const float2*>(out + row * UM + f0) : make_float2(0.f, 0.f);
+        };
         for (int64_t tl = 0;; ++tl) {
             const int s = (int)(tl % C::STAGES);
             mbar_wait_relaxed(full_bar(s), (uint32_t)(tl / C::STAGES) & 1u);   // gather filled this stage
             const int64_t tile = tile_ids[tl % TILE_RING];
             if (tile < 0) break;                                              // closing entry: end of stream
             const uint32_t st0 = smem_base + (uint32_t)(s * C::STAGE_BYTES);
-            float d[16];
+            const int64_t row0 = row_begin + tile * TN;
+            if constexpr (C::SELF_SPLIT) {
+                if (tile != s_tile) {
+#pragma unroll
+                    for (int nb = 0; nb < 4; ++nb)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const float2 sv = self_terms(tile, nb, e);
+                            d[4 * nb + e] = sv.x; d[4 * nb + 2 + e] = sv.y;
+                        }
+                }
+            }
             auto mma_step = [&](int j, const uint32_t (&a)[NS][4]) {
                 const uint32_t boff = (uint32_t)((j >> 2) * (TN * 128) + (j & 3) * 32);
                 uint64_t xb[NS];
 #pragma unroll
                 for (int p = 0; p < NS; ++p) xb[p] = make_b_desc(st0 + (uint32_t)(p * C::PART_BYTES) + boff);   // x term p
                 wgmma_fence();
-                wgmma_rs(d, a[0], xb[0], j > 0 ? 1u : 0u);
+                wgmma_rs(d, a[0], xb[0], (C::SELF_SPLIT || j > 0) ? 1u : 0u);
                 wgmma_rs(d, a[0], xb[1], 1u);
                 wgmma_rs(d, a[1], xb[0], 1u);
                 if constexpr (NS == 3) {
@@ -882,13 +904,21 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
             if (lane == 0) mbar_arrive(empty_bar(s));                         // this warp's MMAs no longer read the stage
 
             // ---- epilogue: + bias, ReLU, one 8-byte store per (row, thread)
-            const int64_t row0 = row_begin + tile * TN;
+            s_tile = -1;
+            if constexpr (C::SELF_SPLIT) {
+                const int nx = tile_ids[(tl + 1) % TILE_RING];
+                if (nx > tile) s_tile = nx;
+            }
             float part[8];
 #pragma unroll
             for (int nb = 0; nb < 4; ++nb) {
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     float2 o = make_float2(d[4 * nb + e] + b2.x, d[4 * nb + 2 + e] + b2.y);
+                    if (C::SELF_SPLIT && s_tile >= 0) {
+                        const float2 sv = self_terms(s_tile, nb, e);
+                        d[4 * nb + e] = sv.x; d[4 * nb + 2 + e] = sv.y;
+                    }
                     if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
                     part[2 * nb + e] = o.x * nw2.x + o.y * nw2.y;
                     const int64_t row = row0 + 8 * nb + 2 * c + e;
@@ -932,16 +962,12 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
     }
 }
 
-// W [K][128] fp32 -> the consumer warpgroups' A fragments, split into NS bf16 terms:
-// wsplit[((2 j + h) NS + p) 128 + t] = uint4 of term p of thread t of warpgroup h at K step j (see the consumer role)
+// W [K][128] fp32 -> the A fragment of thread t of consumer warpgroup h at K step j (W rows 16 j .. 16 j + 15), split
+// into NS bf16 terms
 template <int NS>
-__global__ void __launch_bounds__(256) split_w_kernel(const float* __restrict__ W, int ksteps, uint4* __restrict__ wsplit) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;               // (j, h, t)
-    if (i >= ksteps * 2 * 128) return;
-    const int t = i & 127, h = (i >> 7) & 1, j = i >> 8;
+__device__ __forceinline__ void w_fragment(const float* __restrict__ W, int j, int h, int t, uint32_t (&a)[NS][4]) {
     const int wq = t >> 5, g = (t & 31) >> 2, c = t & 3;
     const int f0 = 64 * h + 16 * wq + 2 * g;
-    uint32_t a[NS][4];
 #pragma unroll
     for (int r = 0; r < 4; ++r) {                                     // register r: row g + 8 (r & 1), K pair r >> 1
         const int k = 16 * j + 2 * c + 8 * (r >> 1), f = f0 + (r & 1);
@@ -950,8 +976,138 @@ __global__ void __launch_bounds__(256) split_w_kernel(const float* __restrict__ 
 #pragma unroll
         for (int p = 0; p < NS; ++p) a[p][r] = pp[p];
     }
+}
+// layout the consumer role reads: wsplit[((2 j + h) NS + p) 128 + t] = uint4 of term p of thread t of warpgroup h at
+// the layer kernel's K step j
+template <int NS>
+__device__ __forceinline__ void store_w_fragment(uint4* __restrict__ wsplit, int j, int h, int t, const uint32_t (&a)[NS][4]) {
 #pragma unroll
     for (int p = 0; p < NS; ++p) wsplit[(size_t)((2 * j + h) * NS + p) * 128 + t] = make_uint4(a[p][0], a[p][1], a[p][2], a[p][3]);
+}
+
+// F = 32: all 2F/16 K steps of W, one fragment per thread
+template <int NS>
+__global__ void __launch_bounds__(256) split_w_kernel(const float* __restrict__ W, int ksteps, uint4* __restrict__ wsplit) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;               // (j, h, t)
+    if (i >= ksteps * 2 * 128) return;
+    const int t = i & 127, h = (i >> 7) & 1, j = i >> 8;
+    uint32_t a[NS][4];
+    w_fragment<NS>(W, j, h, t, a);
+    store_w_fragment<NS>(wsplit, j, h, t, a);
+}
+
+// F = 64 / 128: the prep kernel of a layer launch.  Two jobs:
+//  - the split fragments of the MEAN half of W (rows F .. 2F-1, K steps F/16 .. 2F/16-1) into wsplit, as the layer
+//    kernel's K steps 0 .. F/16-1;
+//  - the SELF half of the GEMM, S[v] = x_v . W[0:F] for v in [row_begin, row_end), written raw (no bias, no ReLU) into
+//    out[v, :] with the consumer role's accumulator -> (row, feature) mapping.  The layer kernel loads S into its
+//    accumulators and continues with the mean K steps.
+// The self product runs exactly the wgmma sequence the fused [x_v || m_v] tile would have run for its first F/16 K steps
+// (same split_pair terms, same m64n32k16 instructions in the same product order, scale-d 0 first), and between wgmma
+// instructions the accumulator is plain fp32 in registers, so the layer's outputs are the bits of the fused K = 2F GEMM.
+// Two consumer-shaped warpgroups; the self half of W stays in registers for the whole launch (96 registers per thread at
+// F = 128 / NS = 3), so W is read from L2 once per CTA; x arrives in 64-row tiles (two 32-row slices sharing each A
+// fragment), the next tile's rows loaded into registers while the current tile's MMAs run.  (A 3- or 4-deep cp.async
+// ring of fp32 tiles, a double-buffered bf16 operand, and a second accumulator set storing tile t-1 under tile t's MMAs
+// all measured no faster: the kernel moves 1 GB at F = 128.)
+constexpr int PREP_ROWS = 64;
+template <int F, int NS>
+struct PrepCfg {
+    static constexpr int KS = F / 16;                         // self K steps (= the mean half's)
+    static constexpr int PART_BYTES = (F / 64) * TN * 128;    // one bf16 term of one 32-row slice
+    static constexpr int SLICE_BYTES = NS * PART_BYTES;
+    static constexpr int SLICES = PREP_ROWS / TN;
+    static constexpr int SMEM = SLICES * SLICE_BYTES + 1024 /*align*/;
+};
+
+template <int F, int NS>
+__global__ void __launch_bounds__(256, 1)
+sage_self_prep_kernel(const float* __restrict__ x, const float* __restrict__ W, float* __restrict__ out, int64_t row_begin,
+                      int64_t row_end, uint4* __restrict__ wsplit) {
+    using P = PrepCfg<F, NS>;
+    constexpr int KS = P::KS, SLICES = P::SLICES;
+    constexpr int LPR = F / 4;                                // float4 per x row
+    constexpr int RPP = 256 / LPR;                            // rows per pass of the CTA
+    constexpr int NV = PREP_ROWS / RPP;                       // float4 per thread and tile
+    extern __shared__ unsigned char smem_dyn[];
+    const uint32_t base = (smem_u32(smem_dyn) + 1023u) & ~1023u;         // SWIZZLE_128B needs 1024-B alignment
+    unsigned char* gen = smem_dyn + (base - smem_u32(smem_dyn));
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int h = warp >> 2, wq = warp & 3, et = tid & 127;
+    const int g = lane >> 2, c = lane & 3;
+    const int f0 = 64 * h + 16 * wq + 2 * g;
+
+    for (int j = blockIdx.x; j < KS; j += gridDim.x) {
+        uint32_t a[NS][4];
+        w_fragment<NS>(W, KS + j, h, et, a);
+        store_w_fragment<NS>(wsplit, j, h, et, a);
+    }
+    uint32_t a[KS][NS][4];
+#pragma unroll
+    for (int j = 0; j < KS; ++j) w_fragment<NS>(W, j, h, et, a[j]);
+
+    const int q = tid % LPR, r0 = tid / LPR;
+    const int64_t n_tiles = (row_end - row_begin + PREP_ROWS - 1) / PREP_ROWS;
+    float4 v[NV];
+    auto load = [&](int64_t tile) {
+#pragma unroll
+        for (int i = 0; i < NV; ++i) {
+            const int64_t row = row_begin + tile * PREP_ROWS + r0 + RPP * i;
+            v[i] = (tile < n_tiles && row < row_end) ? __ldg(reinterpret_cast<const float4*>(x + row * F) + q)
+                                                      : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+    };
+    load(blockIdx.x);
+    for (int64_t tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        __syncthreads();                                      // both warpgroups' MMAs of the last tile have retired
+#pragma unroll
+        for (int i = 0; i < NV; ++i) {                        // bf16 terms into the swizzled K-major slices
+            const int r = r0 + RPP * i;
+            uint2 parts[NS];
+            split4<NS>(v[i], parts);
+            const uint32_t off = (uint32_t)((r / TN) * P::SLICE_BYTES) + sw128_offset<TN>(r % TN, 4 * q);
+#pragma unroll
+            for (int p = 0; p < NS; ++p) *reinterpret_cast<uint2*>(gen + p * P::PART_BYTES + off) = parts[p];
+        }
+        fence_proxy_async();                                  // generic-proxy writes -> async proxy (wgmma)
+        __syncthreads();
+        load(tile + gridDim.x);                               // in flight under the MMAs and the stores
+
+        float d[SLICES][16];
+        wgmma_fence();
+#pragma unroll
+        for (int j = 0; j < KS; ++j) {
+            const uint32_t boff = (uint32_t)((j >> 2) * (TN * 128) + (j & 3) * 32);
+#pragma unroll
+            for (int sl = 0; sl < SLICES; ++sl) {
+                uint64_t xb[NS];
+#pragma unroll
+                for (int p = 0; p < NS; ++p) xb[p] = make_b_desc(base + (uint32_t)(sl * P::SLICE_BYTES + p * P::PART_BYTES) + boff);
+                wgmma_rs(d[sl], a[j][0], xb[0], j > 0 ? 1u : 0u);
+                wgmma_rs(d[sl], a[j][0], xb[1], 1u);
+                wgmma_rs(d[sl], a[j][1], xb[0], 1u);
+                if constexpr (NS == 3) {
+                    wgmma_rs(d[sl], a[j][1], xb[1], 1u);
+                    wgmma_rs(d[sl], a[j][0], xb[2], 1u);
+                    wgmma_rs(d[sl], a[j][2], xb[0], 1u);
+                }
+            }
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+
+        const int64_t row0 = row_begin + tile * PREP_ROWS;
+#pragma unroll
+        for (int sl = 0; sl < SLICES; ++sl)
+#pragma unroll
+            for (int nb = 0; nb < 4; ++nb)
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    const int64_t row = row0 + TN * sl + 8 * nb + 2 * c + e;
+                    if (row < row_end)
+                        *reinterpret_cast<float2*>(out + row * UM + f0) = make_float2(d[sl][4 * nb + e], d[sl][4 * nb + 2 + e]);
+                }
+    }
 }
 
 // per-device ring of launch-private tile counters (1 KB, allocated on first use and kept): a launch zeroes its slot on its
@@ -1011,11 +1167,20 @@ int launch_umma(const float* x, const RP* rowptr, const int32_t* col, const floa
     const int64_t grid = tiles < sm_count() ? tiles : sm_count();
     unsigned* tile_ctr = tile_counter_slot(st);
     if (!tile_ctr) { set_error("could not allocate the tile counter"); return NERRF_ERR_CUDA; }
-    // W^T split into bf16 terms in fragment order, once per launch (the weights may have changed in place since the last one)
+    // W^T split into bf16 terms in fragment order, once per launch (the weights may have changed in place since the last
+    // one); at F = 64 / 128 by the prep kernel, which also writes the self terms into out
     static_assert((size_t)C::KSTEPS * 2 * NS * 128 * sizeof(uint4) <= WSPLIT_MAX_BYTES, "split W scratch");
     uint4* wsplit = wsplit_buffer(st);
     if (!wsplit) { set_error("could not allocate the split-weight scratch"); return NERRF_ERR_CUDA; }
-    split_w_kernel<NS><<<(C::KSTEPS * 2 * 128 + 255) / 256, 256, 0, st>>>(W, C::KSTEPS, wsplit);
+    if constexpr (C::SELF_SPLIT) {
+        using P = PrepCfg<F, NS>;
+        rc = set_max_dynamic_smem((const void*)sage_self_prep_kernel<F, NS>, P::SMEM);
+        if (rc) return rc;
+        const int64_t ptiles = (rows + PREP_ROWS - 1) / PREP_ROWS;
+        sage_self_prep_kernel<F, NS><<<(unsigned)(ptiles < sm_count() ? ptiles : sm_count()), 256, P::SMEM, st>>>(x, W, out, row_begin, row_end, wsplit);
+    } else {
+        split_w_kernel<NS><<<(C::KSTEPS * 2 * 128 + 255) / 256, 256, 0, st>>>(W, C::KSTEPS, wsplit);
+    }
     // the col / ew slices are staged with bulk copies, which only need 4-byte aligned slices (the aligned superset is copied)
     if (lw.cap > 0)
         sage_layer_umma_kernel<F, NS, RP, true><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit);
