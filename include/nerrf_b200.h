@@ -228,6 +228,31 @@ int nerrf_lstm_forward(const float* seq, const int32_t* len, int64_t B, int T, i
                        float* out, void* workspace, size_t workspace_bytes,
                        nerrf_stream_t stream);
 
+/* ------------------------------------------------------------------ BiLSTM training (forward with saved activations +
+ * backward-through-time; the BiLSTM half of ai/train.py "joint GNN+LSTM training script", README.md:75)
+ * nerrf_lstm_forward_train runs the fp32 CUDA-core recurrence of nerrf_lstm_forward (same arguments, same pre-transposed
+ * weights, no head) and writes the top layer's final states hfin_out [B,2H] = [h_fwd_final || h_bwd_final] -- the
+ * head's input -- plus a tape of every layer's output, gates and cell states (tape_bytes from
+ * nerrf_lstm_train_workspace_bytes).  nerrf_lstm_backward differentiates sum(dhfin * hfin) through that tape:
+ *     per step, in reverse direction order:  dc += dh*o*(1 - tanh^2 c);  pre-activation gate gradients dg from the saved
+ *     gates and c_{t-1};  dh_{t-1} = dg W_hh + d out_l[t-1];  dc_{t-1} = dc*f   (padded steps pass dh, dc through)
+ *     dW_ih = dg^T in_l,  dW_hh = dg^T h_{t-1},  db = sum dg,  d in_l = [dg_fwd || dg_bwd] [W_ih_fwd ; W_ih_bwd]
+ * W_ih[2l+d] [4H,D_l], W_hh[2l+d] [4H,H] are in torch's layout (NOT transposed), and so are the gradients it writes:
+ * dW_ih[2l+d], dW_hh[2l+d], db[2l+d] [4H] (db is the gradient of both b_ih and b_hh).  dseq [B,T,D_in] == NULL skips
+ * the input gradient; it is exactly 0 at padded steps.  The backward overwrites the tape's gates, so a tape is
+ * differentiated once.  fp32, no atomics: bit-reproducible.  H must be 256; all pointers device (the pointer arrays are
+ * host arrays of 2*num_layers device pointers), tape and workspace 16-byte aligned.  Asynchronous on `stream`. */
+int nerrf_lstm_train_workspace_bytes(int64_t B, int T, int D_in, int H, int num_layers, size_t* tape_bytes,
+                                     size_t* workspace_bytes);
+int nerrf_lstm_forward_train(const float* seq, const int32_t* len, int64_t B, int T, int D_in, int H,
+                             int num_layers, const float* const* Wih_t, const float* const* Whh_t,
+                             const float* const* bias, float* hfin_out, void* tape, size_t tape_bytes,
+                             nerrf_stream_t stream);
+int nerrf_lstm_backward(const float* seq, const int32_t* len, int64_t B, int T, int D_in, int H, int num_layers,
+                        const float* const* W_ih, const float* const* W_hh, void* tape, size_t tape_bytes,
+                        const float* dhfin, float* dseq, float* const* dW_ih, float* const* dW_hh, float* const* db,
+                        void* workspace, size_t workspace_bytes, nerrf_stream_t stream);
+
 /* ------------------------------------------------------------------ temporal-graph constructor, device half
  * (SURVEY.md 8f rank 1 -- the step immediately before GraphSAGE_T.forward)
  * Replaces: the graph-constructor stage the reference documents but does not ship

@@ -60,6 +60,13 @@ SIGNATURES = {
     "nerrf_lstm_workspace_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "nerrf_lstm_forward": (C.c_int, [vp, vp, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp),
                                      C.POINTER(vp), C.POINTER(vp), vp, vp, vp, vp, C.c_size_t, vp]),
+    "nerrf_lstm_train_workspace_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t),
+                                                   C.POINTER(C.c_size_t)]),
+    "nerrf_lstm_forward_train": (C.c_int, [vp, vp, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp),
+                                           C.POINTER(vp), C.POINTER(vp), vp, vp, C.c_size_t, vp]),
+    "nerrf_lstm_backward": (C.c_int, [vp, vp, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp), C.POINTER(vp),
+                                      vp, C.c_size_t, vp, vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), vp, C.c_size_t,
+                                      vp]),
     "nerrf_graph_csr_workspace_bytes": (C.c_int, [C.c_int64, C.c_int64, C.POINTER(C.c_int64)]),
     "nerrf_graph_build_csr_ex": (C.c_int, [vp, vp, vp, vp, C.c_int64, C.c_int64, C.c_float, C.c_float, vp, C.c_int,
                                            vp, vp, vp, vp, C.c_int64, vp]),

@@ -8,8 +8,10 @@ Training is NOT the north-star hot path (that is inference: GraphSAGE_T.forward,
 rewards.score -- CUDA only).  With `--device cuda` the GraphSAGE-T half trains through the library's own kernels: the
 fused wgmma layer forward and the hand-written backward (`nerrf_sage_layer_bwd`, csrc/sage_bwd.cu) behind a
 torch.autograd.Function (nerrf_b200.ai.autograd); on the CPU it differentiates a plain-torch statement of the same frozen
-spec (also the thing the CUDA gradients are tested against).  The BiLSTM half is torch.nn.LSTM under autograd on either
-device.  Both update the very nn.Parameters the CUDA inference kernels read (GraphSAGE_T.weights / biases / node_w /
+spec (also the thing the CUDA gradients are tested against).  The BiLSTM half is torch.nn.LSTM under autograd by default;
+with `lstm_backward="library"` (`--lstm-backward library`) on a CUDA device it trains through the library's own kernels
+instead: the fp32 recurrence saving its activations (`nerrf_lstm_forward_train`) and the backward-through-time of
+csrc/lstm_bwd.cu (`nerrf_lstm_backward`), behind nerrf_b200.ai.autograd.LSTMFn.  Both update the very nn.Parameters the CUDA inference kernels read (GraphSAGE_T.weights / biases / node_w /
 node_b; LSTMScorer.lstm / head).  Inference never calls anything in this file, and nothing here is a fallback for it:
 GraphSAGE_T.forward / LSTMScorer.forward still refuse CPU tensors.
 
@@ -129,10 +131,20 @@ def _to(ex, device):
     return {k: (v.to(device) if torch.is_tensor(v) else v) for k, v in ex.items()}
 
 
+LSTM_BACKWARDS = ("torch", "library")
+
+
 def train(model: GraphSAGE_T, scorer: LSTMScorer | None, examples, epochs: int = 150, lr: float = 3e-3, device="cpu",
-          log=None):
-    """Joint loss = BCE(node logits over file nodes) + BCE(LSTM encrypt_probability logit); Adam; full batch per trace."""
+          log=None, lstm_backward: str = "torch"):
+    """Joint loss = BCE(node logits over file nodes) + BCE(LSTM encrypt_probability logit); Adam; full batch per trace.
+    lstm_backward: "torch" differentiates torch.nn.LSTM (cuDNN on a GPU); "library" runs the BiLSTM forward and
+    backward on this library's kernels (nerrf_b200.ai.autograd.lstm_logits) when `device` is a CUDA device."""
+    if lstm_backward not in LSTM_BACKWARDS:
+        raise ValueError(f"lstm_backward must be one of {LSTM_BACKWARDS}, got {lstm_backward!r}")
     device = torch.device(device)
+    library_lstm = lstm_backward == "library" and device.type == "cuda"
+    if library_lstm:
+        from . import autograd as AG
     model.to(device)
     params = list(model.parameters())
     if scorer is not None:
@@ -150,7 +162,10 @@ def train(model: GraphSAGE_T, scorer: LSTMScorer | None, examples, epochs: int =
             pos = ex["label"][m].sum().clamp_min(1.0)
             loss = bce(logit[m], ex["label"][m], pos_weight=((m.sum() - pos) / pos).clamp(0.2, 5.0))
             if scorer is not None and ex["seq"].shape[0]:
-                sl = lstm_logits(scorer, ex["seq"], ex["lengths"])
+                if library_lstm:
+                    sl = AG.lstm_logits(scorer, ex["seq"], ex["lengths"])
+                else:
+                    sl = lstm_logits(scorer, ex["seq"], ex["lengths"])
                 loss = loss + bce(sl[:, 0], ex["seq_label"]) + 0.5 * bce(sl[:, 1], ex["seq_label"])
             loss.backward()
             opt.step()
@@ -185,11 +200,13 @@ def main(argv=None):
     ap.add_argument("--layers", type=int, default=2); ap.add_argument("--lr", type=float, default=3e-3)
     ap.add_argument("--device", default="cpu"); ap.add_argument("--out", default=None)
     ap.add_argument("--no-lstm", action="store_true")
+    ap.add_argument("--lstm-backward", choices=LSTM_BACKWARDS, default="torch",
+                    help="BiLSTM training path on a CUDA device: torch.nn.LSTM under autograd, or the library's kernels")
     a = ap.parse_args(argv)
     train_set = toy_set(range(100, 100 + a.traces)); test_set = toy_set(range(900, 903))
     model = GraphSAGE_T(G.F_IN, 128, a.layers); scorer = None if a.no_lstm else LSTMScorer()
     print("before:", evaluate(model, scorer, test_set, a.device))
-    train(model, scorer, train_set, a.epochs, a.lr, a.device, log=print)
+    train(model, scorer, train_set, a.epochs, a.lr, a.device, log=print, lstm_backward=a.lstm_backward)
     print("held-out:", evaluate(model, scorer, test_set, a.device))
     if a.out:
         torch.save({"sage": model.state_dict(), "lstm": None if scorer is None else scorer.state_dict(),

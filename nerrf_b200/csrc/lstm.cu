@@ -7,7 +7,13 @@
 // registers, h lives in shared memory).  Weights are pre-transposed ([K, 4H]) so the 256
 // threads read 1 KB contiguous per (k, gate); they stream from L2 every step (8.2 MB of
 // weights is L2-resident, too big for one SM's shared memory).
+//
+// SAVE = true is the training forward (nerrf_lstm_forward_train): the same arithmetic, and at every valid step it also
+// stores the post-activation gates and the cell state into the tape that csrc/lstm_bwd.cu differentiates.  `out` is then
+// a layer of that tape (lstm_tape.cuh), whose gates and cells follow the output at fixed offsets, so the kernel keeps
+// one signature and the inference instantiation (SAVE = false) compiles exactly as it did before the flag existed.
 #include "common.cuh"
+#include "lstm_tape.cuh"
 
 namespace nerrf {
 
@@ -22,7 +28,7 @@ constexpr int LH = 256;       // hidden size (threads per CTA)
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
 
-template <int BS>
+template <int BS, bool SAVE>
 __global__ void __launch_bounds__(LH, 1)
 lstm_layer_kernel(const float* __restrict__ in, int in_stride_b, int in_stride_t, int D,   // in[b*in_stride_b + t*in_stride_t + k]
                   const int32_t* __restrict__ len, int64_t B, int T,
@@ -112,6 +118,12 @@ lstm_layer_kernel(const float* __restrict__ in, int in_stride_b, int in_stride_t
                 c[b] = fg * c[b] + ig * gg;
                 hval = og * tanhf(c[b]);
                 oval = hval;
+                if constexpr (SAVE) {       // out is a layer of the training tape: its gates and cells follow it
+                    const int64_t bt = B * (int64_t)T, row = dir * bt + (b0 + b) * (int64_t)T + t;
+                    float* gs = out + bt * (2 * LH) + row * (4 * LH) + j;
+                    gs[0] = ig; gs[LH] = fg; gs[2 * LH] = gg; gs[3 * LH] = og;
+                    out[bt * (2 * LH + 2 * 4 * LH) + row * LH + j] = c[b];
+                }
             }
             hn[j * BS + b] = hval;
             if (out && b0 + b < B) out[((b0 + b) * (int64_t)T + t) * (2 * LH) + dir * LH + j] = oval;
@@ -144,16 +156,17 @@ __global__ void __launch_bounds__(256) lstm_head_kernel(const float* __restrict_
     }
 }
 
-template <int BS>
+template <int BS, bool SAVE>
 static int launch_lstm_layer(const float* in, int sb, int stt, int D, const int32_t* len, int64_t B, int T,
                              const float* Wih_f, const float* Whh_f, const float* bias_f, const float* Wih_b,
                              const float* Whh_b, const float* bias_b, float* out, float* hfin, cudaStream_t st) {
     const size_t smem = (size_t)(2 * LH * BS + (size_t)D * BS) * sizeof(float);
     NERRF_REQUIRE(smem <= 200 * 1024, "LSTM input width %d too large for shared memory", D);
-    const int rc = set_max_dynamic_smem((const void*)lstm_layer_kernel<BS>, smem);
+    const int rc = set_max_dynamic_smem((const void*)lstm_layer_kernel<BS, SAVE>, smem);
     if (rc) return rc;
     dim3 grid((unsigned)((B + BS - 1) / BS), 2);
-    lstm_layer_kernel<BS><<<grid, LH, smem, st>>>(in, sb, stt, D, len, B, T, Wih_f, Whh_f, bias_f, Wih_b, Whh_b, bias_b, out, hfin);
+    lstm_layer_kernel<BS, SAVE><<<grid, LH, smem, st>>>(in, sb, stt, D, len, B, T, Wih_f, Whh_f, bias_f, Wih_b, Whh_b, bias_b,
+                                                        out, hfin);
     return launch_status("lstm_layer_kernel");
 }
 
@@ -202,11 +215,39 @@ extern "C" int nerrf_lstm_forward(const float* seq, const int32_t* len, int64_t 
     int sb = T * D_in, stt = D_in, D = D_in;
     for (int l = 0; l < num_layers; ++l) {
         float* o = (l == num_layers - 1) ? nullptr : ((l & 1) ? buf1 : buf0);
-        rc = launch_lstm_layer<8>(in, sb, stt, D, len, B, T, Wih_t[2 * l], Whh_t[2 * l], bias[2 * l], Wih_t[2 * l + 1],
-                                  Whh_t[2 * l + 1], bias[2 * l + 1], o, hfin, st);
+        rc = launch_lstm_layer<8, false>(in, sb, stt, D, len, B, T, Wih_t[2 * l], Whh_t[2 * l], bias[2 * l], Wih_t[2 * l + 1],
+                                         Whh_t[2 * l + 1], bias[2 * l + 1], o, hfin, st);
         if (rc) return rc;
         in = o; sb = T * 2 * H; stt = 2 * H; D = 2 * H;
     }
     lstm_head_kernel<<<(unsigned)((B + 7) / 8), 256, 0, st>>>(hfin, head_W, head_b, out, B, 2 * H);
     return launch_status("lstm_head_kernel");
+}
+
+extern "C" int nerrf_lstm_forward_train(const float* seq, const int32_t* len, int64_t B, int T, int D_in, int H,
+                                        int num_layers, const float* const* Wih_t, const float* const* Whh_t,
+                                        const float* const* bias, float* hfin_out, void* tape, size_t tape_bytes,
+                                        nerrf_stream_t stream) {
+    size_t need = 0, ws = 0;
+    int rc = nerrf_lstm_train_workspace_bytes(B, T, D_in, H, num_layers, &need, &ws);
+    if (rc) return rc;
+    NERRF_REQUIRE(seq && len && Wih_t && Whh_t && bias && hfin_out && tape, "null pointer");
+    NERRF_REQUIRE(((uintptr_t)tape & 15) == 0, "tape must be 16-byte aligned");
+    if (tape_bytes < need) {
+        set_error("lstm tape too small: need %zu bytes, got %zu", need, tape_bytes);
+        return NERRF_ERR_WORKSPACE;
+    }
+    for (int i = 0; i < 2 * num_layers; ++i) NERRF_REQUIRE(Wih_t[i] && Whh_t[i] && bias[i], "null weight pointer");
+    if (B == 0) return NERRF_OK;
+    const LstmTape tp(B, T);
+    const float* in = seq;
+    int sb = T * D_in, stt = D_in, D = D_in;
+    for (int l = 0; l < num_layers; ++l) {
+        float* o = tp.out((float*)tape, l);
+        rc = launch_lstm_layer<8, true>(in, sb, stt, D, len, B, T, Wih_t[2 * l], Whh_t[2 * l], bias[2 * l], Wih_t[2 * l + 1],
+                                        Whh_t[2 * l + 1], bias[2 * l + 1], o, hfin_out, (cudaStream_t)stream);
+        if (rc) return rc;
+        in = o; sb = T * 2 * H; stt = 2 * H; D = 2 * H;
+    }
+    return NERRF_OK;
 }
