@@ -82,6 +82,14 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 __device__ __forceinline__ void fence_proxy_async_all() { asm volatile("fence.proxy.async;" ::: "memory"); }
 __device__ __forceinline__ void named_bar(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
+// ---------------------------------------------------------------- register reallocation
+// setmaxnreg: sets the per-thread register count of the executing warpgroup (all four warps execute it).  dec returns
+// registers to the CTA's pool; inc waits until the pool holds enough.  N is a multiple of 8 in [24, 256].
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N) : "memory"); }
+
 // ---------------------------------------------------------------- wgmma
 // shared-memory matrix descriptor (sm_90): K-major, SWIZZLE_128B, 8-row groups 1024 B apart (SBO); the leading byte
 // offset is unused for swizzled K-major operands.  A K step inside the 128-byte swizzle atom advances the start address
