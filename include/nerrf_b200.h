@@ -135,6 +135,24 @@ int nerrf_sage_layer_bwd(const float* h_in, const float* m, const float* y, cons
                          float* dh, float* dW, float* db, float* workspace, size_t workspace_bytes,
                          int64_t n_nodes, int F, int H, int relu, nerrf_stream_t stream);
 
+/* Edge head backward (training the attack / normal edge classifier).  Forward = nerrf_sage_node_head (proj) +
+ * nerrf_sage_edge_head.  Given d_logit [E,2] = d loss / d edge_logit in CSR-by-destination order:
+ *     g_src[v] = sum_{e: src(e)=v} d_logit[e],   g_dst[v] = sum_{e: dst(e)=v} d_logit[e]
+ *     dh[v] = g_src[v] We[0:H]^T + g_dst[v] We[H:2H]^T    ([n,H])
+ *     d_edge_W = [h^T g_src ; h^T g_dst]  ([2H,2]),   d_edge_b = sum_v g_dst[v]  ([2])
+ * t_rowptr [n+1] / t_eid [E] is the transposed graph (CSR by source): t_eid[j] = CSR-by-destination position of the j-th
+ * out-edge; both int32, or int64 when t_is64.  dh == NULL skips the input gradient, d_edge_W == NULL skips the weight and
+ * bias gradients (and the workspace).  H must be 128; h, edge_W, d_logit, dh, d_edge_W and workspace 16-byte aligned;
+ * workspace from nerrf_sage_edge_head_bwd_workspace_bytes.  fp32, no atomics, chunking a function of n_nodes only:
+ * bit-reproducible. */
+int nerrf_sage_edge_head_bwd_workspace_bytes(int64_t n_nodes, int H, size_t* bytes);
+int nerrf_sage_edge_head_bwd(const float* h, const float* edge_W, const float* d_logit,
+                             const void* rowptr, int rowptr_is64,
+                             const void* t_rowptr, const void* t_eid, int t_is64,
+                             float* dh, float* d_edge_W, float* d_edge_b,
+                             void* workspace, size_t workspace_bytes,
+                             int64_t n_nodes, int H, nerrf_stream_t stream);
+
 /* Host-buffer session (the e2e call): device buffers live in the handle. */
 typedef struct nerrf_sage_session nerrf_sage_session;
 int nerrf_sage_session_create(int64_t max_nodes, int64_t max_edges, int f_in, int hidden,

@@ -6,7 +6,9 @@ named, never written).  Forward = the fused tensor-core (wgmma) layer kernel the
 backward = `nerrf_sage_layer_bwd` (csrc/sage_bwd.cu): dP = dy*[y>0], dW = [h||m]^T dP, db, dZ = dP W^T,
 dh = dZ[:, :F] + A^T dZ[:, F:], the last as a gather over the transposed graph.  The BiLSTM: forward =
 `nerrf_lstm_forward_train` (the fp32 CUDA-core recurrence, saving its activations to a tape), backward =
-`nerrf_lstm_backward` (csrc/lstm_bwd.cu, backward-through-time).  CUDA tensors only; no CPU fallback (ai/train.py keeps
+`nerrf_lstm_backward` (csrc/lstm_bwd.cu, backward-through-time).  The attack / normal edge head: forward =
+`nerrf_sage_node_head` (proj) + `nerrf_sage_edge_head`, backward = `nerrf_sage_edge_head_bwd` (csrc/sage_edge_bwd.cu: row
+sums of dL over the CSR and its transpose, then dh, dWe, dbe).  CUDA tensors only; no CPU fallback (ai/train.py keeps
 its plain-torch restatements for CPU runs and as the thing the gradients are checked against).
 """
 from __future__ import annotations
@@ -39,7 +41,8 @@ class TrainGraph:
         self.t_rowptr = t_rowptr.to(rowptr.dtype).contiguous()
         self.t_col = dst[order].to(torch.int32).contiguous()
         self.t_w = a[order].contiguous()
-        self._ws = None
+        self.t_eid = order.to(rowptr.dtype).contiguous()         # CSR position of each out-edge (edge head backward)
+        self._ws = self._edge_ws = None
 
     def workspace(self, F: int):
         need = C.c_size_t()
@@ -47,6 +50,13 @@ class TrainGraph:
         if self._ws is None or self._ws.numel() * 4 < need.value:
             self._ws = torch.empty((need.value + 3) // 4, dtype=torch.float32, device=self.rowptr.device)
         return self._ws
+
+    def edge_workspace(self, H: int):
+        need = C.c_size_t()
+        L.check(L.lib().nerrf_sage_edge_head_bwd_workspace_bytes(self.n, H, C.byref(need)), "edge_head_bwd_workspace_bytes")
+        if self._edge_ws is None or self._edge_ws.numel() * 4 < need.value:
+            self._edge_ws = torch.empty((need.value + 3) // 4, dtype=torch.float32, device=self.rowptr.device)
+        return self._edge_ws
 
 
 def aggregate(h, tg: TrainGraph):
@@ -98,6 +108,60 @@ def sage_node_logits(model, x, tg: TrainGraph):
     for l, (W, b) in enumerate(zip(model.weights, model.biases)):
         h = SageLayerFn.apply(h, W, b, tg, model, l)
     return h @ model.node_w + model.node_b
+
+
+class EdgeHeadFn(torch.autograd.Function):
+    """edge_logit [E, 2] = [h_src || h_dst] We + be (CSR order) -- forward = `nerrf_sage_node_head` (its proj output) +
+    `nerrf_sage_edge_head`, backward = `nerrf_sage_edge_head_bwd` (csrc/sage_edge_bwd.cu)."""
+
+    @staticmethod
+    def forward(ctx, h, edge_W, edge_b, tg: TrainGraph, model):
+        h = h.contiguous()
+        We = edge_W.detach().contiguous()
+        n = h.shape[0]
+        score = torch.empty(n, device=h.device, dtype=torch.float32)       # the node head's output, not used here
+        proj = torch.empty(n, 4, device=h.device, dtype=torch.float32)
+        el = torch.empty(tg.col.numel(), 2, device=h.device, dtype=torch.float32)
+        with torch.cuda.device(h.device):
+            L.check(L.lib().nerrf_sage_node_head(L.ptr(h), L.ptr(model.node_w), 0.0, L.ptr(score), L.ptr(We), L.ptr(proj), 0,
+                                                 n, h.shape[1], L.current_stream_ptr()), "nerrf_sage_node_head")
+            L.check(L.lib().nerrf_sage_edge_head(L.ptr(proj), L.ptr(tg.rowptr), int(tg.rowptr.dtype == torch.int64),
+                                                 L.ptr(tg.col), L.ptr(edge_b.detach().contiguous()), L.ptr(el), 0, n,
+                                                 L.current_stream_ptr()), "nerrf_sage_edge_head")
+        ctx.save_for_backward(h, We)
+        ctx.tg = tg
+        return el
+
+    @staticmethod
+    def backward(ctx, dlogit):
+        h, We = ctx.saved_tensors
+        tg = ctx.tg
+        dlogit = dlogit.contiguous()
+        need_w = ctx.needs_input_grad[1] or ctx.needs_input_grad[2]
+        dh = torch.empty_like(h) if ctx.needs_input_grad[0] else None
+        dW = torch.empty_like(We) if need_w else None
+        db = torch.empty(2, device=h.device, dtype=torch.float32) if need_w else None
+        ws = tg.edge_workspace(h.shape[1]) if need_w else None
+        with torch.cuda.device(h.device):
+            L.check(L.lib().nerrf_sage_edge_head_bwd(L.ptr(h), L.ptr(We), L.ptr(dlogit), L.ptr(tg.rowptr),
+                                                     int(tg.rowptr.dtype == torch.int64), L.ptr(tg.t_rowptr), L.ptr(tg.t_eid),
+                                                     int(tg.t_rowptr.dtype == torch.int64), L.ptr(dh), L.ptr(dW), L.ptr(db),
+                                                     L.ptr(ws), 0 if ws is None else ws.numel() * 4, tg.n, h.shape[1],
+                                                     L.current_stream_ptr()), "nerrf_sage_edge_head_bwd")
+        return dh, dW, db, None, None
+
+
+def sage_logits(model, x, tg: TrainGraph):
+    """(node logits [N], edge logits [E, 2]) with gradients: the fused layers through SageLayerFn, the node head as in
+    sage_node_logits, the edge head through EdgeHeadFn.  Both heads read the final h, so autograd adds their
+    contributions to dh before the last layer's backward."""
+    if model.edge_W is None:
+        raise ValueError("the model has no edge head (GraphSAGE_T(edge_head=False))")
+    model._check_graph(x, tg.rowptr, tg.col, tg.edge_w)
+    h = x
+    for l, (W, b) in enumerate(zip(model.weights, model.biases)):
+        h = SageLayerFn.apply(h, W, b, tg, model, l)
+    return h @ model.node_w + model.node_b, EdgeHeadFn.apply(h, model.edge_W, model.edge_b, tg, model)
 
 
 # ---------------------------------------------------------------------------------------------------- BiLSTM scorer

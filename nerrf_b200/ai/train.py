@@ -32,9 +32,9 @@ from .models.lstm import LSTMScorer
 
 
 # ------------------------------------------------------------------ differentiable restatements (autograd only)
-def sage_node_logits(model: GraphSAGE_T, x, rowptr, col, ew):
-    """Node-head logits of GraphSAGE-T with autograd: h' = ReLU([h || m] W + b), m = weighted mean over in-edges,
-    logit = h . w_n + b_n  (the spec in ai/models/graphsage_t.py; sigmoid(logit) is what the CUDA forward returns)."""
+def sage_embeddings(model: GraphSAGE_T, x, rowptr, col, ew):
+    """Final GraphSAGE-T embeddings with autograd: h' = ReLU([h || m] W + b), m = weighted mean over in-edges (the spec
+    in ai/models/graphsage_t.py)."""
     N = x.shape[0]
     deg = (rowptr[1:] - rowptr[:-1]).long()
     dst = torch.repeat_interleave(torch.arange(N, device=x.device), deg)
@@ -44,7 +44,36 @@ def sage_node_logits(model: GraphSAGE_T, x, rowptr, col, ew):
     for W, b in zip(model.weights, model.biases):
         agg = torch.zeros(N, h.shape[1], device=x.device, dtype=x.dtype).index_add_(0, dst, h[src] * ew[:, None])
         h = torch.relu(torch.cat([h, agg / wsum[:, None]], 1) @ W + b)
-    return h @ model.node_w + model.node_b
+    return h
+
+
+def sage_node_logits(model: GraphSAGE_T, x, rowptr, col, ew):
+    """Node-head logits of GraphSAGE-T with autograd: logit = h . w_n + b_n over sage_embeddings (sigmoid(logit) is what
+    the CUDA forward returns)."""
+    return sage_embeddings(model, x, rowptr, col, ew) @ model.node_w + model.node_b
+
+
+def edge_logits_from_h(model: GraphSAGE_T, h, rowptr, col):
+    """Edge-head logits [E, 2] (CSR order; column 0 attack, 1 normal) from embeddings h, with autograd:
+    [h_src || h_dst] We + be, computed as (h We[:H])[src] + (h We[H:])[dst] + be (no [E, 2H] intermediate)."""
+    H = h.shape[1]
+    deg = (rowptr[1:] - rowptr[:-1]).long()
+    dst = torch.repeat_interleave(torch.arange(h.shape[0], device=h.device), deg)
+    return (h @ model.edge_W[:H])[col.long()] + (h @ model.edge_W[H:])[dst] + model.edge_b
+
+
+def sage_logits(model: GraphSAGE_T, x, rowptr, col, ew):
+    """(node logits [N], edge logits [E, 2]) with autograd: both heads over the same sage_embeddings."""
+    h = sage_embeddings(model, x, rowptr, col, ew)
+    return h @ model.node_w + model.node_b, edge_logits_from_h(model, h, rowptr, col)
+
+
+def _train_graph(ex):
+    from . import autograd as AG
+    tg = ex.get("_train_graph")
+    if tg is None:
+        tg = ex["_train_graph"] = AG.TrainGraph(ex["rowptr"], ex["col"], ex["ew"])
+    return tg
 
 
 def node_logits(model: GraphSAGE_T, ex):
@@ -52,11 +81,26 @@ def node_logits(model: GraphSAGE_T, ex):
     forward + csrc/sage_bwd.cu backward, nerrf_b200.ai.autograd), on the CPU through the plain-torch restatement above."""
     if ex["x"].is_cuda:
         from . import autograd as AG
-        tg = ex.get("_train_graph")
-        if tg is None:
-            tg = ex["_train_graph"] = AG.TrainGraph(ex["rowptr"], ex["col"], ex["ew"])
-        return AG.sage_node_logits(model, ex["x"], tg)
+        return AG.sage_node_logits(model, ex["x"], _train_graph(ex))
     return sage_node_logits(model, ex["x"], ex["rowptr"], ex["col"], ex["ew"])
+
+
+def node_edge_logits(model: GraphSAGE_T, ex):
+    """(node logits, edge logits) of one example with gradients: on a CUDA device through the library's kernels (the
+    edge head's backward is csrc/sage_edge_bwd.cu), on the CPU through the plain-torch restatement."""
+    if ex["x"].is_cuda:
+        from . import autograd as AG
+        return AG.sage_logits(model, ex["x"], _train_graph(ex))
+    return sage_logits(model, ex["x"], ex["rowptr"], ex["col"], ex["ew"])
+
+
+def edge_loss(edge_logit, edge_label):
+    """Class-balanced cross-entropy of the edge head: column 0 = attack (label 1), column 1 = normal (label 0); the
+    attack class is weighted by #normal / #attack, clamped to 0.2 .. 5 like the node loss's pos_weight."""
+    y = edge_label.to(torch.float32)
+    pos = y.sum().clamp_min(1.0)
+    w = torch.stack([((y.numel() - pos) / pos).clamp(0.2, 5.0), torch.ones((), device=y.device)])
+    return nn.functional.cross_entropy(edge_logit, (1 - edge_label.long()), weight=w)
 
 
 def lstm_logits(scorer: LSTMScorer, seq, lengths):
@@ -86,15 +130,16 @@ def roc_auc(scores, labels) -> float:
 
 
 # ------------------------------------------------------------------ toy set (simulator-schema LockBit traces)
-def make_example(seed: int, n_files: int = 30, benign_files: int = 40, window=None) -> dict:
+def make_example(seed: int, n_files: int = 30, benign_files: int = 40, window=None, bystanders: int = 0) -> dict:
     """One labelled example: a simulated LockBit trace -> graph tensors + per-file sequences.  Labels: a file node
     is positive iff it was encrypted (graph.graph_from_events meta['label'], from the simulator's annotations).
     Features are OBSERVABLE-ONLY (graph.OBSERVABLE_SLOT): the annotation event kinds that define the label
     (file_encrypt_start / _complete, ...) are folded onto the syscalls the tracker can actually see
     (openat / write / rename), so the gate below is not satisfied by reading the label back from the input.
     What remains is what a wire trace carries: write / rename counts, byte counts, timing, the .lockbit extension
-    ("extension pattern", threat-model.mdx:178-184).  The toy set is still easy; see DESIGN.md 2.7."""
-    ev = trace_sim.lockbit_trace(n_files=n_files, seed=seed, benign_files=benign_files)
+    ("extension pattern", threat-model.mdx:178-184).  The toy set is still easy; see DESIGN.md 2.7.
+    bystanders: benign processes touching the files (trace_sim.lockbit_trace); edge labels: graph meta['edge_label']."""
+    ev = trace_sim.lockbit_trace(n_files=n_files, seed=seed, benign_files=benign_files, bystanders=bystanders)
     if window is not None:
         # what the streaming pipeline sees (nerrf_b200.stream): only the events of one sliding window, so a file's
         # history may start with its encryption and the clock features are relative to the window
@@ -107,7 +152,7 @@ def make_example(seed: int, n_files: int = 30, benign_files: int = 40, window=No
     return {"x": t(g.x), "rowptr": t(g.rowptr), "col": t(g.col), "ew": t(g.ew),
             "label": t(g.meta["label"].astype(np.float32)), "is_file": t(g.meta["node_kind"] == 0),
             "seq": t(seq), "lengths": t(lengths), "seq_label": t(g.meta["label"][nodes].astype(np.float32)),
-            "graph": g, "events": ev, "seq_nodes": nodes}
+            "edge_label": t(g.meta["edge_label"]), "graph": g, "events": ev, "seq_nodes": nodes}
 
 
 def toy_set(seeds, windows: int = 2, **kw):
@@ -135,12 +180,18 @@ LSTM_BACKWARDS = ("torch", "library")
 
 
 def train(model: GraphSAGE_T, scorer: LSTMScorer | None, examples, epochs: int = 150, lr: float = 3e-3, device="cpu",
-          log=None, lstm_backward: str = "torch"):
+          log=None, lstm_backward: str = "torch", edge_weight: float = 0.0):
     """Joint loss = BCE(node logits over file nodes) + BCE(LSTM encrypt_probability logit); Adam; full batch per trace.
     lstm_backward: "torch" differentiates torch.nn.LSTM (cuDNN on a GPU); "library" runs the BiLSTM forward and
-    backward on this library's kernels (nerrf_b200.ai.autograd.lstm_logits) when `device` is a CUDA device."""
+    backward on this library's kernels (nerrf_b200.ai.autograd.lstm_logits) when `device` is a CUDA device.
+    edge_weight > 0: the loss also gains edge_weight * the class-balanced cross-entropy of the edge head against
+    the examples' edge labels (edge_loss), and the model is marked `edge_head_trained` (a plain attribute, not a
+    state_dict entry), which lets pipeline.run attribute files to processes by the edge head."""
     if lstm_backward not in LSTM_BACKWARDS:
         raise ValueError(f"lstm_backward must be one of {LSTM_BACKWARDS}, got {lstm_backward!r}")
+    edges = edge_weight > 0
+    if edges and model.edge_W is None:
+        raise ValueError("edge_weight > 0 needs a model with an edge head")
     device = torch.device(device)
     library_lstm = lstm_backward == "library" and device.type == "cuda"
     if library_lstm:
@@ -157,10 +208,15 @@ def train(model: GraphSAGE_T, scorer: LSTMScorer | None, examples, epochs: int =
         total = 0.0
         for ex in data:
             opt.zero_grad()
-            logit = node_logits(model, ex)
+            if edges:
+                logit, el = node_edge_logits(model, ex)
+            else:
+                logit = node_logits(model, ex)
             m = ex["is_file"]
             pos = ex["label"][m].sum().clamp_min(1.0)
             loss = bce(logit[m], ex["label"][m], pos_weight=((m.sum() - pos) / pos).clamp(0.2, 5.0))
+            if edges and el.shape[0]:
+                loss = loss + edge_weight * edge_loss(el, ex["edge_label"])
             if scorer is not None and ex["seq"].shape[0]:
                 if library_lstm:
                     sl = AG.lstm_logits(scorer, ex["seq"], ex["lengths"])
@@ -172,17 +228,30 @@ def train(model: GraphSAGE_T, scorer: LSTMScorer | None, examples, epochs: int =
             total += float(loss.detach())
         if log and (ep % 25 == 0 or ep == epochs - 1):
             log(f"epoch {ep:4d}  loss {total / len(data):.4f}")
+    if edges:
+        model.edge_head_trained = True
     return model, scorer
 
 
 @torch.no_grad()
-def evaluate(model: GraphSAGE_T, scorer: LSTMScorer | None, examples, device="cpu") -> dict:
+def evaluate(model: GraphSAGE_T, scorer: LSTMScorer | None, examples, device="cpu", edges: bool = False) -> dict:
     """ROC-AUC of the node scores over file nodes and of the LSTM encrypt_probability over sequences (autograd
-    restatement; tests/test_gpu_train.py checks the CUDA inference path gives the same scores)."""
+    restatement; tests/test_gpu_train.py checks the CUDA inference path gives the same scores).
+    edges=True adds edge_auc (P(attack) = softmax column 0 over every labelled edge) and edge_auc_encrypted (only the
+    edges incident to an encrypted file: attacker vs. bystander, which the file scores cannot separate)."""
     device = torch.device(device)
     ns, nl, ss, sl_ = [], [], [], []
+    es, el_, enc = [], [], []
     for ex in (_to(e, device) for e in examples):
-        logit = sage_node_logits(model.to(device), ex["x"], ex["rowptr"], ex["col"], ex["ew"])
+        if edges:
+            logit, elog = sage_logits(model.to(device), ex["x"], ex["rowptr"], ex["col"], ex["ew"])
+            es.append(torch.softmax(elog, 1)[:, 0].cpu().numpy()); el_.append(ex["edge_label"].cpu().numpy())
+            lab = ex["label"].cpu().numpy() > 0
+            rp = ex["rowptr"].cpu().numpy().astype(np.int64)
+            dst = np.repeat(np.arange(rp.size - 1), np.diff(rp))
+            enc.append(lab[ex["col"].cpu().numpy()] | lab[dst])
+        else:
+            logit = sage_node_logits(model.to(device), ex["x"], ex["rowptr"], ex["col"], ex["ew"])
         m = ex["is_file"]
         ns.append(torch.sigmoid(logit[m]).cpu().numpy()); nl.append(ex["label"][m].cpu().numpy())
         if scorer is not None and ex["seq"].shape[0]:
@@ -191,6 +260,10 @@ def evaluate(model: GraphSAGE_T, scorer: LSTMScorer | None, examples, device="cp
     out = {"gnn_auc": roc_auc(np.concatenate(ns), np.concatenate(nl))}
     if ss:
         out["lstm_auc"] = roc_auc(np.concatenate(ss), np.concatenate(sl_))
+    if edges:
+        s, y, e = np.concatenate(es), np.concatenate(el_), np.concatenate(enc)
+        out["edge_auc"] = roc_auc(s, y)
+        out["edge_auc_encrypted"] = roc_auc(s[e], y[e])
     return out
 
 
@@ -202,15 +275,23 @@ def main(argv=None):
     ap.add_argument("--no-lstm", action="store_true")
     ap.add_argument("--lstm-backward", choices=LSTM_BACKWARDS, default="torch",
                     help="BiLSTM training path on a CUDA device: torch.nn.LSTM under autograd, or the library's kernels")
+    ap.add_argument("--edge-loss", type=float, default=0.0, metavar="W",
+                    help="also train the attack/normal edge head with this loss weight (toy traces get 2 bystander "
+                         "processes, so the edge labels differ from the file labels)")
     a = ap.parse_args(argv)
-    train_set = toy_set(range(100, 100 + a.traces)); test_set = toy_set(range(900, 903))
+    edges = a.edge_loss > 0
+    kw = {"bystanders": 2} if edges else {}
+    train_set = toy_set(range(100, 100 + a.traces), **kw); test_set = toy_set(range(900, 903), **kw)
     model = GraphSAGE_T(G.F_IN, 128, a.layers); scorer = None if a.no_lstm else LSTMScorer()
-    print("before:", evaluate(model, scorer, test_set, a.device))
-    train(model, scorer, train_set, a.epochs, a.lr, a.device, log=print, lstm_backward=a.lstm_backward)
-    print("held-out:", evaluate(model, scorer, test_set, a.device))
+    print("before:", evaluate(model, scorer, test_set, a.device, edges=edges))
+    train(model, scorer, train_set, a.epochs, a.lr, a.device, log=print, lstm_backward=a.lstm_backward,
+          edge_weight=a.edge_loss)
+    print("held-out:", evaluate(model, scorer, test_set, a.device, edges=edges))
     if a.out:
-        torch.save({"sage": model.state_dict(), "lstm": None if scorer is None else scorer.state_dict(),
-                    "layers": a.layers}, a.out)
+        ck = {"sage": model.state_dict(), "lstm": None if scorer is None else scorer.state_dict(), "layers": a.layers}
+        if edges:
+            ck["edge_head_trained"] = True
+        torch.save(ck, a.out)
         print("wrote", a.out)
 
 

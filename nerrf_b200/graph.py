@@ -208,7 +208,9 @@ def graph_from_events(events, merge_renames=True, window=None, observable=False)
     """Events -> temporal graph.  Nodes: one per pid (process) and one per file identity.
     Edges (both directions, so files aggregate from the process that touched them and the
     process from its files): process<->file per event with time t_e and conf_e = 1; rename /
-    encrypt pairs are merged into one file node when merge_renames (else linked file<->file)."""
+    encrypt pairs are merged into one file node when merge_renames (else linked file<->file).
+    meta['edge_label'] (uint8 [E], CSR order): 1 on both edges of a process <-> file pair iff that process emitted an
+    ATTACK_EVENTS event on that file; 0 elsewhere (rename links included)."""
     evs = resolve_event_paths(events)
     if not evs:
         raise ValueError("empty trace")
@@ -227,6 +229,7 @@ def graph_from_events(events, merge_renames=True, window=None, observable=False)
     src, dst, tt = [], [], []
     feats: dict = {}
     labels: dict = {}
+    attack_pairs: set = set()          # (process, file) pairs with an ATTACK_EVENTS event of that process on that file
     for e in evs:
         t = _parse_ts(e["timestamp"]) - t0
         p = nid(("p", e["pid"]), 1, f"pid:{e['pid']}")
@@ -259,6 +262,8 @@ def graph_from_events(events, merge_renames=True, window=None, observable=False)
         fv["lockbit"] = max(fv["lockbit"], 1.0 if ".lockbit" in path or (merge_renames and ".lockbit" in new_path) else 0.0)
         fv["note"] = max(fv["note"], 1.0 if "README" in path.upper() or "RANSOM" in path.upper() else 0.0)
         fv["tmp"] = max(fv["tmp"], 1.0 if path.startswith("/tmp") or path.startswith("/proc") else 0.0)
+        if e["event"] in ATTACK_EVENTS:
+            attack_pairs.add((p, f))
         attacked = e["event"] in ATTACK_EVENTS or e.get("phase") == "attack" and e["event"].startswith("file_encrypt")
         labels[f] = max(labels.get(f, 0), 1 if (attacked and e["event"] != "ransom_note_created"
                                                  and e["event"].startswith("file_encrypt")) else 0)
@@ -267,6 +272,11 @@ def graph_from_events(events, merge_renames=True, window=None, observable=False)
     tt = np.asarray(tt, np.float32)
     conf = np.ones(src.shape[0], np.float32)
     rowptr, col, ew = csr_from_edges(src, dst, tt, conf, N, t_ref=float(span), tau=TAU)
+    # per-pair edge labels in CSR order (the edge head sees only [h_src || h_dst], the same for every event of a pair):
+    # 1 in both directions iff the process attacked the file; file <-> file rename links are 0
+    pair = src * N + dst
+    hit = np.asarray([p_ * N + f_ for p_, f_ in attack_pairs] + [f_ * N + p_ for p_, f_ in attack_pairs], np.int64)
+    edge_label = np.isin(pair, hit).astype(np.uint8)[np.lexsort((tt, dst))]
     indeg = np.bincount(dst, minlength=N).astype(np.float32)
     outdeg = np.bincount(src, minlength=N).astype(np.float32)
     x = np.zeros((N, F_IN), np.float32)
@@ -293,7 +303,8 @@ def graph_from_events(events, merge_renames=True, window=None, observable=False)
     file_keys = {k[1]: v for k, v in node_id.items() if k[0] == "f"}      # merge key (or path) -> node, incl. rename aliases
     return TemporalGraph(rowptr, col, ew, x, {"kind": "trace", "names": names, "node_kind": np.asarray(kinds),
                                               "label": y, "size_mb": size_mb, "t0": t0, "span": span,
-                                              "file_keys": file_keys, "merge_renames": bool(merge_renames)})
+                                              "file_keys": file_keys, "merge_renames": bool(merge_renames),
+                                              "edge_label": edge_label})
 
 
 def graph_from_jsonl(path, **kw) -> TemporalGraph:

@@ -72,6 +72,8 @@ class PipelineResult:
     plan_nodes: list                  # node ids to revert, in plan order
     timings_ms: dict = field(default_factory=dict)
     n_kill: int = 0                   # the first n_kill candidates are process nodes ("kill process" actions)
+    kill_attribution: str | None = None   # how files were attributed to processes: "writer" (last process in-edge) or
+                                          # "edges" (the trained edge head); None when no kill actions were proposed
 
 
 @dataclass
@@ -87,9 +89,11 @@ class DistContext:
 
 
 def _sage_scores(g_dev, model, ctx):
+    """-> (node scores, final embeddings h); h is None on the sharded multi-GPU path."""
     x, rp, col, ew = g_dev
     if ctx is None or ctx.world == 1:
-        return model(x, rp, col, ew)[1]
+        h, score = model(x, rp, col, ew)
+        return score, h
     import torch.distributed as dist
     from . import dist as ND
     ss = ND.ShardedSage(model, rp, col, ew, ctx.rank, ctx.world, x.device, exchange=ctx.exchange)
@@ -98,7 +102,7 @@ def _sage_scores(g_dev, model, ctx):
     cuts = ss.shard.cuts
     parts = [torch.empty(int(cuts[p + 1] - cuts[p]), device=x.device) for p in range(ctx.world)]
     dist.all_gather(parts, score[int(cuts[ctx.rank]):int(cuts[ctx.rank + 1])].contiguous())
-    return torch.cat(parts)
+    return torch.cat(parts), None
 
 
 def _lstm_probs(seq_model, seq_sel, len_sel, dev, ctx):
@@ -118,14 +122,29 @@ def _lstm_probs(seq_model, seq_sel, len_sel, dev, ctx):
     return torch.cat(parts)[:a]
 
 
-def process_kill_candidates(g: G.TemporalGraph, candidates: np.ndarray, max_kills: int = 32):
+def _edge_rows(rp: torch.Tensor, cand: torch.Tensor):
+    """CSR positions of the in-edges of the rows `cand`, row by row: (edge index [m], candidate index [m])."""
+    deg = (rp[cand + 1] - rp[cand]).numpy()
+    seg = np.repeat(np.arange(cand.shape[0], dtype=np.int64), deg)
+    start = np.cumsum(deg) - deg
+    idx = np.repeat(rp[cand].numpy(), deg) + np.arange(seg.shape[0], dtype=np.int64) - np.repeat(start, deg)
+    return idx, seg
+
+
+def process_kill_candidates(g: G.TemporalGraph, candidates: np.ndarray, max_kills: int = 32, edge_attack=None):
     """Non-revert undo candidates derived from the graph (threat-model.mdx:208-222 "Kill process", cost 10): the
-    process nodes that wrote the candidate files, the ones with the most candidate files first.
-    -> (pid_nodes [k], guard [A] = index into pid_nodes of the process that wrote each candidate file, or -1)."""
+    process nodes that own the candidate files, the ones with the most candidate files first.
+    A file's owner is its last writer (the source of its most recent process in-edge) -- or, given `edge_attack`
+    (P(attack) [E] per CSR edge, from a trained edge head), the process source in its row with the highest P(attack),
+    ties to the latest edge: a backup agent or scanner that opened an encrypted file after the ransomware is then not
+    taken for its writer.
+    -> (pid_nodes [k], guard [A] = index into pid_nodes of the owner of each candidate file, or -1)."""
     kind = torch.as_tensor(np.asarray(g.meta["node_kind"]))
     rp = (g.rowptr.cpu() if torch.is_tensor(g.rowptr) else torch.from_numpy(np.asarray(g.rowptr))).long()
     col = (g.col.cpu() if torch.is_tensor(g.col) else torch.from_numpy(np.asarray(g.col))).long()
     cand = torch.from_numpy(np.asarray(candidates, np.int64))
+    if edge_attack is not None:
+        return _owners_to_kills(_edge_owners(kind, rp, col, cand, np.asarray(edge_attack, np.float32)), max_kills)
     # the most recent in-edge of a file node (rows are time-sorted) whose source is a process = its last writer
     owner = np.full(cand.shape[0], -1, np.int64)
     last = rp[cand + 1] - 1
@@ -137,13 +156,47 @@ def process_kill_candidates(g: G.TemporalGraph, candidates: np.ndarray, max_kill
         n = int(cand[i]); s_ = col[rp[n]:rp[n + 1]]; s_ = s_[kind[s_] == 1]
         if s_.numel():
             owner[i] = int(s_[-1])
+    return _owners_to_kills(owner, max_kills)
+
+
+def _owners_to_kills(owner: np.ndarray, max_kills: int):
     pids, counts = np.unique(owner[owner >= 0], return_counts=True)
     if pids.size == 0:
-        return np.zeros(0, np.int64), np.full(cand.shape[0], -1, np.int64)
+        return np.zeros(0, np.int64), np.full(owner.shape[0], -1, np.int64)
     chosen = pids[np.lexsort((pids, -counts))[:max_kills]]
     slot = np.full(int(max(pids.max(), 0)) + 1, -1, np.int64); slot[chosen] = np.arange(chosen.shape[0])
     guard = np.where(owner >= 0, slot[np.maximum(owner, 0)], -1)
     return chosen, guard
+
+
+def _edge_owners(kind, rp, col, cand, edge_attack):
+    """Per candidate file: the process source of its row with the highest P(attack), ties to the latest edge; -1 if none."""
+    idx, seg = _edge_rows(rp, cand)
+    src = col.numpy()[idx]
+    keep = kind.numpy()[src] == 1
+    idx, seg, src = idx[keep], seg[keep], src[keep]
+    owner = np.full(cand.shape[0], -1, np.int64)
+    if idx.size:
+        o = np.lexsort((idx, edge_attack[idx], seg))           # per row ascending (P(attack), position): the last one wins
+        last = np.ones(o.shape[0], bool); last[:-1] = seg[o][1:] != seg[o][:-1]
+        owner[seg[o][last]] = src[o][last]
+    return owner
+
+
+def edge_kill_confidence(g: G.TemporalGraph, candidates: np.ndarray, pids: np.ndarray, edge_attack) -> np.ndarray:
+    """Confidence that each process in `pids` is malicious: the highest P(attack) over its edges into the candidate
+    files (0 if it has none)."""
+    rp = (g.rowptr.cpu() if torch.is_tensor(g.rowptr) else torch.from_numpy(np.asarray(g.rowptr))).long()
+    col = (g.col.cpu() if torch.is_tensor(g.col) else torch.from_numpy(np.asarray(g.col))).long()
+    idx, _ = _edge_rows(rp, torch.from_numpy(np.asarray(candidates, np.int64)))
+    src = col.numpy()[idx]
+    ea = np.asarray(edge_attack, np.float32)[idx]
+    out = np.zeros(len(pids), np.float32)
+    for k, p_ in enumerate(np.asarray(pids).tolist()):
+        m = src == p_
+        if m.any():
+            out[k] = ea[m].max()
+    return out
 
 
 def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_model, top_a=1024, confidence=None,
@@ -155,7 +208,9 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
     confidence: optional override of p_a per NODE (e.g. ground-truth labels when no trained weights exist).
     exclude: bool [len(seq_nodes)] -- sequences whose file was already reverted by an earlier tick of the stream.
     kill_candidates: also propose "kill process" actions (cost 10) for the processes that wrote the candidate files;
-    a file reversion only sticks once its writer is gone (planner spec v1, DESIGN.md 1.3)."""
+    a file reversion only sticks once its writer is gone (planner spec v1, DESIGN.md 1.3).  A model marked
+    `edge_head_trained` (ai.train with edge_weight > 0) attributes files to processes by its edge head instead of the
+    last-writer rule, on one GPU; res.kill_attribution records which rule ran."""
     dev = torch.device(device)
     tm = {}
     sync = torch.cuda.synchronize
@@ -167,7 +222,7 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
     sync(); tm["h2d_graph"] = (time.perf_counter() - t0) * 1e3
 
     t0 = time.perf_counter()
-    score = _sage_scores((x, rp, col, ew), model, dist_ctx)
+    score, h_final = _sage_scores((x, rp, col, ew), model, dist_ctx)
     sync(); tm["graphsage_t"] = (time.perf_counter() - t0) * 1e3
 
     t0 = time.perf_counter()
@@ -208,14 +263,23 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
         p = np.asarray(confidence, np.float32)[cand]
         actions = Actions(p, size_mb, np.ones(a, np.float32))
     elif kill_candidates:
-        pids, guard = process_kill_candidates(g, cand)
+        edge_attack = None
+        if getattr(model, "edge_head_trained", False) and h_final is not None and model.edge_W is not None:
+            # files are attributed to processes by the trained edge head (P(attack) of each CSR edge)
+            _, el = model.heads(h_final, rp, col, return_edge_logits=True)
+            edge_attack = torch.softmax(el, 1)[:, 0].cpu().numpy()
+        pids, guard = process_kill_candidates(g, cand, edge_attack=edge_attack)
         n_kill = int(pids.shape[0])
         a_rev = min(a, 4096 - n_kill)                                  # kill actions occupy the first slots (spec v1: guards < 32)
         p_rev = 0.5 * (score[candidates[:a_rev]].cpu().numpy() + probs[:a_rev, 0].cpu().numpy())
-        # confidence that a process is malicious = mean confidence of the candidate files it wrote (the model's node head
-        # is trained on file nodes only)
         gr = guard[:a_rev]
-        p_kill = np.array([p_rev[gr == k].mean() if (gr == k).any() else 0.0 for k in range(n_kill)], np.float32)
+        if edge_attack is not None:
+            # confidence that a process is malicious = the highest P(attack) over its edges into the candidate files
+            p_kill = edge_kill_confidence(g, cand, pids, edge_attack)
+        else:
+            # confidence that a process is malicious = mean confidence of the candidate files it wrote (the model's node
+            # head is trained on file nodes only)
+            p_kill = np.array([p_rev[gr == k].mean() if (gr == k).any() else 0.0 for k in range(n_kill)], np.float32)
         p_all = np.concatenate([p_kill, p_rev]).astype(np.float32)
         size_all = np.concatenate([np.zeros(n_kill, np.float32), size_mb[:a_rev]])
         kind = np.concatenate([np.full(n_kill, RW_KIND_KILL, np.int64), np.zeros(a_rev, np.int64)])
@@ -234,4 +298,6 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
     tm["total"] = sum(tm.values())
     res = PipelineResult(score, cand, probs, pl, [int(cand[i]) for i in pl.actions], tm)
     res.n_kill = n_kill
+    if confidence is None and kill_candidates:
+        res.kill_attribution = "writer" if edge_attack is None else "edges"
     return res

@@ -44,6 +44,8 @@ def load_models(weights: str | None, train_epochs: int, layers: int = 2, log=pri
         ck = torch.load(weights, map_location="cpu")
         model = GraphSAGE_T(G.F_IN, 128, int(ck.get("layers", layers)))
         model.load_state_dict(ck["sage"])
+        if ck.get("edge_head_trained"):                             # ai.train --edge-loss: files are attributed by the edge head
+            model.edge_head_trained = True
         if ck.get("lstm") is not None:
             scorer.load_state_dict(ck["lstm"])
     elif train_epochs > 0:
