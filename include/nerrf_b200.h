@@ -45,6 +45,11 @@ extern "C" {
 /* OR into `algo` of nerrf_sage_layer_fwd_ex: long_ws already holds the hub-row scan of THIS graph and row
  * range (it depends on rowptr only), e.g. layers 2..L of one forward: skip the re-scan. */
 #define NERRF_SAGE_FLAG_REUSE_LONG_SCAN 0x100
+/* OR into `algo` (layer calls, nerrf_sage_forward, the host session): no L2 eviction-priority hints in the tensor-core
+ * layer, every access at normal priority.  By default, at F = 64 / 128, its gathered source rows, self terms, output
+ * rows and edge slices are loaded and stored evict-first.  The results are the same bits either way; the flag is there
+ * to compare the two. */
+#define NERRF_SAGE_FLAG_NO_L2_POLICY 0x200
 
 typedef void* nerrf_stream_t;    /* cudaStream_t */
 

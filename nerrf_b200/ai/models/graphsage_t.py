@@ -32,6 +32,9 @@ class GraphSAGE_T(nn.Module):
         if in_dim not in (32, 64, 128):
             raise ValueError("in_dim must be 32, 64 or 128 (pad the node features)")
         self.in_dim, self.hidden, self.num_layers, self.algo = in_dim, hidden, num_layers, algo
+        # L2 eviction-priority hints of the tensor-core layer (NERRF_SAGE_FLAG_NO_L2_POLICY when off); no result bit
+        # depends on it
+        self.l2_policy = True
         g = torch.Generator().manual_seed(seed) if seed is not None else None
 
         def xavier(fi, fo):
@@ -55,6 +58,9 @@ class GraphSAGE_T(nn.Module):
         self._node_b_cache = (None, 0.0)
 
     # -- helpers ------------------------------------------------------------------------
+    def _algo_flags(self) -> int:
+        return ALGOS[self.algo] | (0 if self.l2_policy else 0x200)
+
     def oracle_params(self):
         """The same weights in the dict layout oracle/sage_ref.py takes (tests only use this)."""
         p = {"layers": [(w.detach().cpu(), b.detach().cpu()) for w, b in zip(self.weights, self.biases)],
@@ -122,7 +128,7 @@ class GraphSAGE_T(nn.Module):
         else:
             colp, ewp = L.ptr(col), L.ptr(edge_w)
         lws, lws_bytes = self._long_rows_ws(col.numel(), h.device) if self._has_hub_rows(rowptr) else (None, 0)
-        algo_flags = ALGOS[self.algo] | (0x100 if reuse_long_scan else 0)
+        algo_flags = self._algo_flags() | (0x100 if reuse_long_scan else 0)
         if multicast_ptr:                       # NVSwitch multicast address of `out` on every rank (nerrf_b200.dist)
             import ctypes as C
             pp = (C.c_void_p * 1)(multicast_ptr); npeers = -1
@@ -197,7 +203,7 @@ class GraphSAGE_T(nn.Module):
             L.check(L.lib().nerrf_sage_forward(L.ptr(x), L.ptr(rowptr), int(rowptr.dtype == torch.int64), L.ptr(col),
                                                L.ptr(edge_w), N, self.in_dim, self.hidden, self.num_layers, Wp, bp,
                                                L.ptr(self.node_w), self._node_b_host(), L.ptr(h), L.ptr(score), L.ptr(ws),
-                                               ws.numel(), ALGOS[self.algo],
+                                               ws.numel(), self._algo_flags(),
                                                L.current_stream_ptr()), "nerrf_sage_forward")
         if return_edge_logits and self.edge_W is not None:
             _, el = self.heads(h, rowptr, col, return_edge_logits=True)
@@ -229,7 +235,7 @@ class HostSession:
                 raise L.NerrfError("HostSession takes host tensors")
         if rowptr.dtype != torch.int32:
             raise TypeError("host session uses int32 rowptr")
-        algo = ALGOS[self.model.algo]
+        algo = self.model._algo_flags()
         L.check(L.lib().nerrf_sage_session_forward_host(self._h, L.ptr(x), L.ptr(rowptr), L.ptr(col), L.ptr(edge_w),
                                                         x.shape[0], col.numel(), L.ptr(score_out), L.ptr(h_out), algo),
                 "nerrf_sage_session_forward_host")
@@ -248,7 +254,7 @@ class HostSession:
         ticket = C.c_uint64(0)
         L.check(L.lib().nerrf_sage_session_submit_host(self._h, L.ptr(x), L.ptr(rowptr), L.ptr(col), L.ptr(edge_w),
                                                        x.shape[0], col.numel(), L.ptr(score_out), L.ptr(h_out),
-                                                       ALGOS[self.model.algo], C.byref(ticket)),
+                                                       self.model._algo_flags(), C.byref(ticket)),
                 "nerrf_sage_session_submit_host")
         self._inflight[ticket.value] = (x, rowptr, col, edge_w, score_out, h_out)
         return ticket.value

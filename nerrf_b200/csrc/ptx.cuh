@@ -72,6 +72,52 @@ __device__ __forceinline__ void cp_async16_pred(uint32_t smem_dst, const void* g
         ::"r"(smem_dst), "l"(gsrc), "r"((uint32_t)pred)
         : "memory");
 }
+// ---------------------------------------------------------------- L2 eviction-priority hints
+// A policy (createpolicy, applied to every access that carries it) is passed to the .L2::cache_hint form of an access.
+// The operand ends up in a uniform register: pass a value that is the same in every lane, or ptxas emits a loop over
+// the distinct values.  Hints only change which lines L2 evicts first, never the data an access returns.  createpolicy
+// is volatile so that it is issued where the policy is used instead of holding two registers for the whole kernel.
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_normal() {
+    uint64_t p;
+    asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(p));
+    return p;
+}
+__device__ __forceinline__ void bulk_g2s_hint(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t bar, uint64_t pol) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(smem_dst), "l"(gsrc), "r"(bytes), "r"(bar), "l"(pol)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_prefetch_l2_hint(const void* gsrc, uint32_t bytes, uint64_t pol) {
+    asm volatile("cp.async.bulk.prefetch.L2.global.L2::cache_hint [%0], %1, %2;" ::"l"(gsrc), "r"(bytes), "l"(pol) : "memory");
+}
+__device__ __forceinline__ void cp_async16_pred_hint(uint32_t smem_dst, const void* gsrc, bool pred, uint64_t pol) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %2, 0;\n\t"
+        "@p cp.async.cg.shared.global.L2::cache_hint [%0], [%1], 16, %3;\n\t}"
+        ::"r"(smem_dst), "l"(gsrc), "r"((uint32_t)pred), "l"(pol)
+        : "memory");
+}
+// read-only loads that do not allocate in L1, and a store, with an L2 policy
+__device__ __forceinline__ float2 ld_nc_na_hint(const float2* p, uint64_t pol) {
+    float2 v;
+    asm("ld.global.nc.L1::no_allocate.L2::cache_hint.v2.f32 {%0, %1}, [%2], %3;" : "=f"(v.x), "=f"(v.y) : "l"(p), "l"(pol));
+    return v;
+}
+__device__ __forceinline__ float4 ld_nc_na_hint(const float4* p, uint64_t pol) {
+    float4 v;
+    asm("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.f32 {%0, %1, %2, %3}, [%4], %5;"
+                 : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p), "l"(pol));
+    return v;
+}
+__device__ __forceinline__ void st_hint(float2* p, float2 v, uint64_t pol) {
+    asm volatile("st.global.L2::cache_hint.v2.f32 [%0], {%1, %2}, %3;" ::"l"(p), "f"(v.x), "f"(v.y), "l"(pol) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }

@@ -15,7 +15,12 @@ int sage_layer_umma(const float* x, const void* rowptr, int is64, const int32_t*
                     const float* W, const float* b, float* out, int64_t n_nodes, int64_t row_begin,
                     int64_t row_end, int F, int relu, int nsplit, const float* node_w, float node_b, float* score,
                     void* long_ws, size_t long_ws_bytes, bool reuse_scan, float* const* peer_out, int n_peers,
-                    const uint8_t* peer_need, cudaStream_t st);   // sage_umma.cu (node_w != NULL: node head fused into the epilogue)
+                    const uint8_t* peer_need, int l2_policy, cudaStream_t st);   // sage_umma.cu (node_w != NULL: node head fused into the epilogue)
+
+// `algo` of one layer call of a multi-layer driver: the caller's selector and L2 flag, REUSE_LONG_SCAN set by the driver
+static int layer_algo(int algo, bool reuse_scan) {
+    return (algo & ~NERRF_SAGE_FLAG_REUSE_LONG_SCAN) | (reuse_scan ? NERRF_SAGE_FLAG_REUSE_LONG_SCAN : 0);
+}
 
 // ------------------------------------------------------------------------------------------
 // K1 standalone: one warp per destination row.
@@ -281,12 +286,13 @@ static int layer_fwd_impl(const float* x, const void* rowptr, int rowptr_is64, c
     NERRF_REQUIRE(!node_w || score, "score output required with node_w");
     cudaStream_t st = (cudaStream_t)stream;
     const bool reuse_scan = (algo & NERRF_SAGE_FLAG_REUSE_LONG_SCAN) != 0;
+    const int l2_policy = (algo & NERRF_SAGE_FLAG_NO_L2_POLICY) ? 0 : 1;
     algo &= 0xFF;
     if (algo == NERRF_SAGE_ALGO_AUTO) algo = NERRF_SAGE_ALGO_UMMA;
     if (algo == NERRF_SAGE_ALGO_UMMA || algo == NERRF_SAGE_ALGO_UMMA2)
         return sage_layer_umma(x, rowptr, rowptr_is64, col, ew, W, b, out, n_nodes, row_begin, row_end, F, relu,
                                algo == NERRF_SAGE_ALGO_UMMA ? 3 : 2, node_w, node_b, score, long_ws, long_ws_bytes,
-                               reuse_scan, peer_out, n_peers, peer_need, st);
+                               reuse_scan, peer_out, n_peers, peer_need, l2_policy, st);
     NERRF_REQUIRE(n_peers == 0, "the fused peer exchange needs the tensor-core layer (algo umma)");
     NERRF_REQUIRE(algo == NERRF_SAGE_ALGO_FFMA, "unknown algo %d", algo);
     rc = rowptr_is64
@@ -388,7 +394,7 @@ extern "C" int nerrf_sage_forward(const float* x, const void* rowptr, int rowptr
         float* o = ((num_layers - 1 - l) % 2 == 0) ? h_out : workspace;
         const bool last = l == num_layers - 1;
         int rc = layer_fwd_impl(in, rowptr, rowptr_is64, col, ew, W[l], b[l], o, n_nodes, 0, n_nodes, F, hidden, 1,
-                                (algo & 0xFF) | (l > 0 ? NERRF_SAGE_FLAG_REUSE_LONG_SCAN : 0),
+                                layer_algo(algo, l > 0),
                                 (last && score_out) ? node_w : nullptr, node_b, (last && score_out) ? score_out : nullptr,
                                 long_ws, long_ws_bytes, nullptr, 0, nullptr, stream);
         if (rc) return rc;
@@ -550,13 +556,13 @@ extern "C" int nerrf_sage_session_submit_host(nerrf_sage_session* s, const float
                     NERRF_CHECK_CUDA(cudaStreamWaitEvent(st, s->ev[k][c], 0));
                     if (cut[c + 1] > cut[c]) {
                         rc = layer_fwd_impl(in, drp, 0, dcol, dew, s->Wd[l], s->bd[l], o, n_nodes, cut[c], cut[c + 1], F, s->hidden, 1,
-                                            algo & 0xFF, nullptr, 0.f, nullptr, long_ws, long_ws_bytes, nullptr, 0, nullptr, st);
+                                            layer_algo(algo, false), nullptr, 0.f, nullptr, long_ws, long_ws_bytes, nullptr, 0, nullptr, st);
                         if (rc) return rc;
                     }
                 }
             } else {
                 rc = layer_fwd_impl(in, drp, 0, dcol, dew, s->Wd[l], s->bd[l], o, n_nodes, 0, n_nodes, F, s->hidden, 1,
-                                    (algo & 0xFF) | (l > 1 ? NERRF_SAGE_FLAG_REUSE_LONG_SCAN : 0), last ? s->node_w : nullptr, s->node_b,
+                                    layer_algo(algo, l > 1), last ? s->node_w : nullptr, s->node_b,
                                     last ? dscore : nullptr, long_ws, long_ws_bytes, nullptr, 0, nullptr, st);
                 if (rc) return rc;
             }

@@ -246,9 +246,14 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                        const float* __restrict__ ew, const float* __restrict__ W, const float* __restrict__ bias,
                        float* __restrict__ out, int64_t row_begin, int64_t row_end, int relu,
                        const float* __restrict__ node_w, float node_b, float* __restrict__ score, const LongWs lw,
-                       const Peers peers, unsigned* __restrict__ tile_ctr, const uint4* __restrict__ wsplit) {
+                       const Peers peers, unsigned* __restrict__ tile_ctr, const uint4* __restrict__ wsplit,
+                       int l2_policy) {
     using C = UmmaCfg<F, NS>;
     constexpr int LPR = F / 4;
+    // L2 policy, F = 64 / 128 (l2_policy == 0: every access at normal priority): the gathered source rows, S, the output rows
+    // and the col / ew slices are evict-first; the F = 32 layer (QUAD below) gives no hints (measured, DESIGN 2.1).
+    // Created where it is used, so that it holds no register across the roles.
+    auto pol = [l2_policy]() { return l2_policy ? l2_policy_evict_first() : l2_policy_evict_normal(); };
     constexpr int GATHER_WARPS = C::GATHER_WARPS, IDX_STAGES = C::IDX_STAGES;
     extern __shared__ unsigned char smem_dyn[];
     const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;          // SWIZZLE_128B needs 1024-B alignment
@@ -616,7 +621,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                         for (int t = 0; t < QS; t += G) src[t / G] = (uint32_t)icol[kbase + t + grp];   // slack reads stay in smem
 #pragma unroll
                         for (int t = 0; t < QS; t += G)
-                            cp_async16_pred(dst + (uint32_t)(t * F * 4), xs + (size_t)src[t / G] * F, t + grp < nitems);
+                            cp_async16_pred_hint(dst + (uint32_t)(t * F * 4), xs + (size_t)src[t / G] * F, t + grp < nitems, pol());
                     } else if (LONG && ilong >= 0) {                     // hub row: items are pre-aggregated chunk partials
 #pragma unroll
                         for (int t = 0; t < QS; t += G) {
@@ -805,7 +810,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                 if constexpr (C::SELF_SPLIT) {                           // the tile's self terms, read by the consumers
                     const int64_t row0 = row_begin + tile * TN;
                     const int64_t nr = row_end - row0 < TN ? row_end - row0 : TN;
-                    bulk_prefetch_l2(out + row0 * UM, (uint32_t)(nr * UM * 4));
+                    bulk_prefetch_l2_hint(out + row0 * UM, (uint32_t)(nr * UM * 4), pol());
                 }
             }
             __syncwarp();                                                // every lane's rowptr words are written ...
@@ -813,8 +818,13 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                 const uint32_t cs = idx_base + (uint32_t)(q * IDX_STAGE_BYTES), ws = cs + EPAD * 4;
                 mbar_arrive_expect_tx(idxf_bar(q), c_bytes + w_bytes);   // ... and published by this release-arrive
                 if (n) {
-                    bulk_g2s(cs, reinterpret_cast<const void*>(ca & ~(uintptr_t)15), c_bytes, idxf_bar(q));
-                    bulk_g2s(ws, reinterpret_cast<const void*>(wa & ~(uintptr_t)15), w_bytes, idxf_bar(q));
+                    if constexpr (QUAD) {
+                        bulk_g2s(cs, reinterpret_cast<const void*>(ca & ~(uintptr_t)15), c_bytes, idxf_bar(q));
+                        bulk_g2s(ws, reinterpret_cast<const void*>(wa & ~(uintptr_t)15), w_bytes, idxf_bar(q));
+                    } else {
+                        bulk_g2s_hint(cs, reinterpret_cast<const void*>(ca & ~(uintptr_t)15), c_bytes, idxf_bar(q), pol());
+                        bulk_g2s_hint(ws, reinterpret_cast<const void*>(wa & ~(uintptr_t)15), w_bytes, idxf_bar(q), pol());
+                    }
                 }
             }
             return false;
@@ -882,7 +892,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
         for (int u = 0; u < TP; ++u) s_tile[u] = -1;
         auto self_terms = [&](int64_t t, int nb, int e) -> float2 {           // (row 8 nb + 2 c + e of tile t, f0)
             const int64_t row = row_begin + t * TN + 8 * nb + 2 * c + e;
-            return row < row_end ? *reinterpret_cast<const float2*>(out + row * UM + f0) : make_float2(0.f, 0.f);
+            return row < row_end ? ld_nc_na_hint(reinterpret_cast<const float2*>(out + row * UM + f0), pol()) : make_float2(0.f, 0.f);
         };
         auto wait_full = [&](int64_t t) -> int {                              // the CTA's t-th tile id, once gathered
             mbar_wait_relaxed(full_bar((int)(t % C::STAGES)), (uint32_t)(t / C::STAGES) & 1u);
@@ -978,7 +988,8 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                             if (peers.mc) {                                   // NVSwitch multicast: every rank's buffer at once
                                 multimem_st2(peers.mc + off, o);
                             } else {
-                                *reinterpret_cast<float2*>(out + off) = o;
+                                if constexpr (QUAD) *reinterpret_cast<float2*>(out + off) = o;
+                                else st_hint(reinterpret_cast<float2*>(out + off), o, pol());
                                 if (peers.n) {                                // fused exchange over NVLink
                                     const unsigned need = peers.need ? (unsigned)__ldg(peers.need + row) : 0xFFu;
 #pragma unroll
@@ -1080,8 +1091,9 @@ struct PrepCfg {
 template <int F, int NS>
 __global__ void __launch_bounds__(256, 1)
 sage_self_prep_kernel(const float* __restrict__ x, const float* __restrict__ W, float* __restrict__ out, int64_t row_begin,
-                      int64_t row_end, uint4* __restrict__ wsplit) {
+                      int64_t row_end, uint4* __restrict__ wsplit, int l2_policy) {
     using P = PrepCfg<F, NS>;
+    const uint64_t pol = l2_policy ? l2_policy_evict_first() : l2_policy_evict_normal();   // x and S: read / written once
     constexpr int KS = P::KS, SLICES = P::SLICES;
     constexpr int LPR = F / 4;                                // float4 per x row
     constexpr int RPP = 256 / LPR;                            // rows per pass of the CTA
@@ -1110,7 +1122,7 @@ sage_self_prep_kernel(const float* __restrict__ x, const float* __restrict__ W, 
 #pragma unroll
         for (int i = 0; i < NV; ++i) {
             const int64_t row = row_begin + tile * PREP_ROWS + r0 + RPP * i;
-            v[i] = (tile < n_tiles && row < row_end) ? __ldg(reinterpret_cast<const float4*>(x + row * F) + q)
+            v[i] = (tile < n_tiles && row < row_end) ? ld_nc_na_hint(reinterpret_cast<const float4*>(x + row * F) + q, pol)
                                                       : make_float4(0.f, 0.f, 0.f, 0.f);
         }
     };
@@ -1162,7 +1174,7 @@ sage_self_prep_kernel(const float* __restrict__ x, const float* __restrict__ W, 
                 for (int e = 0; e < 2; ++e) {
                     const int64_t row = row0 + TN * sl + 8 * nb + 2 * c + e;
                     if (row < row_end)
-                        *reinterpret_cast<float2*>(out + row * UM + f0) = make_float2(d[sl][4 * nb + e], d[sl][4 * nb + 2 + e]);
+                        st_hint(reinterpret_cast<float2*>(out + row * UM + f0), make_float2(d[sl][4 * nb + e], d[sl][4 * nb + 2 + e]), pol);
                 }
     }
 }
@@ -1199,7 +1211,7 @@ inline uint4* wsplit_buffer(cudaStream_t st) {
 template <int F, int NS, typename RP>
 int launch_umma(const float* x, const RP* rowptr, const int32_t* col, const float* ew, const float* W, const float* b,
                 float* out, int64_t row_begin, int64_t row_end, int relu, const float* node_w, float node_b, float* score,
-                void* long_ws, size_t long_ws_bytes, bool reuse_scan, const Peers& peers, cudaStream_t st) {
+                void* long_ws, size_t long_ws_bytes, bool reuse_scan, const Peers& peers, int l2_policy, cudaStream_t st) {
     using C = UmmaCfg<F, NS>;
     int rc = set_max_dynamic_smem((const void*)sage_layer_umma_kernel<F, NS, RP, false>, C::SMEM);
     if (!rc) rc = set_max_dynamic_smem((const void*)sage_layer_umma_kernel<F, NS, RP, true>, C::SMEM);
@@ -1234,15 +1246,16 @@ int launch_umma(const float* x, const RP* rowptr, const int32_t* col, const floa
         rc = set_max_dynamic_smem((const void*)sage_self_prep_kernel<F, NS>, P::SMEM);
         if (rc) return rc;
         const int64_t ptiles = (rows + PREP_ROWS - 1) / PREP_ROWS;
-        sage_self_prep_kernel<F, NS><<<(unsigned)(ptiles < sm_count() ? ptiles : sm_count()), 256, P::SMEM, st>>>(x, W, out, row_begin, row_end, wsplit);
+        sage_self_prep_kernel<F, NS><<<(unsigned)(ptiles < sm_count() ? ptiles : sm_count()), 256, P::SMEM, st>>>(x, W, out, row_begin, row_end, wsplit,
+                                                                                                            l2_policy);
     } else {
         split_w_kernel<NS><<<(C::KSTEPS * 2 * 128 + 255) / 256, 256, 0, st>>>(W, C::KSTEPS, wsplit);
     }
     // the col / ew slices are staged with bulk copies, which only need 4-byte aligned slices (the aligned superset is copied)
     if (lw.cap > 0)
-        sage_layer_umma_kernel<F, NS, RP, true><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit);
+        sage_layer_umma_kernel<F, NS, RP, true><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit, l2_policy);
     else
-        sage_layer_umma_kernel<F, NS, RP, false><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit);
+        sage_layer_umma_kernel<F, NS, RP, false><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit, l2_policy);
     return launch_status("sage_layer_umma_kernel");
 }
 
@@ -1251,7 +1264,8 @@ int launch_umma(const float* x, const RP* rowptr, const int32_t* col, const floa
 int sage_layer_umma(const float* x, const void* rowptr, int is64, const int32_t* col, const float* ew, const float* W,
                     const float* b, float* out, int64_t n_nodes, int64_t row_begin, int64_t row_end, int F, int relu,
                     int nsplit, const float* node_w, float node_b, float* score, void* long_ws, size_t long_ws_bytes,
-                    bool reuse_scan, float* const* peer_out, int n_peers, const uint8_t* peer_need, cudaStream_t st) {
+                    bool reuse_scan, float* const* peer_out, int n_peers, const uint8_t* peer_need, int l2_policy,
+                    cudaStream_t st) {
     (void)n_nodes;
     Peers peers{};
     peers.need = peer_need;
@@ -1263,8 +1277,8 @@ int sage_layer_umma(const float* x, const void* rowptr, int is64, const int32_t*
         peers.n = n_peers;
     }
 #define GO(FV, NSV)                                                                                                                                                                               \
-    return is64 ? launch_umma<FV, NSV, int64_t>(x, (const int64_t*)rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, long_ws, long_ws_bytes, reuse_scan, peers, st) \
-                : launch_umma<FV, NSV, int32_t>(x, (const int32_t*)rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, long_ws, long_ws_bytes, reuse_scan, peers, st)
+    return is64 ? launch_umma<FV, NSV, int64_t>(x, (const int64_t*)rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, long_ws, long_ws_bytes, reuse_scan, peers, l2_policy, st) \
+                : launch_umma<FV, NSV, int32_t>(x, (const int32_t*)rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, long_ws, long_ws_bytes, reuse_scan, peers, l2_policy, st)
     if (nsplit == 3) {
         switch (F) {
             case 32: GO(32, 3);
