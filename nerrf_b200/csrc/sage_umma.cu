@@ -7,7 +7,8 @@
 //   D^T[H=128 features, rows] = W^T[128, K=2F] . X^T[K, rows]      (one m64n32k16 wgmma half per consumer warpgroup)
 //     A operand = W^T, register fragments split into bf16 terms once per launch and read from L2 by the consumer
 //                 warpgroups: the split W^T of an F=128 layer (192 KB) does not fit in shared memory next to the gather
-//                 rings and operand stages, and Hopper has no tensor memory to hold it
+//                 rings and operand stages, and Hopper has no tensor memory to hold it.  F = 32: all of the split W^T
+//                 (48 registers per thread at NS = 3) is loaded once per CTA and stays in the consumers' registers
 //     F = 64 / 128: the self half x_v . W[0:F] needs no gather; a prep kernel (sage_self_prep_kernel) computes it over
 //                 contiguous rows of x with W resident in registers and stores the raw accumulators in out, and the
 //                 layer kernel starts from them and runs only the mean half (K = F), which halves its weight traffic.
@@ -32,8 +33,9 @@
 //   warps 9-..  gather: one CSR row per warp at a time (four at F=32), rows round-robin; source rows are copied into the
 //               warp's shared-memory ring with cp.async (LDGSTS, 16 B per lane), NQ-1 sub-batches in flight;
 //               indices come from shared memory, so the only global latency a row exposes is its x rows
-//   warp  23    (F = 64 / 128) spare: completes the sixth warpgroup, so that setmaxnreg can give the consumer warpgroups
-//               128 registers per thread and the four producer warpgroups (loader, gather, spare) 56
+//   warp  23    F = 64 / 128: spare, completes the sixth warpgroup, so that setmaxnreg can give the consumer warpgroups
+//               128 registers per thread and the four producer warpgroups (loader, gather, spare) 56.  F = 32: the 15th
+//               gather warp; the consumers get 112 registers per thread, the producers 64
 // Pipelines: idx stages full/empty (loader <-> gather), smem operand stages full/empty (gather <-> consumer).
 #include <map>
 #include <mutex>
@@ -63,16 +65,16 @@ constexpr int NQ = 4;                  // sub-batch slots in a warp's ring; NQ-1
 // terms below 2^-24: fp32-equivalent.  NS = 2 with three products is ~1e-5 relative.
 template <int F, int NS>
 struct UmmaCfg {
-    static constexpr int GATHER_WARPS = (F == 32) ? 16 : 14;  // F=32 leaves room for more rings (and needs more TLP);
-                                                                // 25 warps keep 80 registers per thread
-    // F = 64 / 128: the CTA is six whole warpgroups (one spare warp after the gather warps), so that setmaxnreg can move
-    // registers from the four producer warpgroups (loader, gather, spare) to the two consumer warpgroups, which hold two
-    // tiles' accumulators: 768 threads x 80 = 2 x 128 x CONSUMER_REGS + 4 x 128 x PRODUCER_REGS
-    static constexpr int WARPS = (F == 32) ? GATHER_WARP0 + GATHER_WARPS : 24;
+    static constexpr int GATHER_WARPS = (F == 32) ? 15 : 14;  // F=32 leaves room for more rings (and needs more TLP)
+    // The CTA is six whole warpgroups (F = 64 / 128: one spare warp after the gather warps), so that setmaxnreg can move
+    // registers from the four producer warpgroups (loader, gather, spare) to the two consumer warpgroups: 768 threads x 80
+    // = 2 x 128 x CONSUMER_REGS + 4 x 128 x PRODUCER_REGS.  F = 64 / 128: the consumers hold two tiles' accumulators;
+    // F = 32: all of the split W^T (KSTEPS x NS x 4 = 48 registers at NS = 3)
+    static constexpr int WARPS = 24;
     static constexpr int THREADS = WARPS * 32;
-    static constexpr int CONSUMER_REGS = 128, PRODUCER_REGS = 56;
-    static_assert(F == 32 || (WARPS % 4 == 0 && WARPS >= GATHER_WARP0 + GATHER_WARPS &&
-                              (EPI_WARPS * CONSUMER_REGS + (WARPS - EPI_WARPS) * PRODUCER_REGS) * 32 <= THREADS * 80),
+    static constexpr int CONSUMER_REGS = (F == 32) ? 112 : 128, PRODUCER_REGS = (F == 32) ? 64 : 56;
+    static_assert(WARPS % 4 == 0 && WARPS >= GATHER_WARP0 + GATHER_WARPS &&
+                  (EPI_WARPS * CONSUMER_REGS + (WARPS - EPI_WARPS) * PRODUCER_REGS) * 32 <= THREADS * 80,
                   "register budget: 80 registers per thread at launch");
     // F = 32 (quad-mode gather): a warp runs up to 3 units = ~7 tiles ahead of what it has consumed and holds a tile's edge
     // block from issue to completion, so the look-ahead is bounded by the number of edge-block stages, not by the rings
@@ -89,7 +91,7 @@ struct UmmaCfg {
     static constexpr int STAGE_BYTES = NS * PART_BYTES;
     static constexpr int QS = qs_for<F>();                    // 4 (F=128), 8 (F=64), 16 (F=32): always 2 KB per sub-batch
     static constexpr int RING_BYTES = NQ * QS * F * 4;       // per gather warp: NQ sub-batches x QS source rows
-    static constexpr int STAGES = (F == 32) ? 3 : 4;
+    static constexpr int STAGES = 4;
     static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + IDX_STAGES * IDX_STAGE_BYTES +
                                    (size_t)GATHER_WARPS * RING_BYTES + 2048 /*head reduce*/ + 1024 /*align*/ + 1024 /*barriers*/;
     static_assert(SMEM <= 227 * 1024, "shared memory budget");
@@ -103,6 +105,21 @@ __device__ __forceinline__ void split4(const float4 v, uint2 (&parts)[NS]) {
     split_pair<NS>(v.z, v.w, hi);
 #pragma unroll
     for (int p = 0; p < NS; ++p) parts[p] = make_uint2(lo[p], hi[p]);
+}
+
+// the products of one K step over the split terms (a = W^T terms, xb = descriptors of the x terms), in the fixed order
+// x0w0, x1w0, x0w1 [, x1w1, x2w0, x0w2]; scale_d 0 on the first product starts the accumulator
+template <int NS>
+__device__ __forceinline__ void wgmma_split_products(float (&d)[16], const uint32_t (&a)[NS][4], const uint64_t (&xb)[NS],
+                                                     uint32_t scale_d) {
+    wgmma_rs(d, a[0], xb[0], scale_d);
+    wgmma_rs(d, a[0], xb[1], 1u);
+    wgmma_rs(d, a[1], xb[0], 1u);
+    if constexpr (NS == 3) {
+        wgmma_rs(d, a[1], xb[1], 1u);
+        wgmma_rs(d, a[0], xb[2], 1u);
+        wgmma_rs(d, a[2], xb[0], 1u);
+    }
 }
 
 // ---------------------------------------------------------------- fused exchange (multi-GPU)
@@ -309,6 +326,8 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
         constexpr int UPT = TN / 4;                                       // units (4 rows) per tile
         constexpr int SLOT_BYTES = 4 * 4 * F * 4;                         // a sub-batch = 4 steps x 4 rows x 128 B = 2 KB
         static_assert(SLOT_BYTES * NQ == C::RING_BYTES, "ring layout");
+        static_assert(C::WARPS == GATHER_WARP0 + GATHER_WARPS, "every warp after the loader gathers");
+        setmaxnreg_dec<C::PRODUCER_REGS>();
         const int g = warp - GATHER_WARP0;
         const int grp = lane >> 3, sub = lane & 7;
         // ring slot layout [step][group][8 lanes x 16 B] = lane-linear: conflict-free 16-byte shared loads
@@ -751,7 +770,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
       }
     } else if (warp == LOADER_WARP) {
         // =========================================================== edge-block loader
-        if constexpr (C::SELF_SPLIT) setmaxnreg_dec<C::PRODUCER_REGS>();
+        setmaxnreg_dec<C::PRODUCER_REGS>();
         constexpr int RPW = (TN + 1 + 31) / 32;
         auto load_rp = [&](int64_t tile, int64_t (&rp)[RPW]) {          // rowptr[row0 .. row0+TN], clamped to row_end
             const int64_t row0 = row_begin + tile * TN;
@@ -840,18 +859,13 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
         }
     } else if (warp < EPI_WARPS) {
         // =========================================================== consumer warpgroups: wgmma + epilogue
-        if constexpr (C::SELF_SPLIT) setmaxnreg_inc<C::CONSUMER_REGS>();
+        setmaxnreg_inc<C::CONSUMER_REGS>();
         // Warpgroup h computes output features [64 h, 64 h + 64).  Its accumulator row m = 16 wq + i (warp wq of the
         // warpgroup, i < 16) is feature 64 h + 16 wq + 2 (i & 7) + (i >> 3): a thread's two rows are two CONSECUTIVE
         // features f0, f0 + 1, so its outputs are 8-byte stores and a warp writes 64 contiguous bytes of a row.  The
         // accumulator register d[4 nb + 2 b + e] of thread (wq, lane = 4 g + c) holds feature f0 + b of tile row
-        // 8 nb + 2 c + e.  The A fragments (W^T terms) come pre-split from `wsplit` (the prep kernel), 16 bytes per
-        // thread, term and K step, from L2.  They are the same for every tile, so their loads run AHEAD K steps ahead of
-        // the MMAs across tile boundaries: an L2 round trip under the gather's load is longer than one K step of one tile.
-        // With tile pairs (below) a K step issues twice the MMAs, so one step ahead covers as long as two did for a single
-        // tile, and the 12 registers of a second fragment set (NS = 3) go to the second tile's accumulators.
-        constexpr int TP = C::SELF_SPLIT ? 2 : 1;                             // tiles per pass
-        constexpr int AHEAD = 3 - TP;                                         // K steps the fragment loads run ahead
+        // 8 nb + 2 c + e.  The A fragments (W^T terms) come pre-split from `wsplit` (the prep kernel; F = 32:
+        // split_w_kernel), 16 bytes per thread, term and K step.
         const int h = warp >> 2, wq = warp & 3, et = tid & 127;
         const int g = lane >> 2, c = lane & 3;
         const int f0 = 64 * h + 16 * wq + 2 * g;
@@ -865,31 +879,6 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                 a[p][0] = v.x; a[p][1] = v.y; a[p][2] = v.z; a[p][3] = v.w;
             }
         };
-        auto copy_a = [](uint32_t (&dst)[NS][4], const uint32_t (&src)[NS][4]) {
-#pragma unroll
-            for (int p = 0; p < NS; ++p)
-#pragma unroll
-                for (int r = 0; r < 4; ++r) dst[p][r] = src[p][r];
-        };
-        uint32_t a_n[AHEAD][NS][4];                                           // fragments of the next AHEAD K steps
-#pragma unroll
-        for (int i = 0; i < AHEAD; ++i) load_a(i, a_n[i]);
-        // F = 64 / 128: the accumulators start from the prep kernel's self terms (the first F/16 K steps), stored raw in
-        // out -- the local buffer: peers and the multicast address never hold this rank's self terms.
-        // TILE PAIRS (F = 64 / 128): a warpgroup takes the CTA's tiles two at a time (operand stages tl and tl + 1) and
-        // issues each K step's products for both tiles from ONE fragment load into two independent accumulator sets: half
-        // the fragment traffic and half the K-step waits per row, and two MMA chains the tensor pipe can overlap.  Each
-        // tile runs the same wgmma sequence as it would alone, so its outputs do not depend on its partner.  A closing entry
-        // (-1) in the second slot ends the stream: that pass stores only the first tile (the products over the closing
-        // stage are discarded).  F = 32 takes one tile per pass.
-        // The epilogue of a pass already loads the next pass's self terms into d when the loader has published those tiles'
-        // ids: the ids of a CTA's tiles increase, so a ring entry greater than the pass's last tile is a later tile's, not
-        // a stale one.
-        static_assert(C::STAGES % TP == 0 && C::STAGES >= 2 * TP, "operand stages per pass");
-        float d[TP][16];
-        int s_tile[TP];                                                       // tile whose self terms d[u] holds
-#pragma unroll
-        for (int u = 0; u < TP; ++u) s_tile[u] = -1;
         auto self_terms = [&](int64_t t, int nb, int e) -> float2 {           // (row 8 nb + 2 c + e of tile t, f0)
             const int64_t row = row_begin + t * TN + 8 * nb + 2 * c + e;
             return row < row_end ? ld_nc_na_hint(reinterpret_cast<const float2*>(out + row * UM + f0), pol()) : make_float2(0.f, 0.f);
@@ -898,99 +887,52 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
             mbar_wait_relaxed(full_bar((int)(t % C::STAGES)), (uint32_t)(t / C::STAGES) & 1u);
             return tile_ids[t % TILE_RING];
         };
-        for (int64_t tl = 0;; tl += TP) {
-            const int s0 = (int)(tl % C::STAGES);                             // stages s0 .. s0 + TP - 1
-            int tile[TP];
-            tile[0] = wait_full(tl);
-            if (tile[0] < 0) break;                                           // closing entry: end of stream
-            if constexpr (TP == 2) tile[1] = wait_full(tl + 1);               // (-1: the closing entry)
-            if constexpr (C::SELF_SPLIT) {
+        if constexpr (QUAD) {
+            // F = 32: all of the split W^T (K = 2F: KSTEPS x NS fragments, 48 registers at NS = 3) is loaded once and stays
+            // in registers, so no fragment register is ever redefined while a wgmma runs and a tile is all its products in
+            // ONE commit group with one wait -- the same instructions on the same registers in the same order (scale-d 0 on
+            // the first only) as one K step at a time, hence the same bits.
+            uint32_t a[C::KSTEPS][NS][4];
 #pragma unroll
-                for (int u = 0; u < TP; ++u) {
-                    if (tile[u] >= 0 && tile[u] != s_tile[u]) {
-#pragma unroll
-                        for (int nb = 0; nb < 4; ++nb)
-#pragma unroll
-                            for (int e = 0; e < 2; ++e) {
-                                const float2 sv = self_terms(tile[u], nb, e);
-                                d[u][4 * nb + e] = sv.x; d[u][4 * nb + 2 + e] = sv.y;
-                            }
-                    }
-                }
-            }
-            auto mma_step = [&](int j, const uint32_t (&a)[NS][4]) {
-                const uint32_t boff = (uint32_t)((j >> 2) * (TN * 128) + (j & 3) * 32);
+            for (int j = 0; j < C::KSTEPS; ++j) load_a(j, a[j]);
+            float d[16];
+            for (int64_t tl = 0;; ++tl) {
+                const int tile = wait_full(tl);
+                if (tile < 0) break;                                          // closing entry: end of stream
+                const int s = (int)(tl % C::STAGES);
+                const uint32_t st0 = smem_base + (uint32_t)(s * C::STAGE_BYTES);
                 wgmma_fence();
 #pragma unroll
-                for (int u = 0; u < TP; ++u) {
-                    const uint32_t st0 = smem_base + (uint32_t)((s0 + u) * C::STAGE_BYTES);
+                for (int j = 0; j < C::KSTEPS; ++j) {
+                    const uint32_t boff = (uint32_t)((j >> 2) * (TN * 128) + (j & 3) * 32);
                     uint64_t xb[NS];
 #pragma unroll
                     for (int p = 0; p < NS; ++p) xb[p] = make_b_desc(st0 + (uint32_t)(p * C::PART_BYTES) + boff);   // x term p
-                    wgmma_rs(d[u], a[0], xb[0], (C::SELF_SPLIT || j > 0) ? 1u : 0u);
-                    wgmma_rs(d[u], a[0], xb[1], 1u);
-                    wgmma_rs(d[u], a[1], xb[0], 1u);
-                    if constexpr (NS == 3) {
-                        wgmma_rs(d[u], a[1], xb[1], 1u);
-                        wgmma_rs(d[u], a[0], xb[2], 1u);
-                        wgmma_rs(d[u], a[2], xb[0], 1u);
-                    }
+                    wgmma_split_products<NS>(d, a[j], xb, j > 0 ? 1u : 0u);
                 }
                 wgmma_commit();
-            };
-            // (registers a running wgmma reads must not be written before it retires, and ptxas serializes the MMAs of a
-            // step when any wgmma input is written while one is in flight: the next fragments are loaded before the step)
-#pragma unroll 1
-            for (int j = 0; j < C::KSTEPS; ++j) {
-                uint32_t a_cur[NS][4];
-                copy_a(a_cur, a_n[0]);
-#pragma unroll
-                for (int i = 0; i + 1 < AHEAD; ++i) copy_a(a_n[i], a_n[i + 1]);
-                load_a(j + AHEAD < C::KSTEPS ? j + AHEAD : j + AHEAD - C::KSTEPS, a_n[AHEAD - 1]);   // K >= 64: >= 4 K steps
-                mma_step(j, a_cur);
                 wgmma_wait_all();
-            }
-            __syncwarp();
-            if (lane == 0) {
-#pragma unroll
-                for (int u = 0; u < TP; ++u) mbar_arrive(empty_bar(s0 + u));  // this warp's MMAs no longer read the stages
-            }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty_bar(s));                     // this warp's MMAs no longer read the stage
 
-            // ---- epilogue, per tile: + bias, ReLU, one 8-byte store per (row, thread)
-            int s_next[TP];
-#pragma unroll
-            for (int u = 0; u < TP; ++u) {
-                s_next[u] = -1;
-                if constexpr (C::SELF_SPLIT) {
-                    const int nx = tile_ids[(tl + TP + u) % TILE_RING];
-                    if (tile[TP - 1] >= 0 && nx > tile[TP - 1]) s_next[u] = nx;
-                }
-            }
-#pragma unroll
-            for (int u = 0; u < TP; ++u) {
-                if (tile[u] < 0) break;                                       // the closing entry in the second slot
-                const int64_t row0 = row_begin + (int64_t)tile[u] * TN;
+                // ---- epilogue: + bias, ReLU, one 8-byte store per (row, thread), the fused node head (as below)
+                const int64_t row0 = row_begin + (int64_t)tile * TN;
                 float part[8];
 #pragma unroll
                 for (int nb = 0; nb < 4; ++nb) {
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
-                        float2 o = make_float2(d[u][4 * nb + e] + b2.x, d[u][4 * nb + 2 + e] + b2.y);
-                        if (C::SELF_SPLIT && s_next[u] >= 0) {
-                            const float2 sv = self_terms(s_next[u], nb, e);
-                            d[u][4 * nb + e] = sv.x; d[u][4 * nb + 2 + e] = sv.y;
-                        }
+                        float2 o = make_float2(d[4 * nb + e] + b2.x, d[4 * nb + 2 + e] + b2.y);
                         if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
                         part[2 * nb + e] = o.x * nw2.x + o.y * nw2.y;
                         const int64_t row = row0 + 8 * nb + 2 * c + e;
                         if (row < row_end) {
                             const int64_t off = row * UM + f0;
-                            if (peers.mc) {                                   // NVSwitch multicast: every rank's buffer at once
+                            if (peers.mc) {
                                 multimem_st2(peers.mc + off, o);
                             } else {
-                                if constexpr (QUAD) *reinterpret_cast<float2*>(out + off) = o;
-                                else st_hint(reinterpret_cast<float2*>(out + off), o, pol());
-                                if (peers.n) {                                // fused exchange over NVLink
+                                *reinterpret_cast<float2*>(out + off) = o;
+                                if (peers.n) {
                                     const unsigned need = peers.need ? (unsigned)__ldg(peers.need + row) : 0xFFu;
 #pragma unroll
                                     for (int pr = 0; pr < MAX_PEERS; ++pr)
@@ -1000,18 +942,14 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                         }
                     }
                 }
-                s_tile[u] = s_next[u];
                 if (node_w) {
-                    // fused node head: score[row] = sigmoid(h[row,:] . node_w + node_b); a warp's 16 features summed over g.
-                    // The halves of head_red alternate by tile (the first and second tile of a pass); warp 0 reads a half
-                    // before it reaches the next tile's barrier, which orders that read before the half is written again.
 #pragma unroll
                     for (int i = 0; i < 8; ++i) {
                         part[i] += __shfl_xor_sync(0xffffffffu, part[i], 4);
                         part[i] += __shfl_xor_sync(0xffffffffu, part[i], 8);
                         part[i] += __shfl_xor_sync(0xffffffffu, part[i], 16);
                     }
-                    const int half = (int)((tl + u) & 1);
+                    const int half = (int)(tl & 1);
                     float* hb = head_red + (half * EPI_WARPS + warp) * 32;
                     if (g == 0) {
 #pragma unroll
@@ -1025,7 +963,161 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                     }
                 }
             }
-            if (tile[TP - 1] < 0) break;                                      // the pass held the closing entry
+        } else {
+            // F = 64 / 128: the fragments are re-read from L2 for every pass (the split W^T of an F = 128 layer would take 96
+            // registers per thread).  They are the same for every tile, so their loads run AHEAD K steps ahead of the MMAs
+            // across tile boundaries: an L2 round trip under the gather's load is longer than one K step of one tile.  With
+            // tile pairs (below) a K step issues twice the MMAs, so one step ahead covers as long as two did for a single
+            // tile, and the 12 registers of a second fragment set (NS = 3) go to the second tile's accumulators.
+            constexpr int TP = C::SELF_SPLIT ? 2 : 1;                             // tiles per pass
+            constexpr int AHEAD = 3 - TP;                                         // K steps the fragment loads run ahead
+            auto copy_a = [](uint32_t (&dst)[NS][4], const uint32_t (&src)[NS][4]) {
+#pragma unroll
+                for (int p = 0; p < NS; ++p)
+#pragma unroll
+                    for (int r = 0; r < 4; ++r) dst[p][r] = src[p][r];
+            };
+            uint32_t a_n[AHEAD][NS][4];                                           // fragments of the next AHEAD K steps
+#pragma unroll
+            for (int i = 0; i < AHEAD; ++i) load_a(i, a_n[i]);
+            // The accumulators start from the prep kernel's self terms (the first F/16 K steps), stored raw in out -- the
+            // local buffer: peers and the multicast address never hold this rank's self terms.
+            // TILE PAIRS: a warpgroup takes the CTA's tiles two at a time (operand stages tl and tl + 1) and issues each K
+            // step's products for both tiles from ONE fragment load into two independent accumulator sets: half the fragment
+            // traffic and half the K-step waits per row, and two MMA chains the tensor pipe can overlap.  Each tile runs the
+            // same wgmma sequence as it would alone, so its outputs do not depend on its partner.  A closing entry (-1) in the
+            // second slot ends the stream: that pass stores only the first tile (the products over the closing stage are
+            // discarded).
+            // The epilogue of a pass already loads the next pass's self terms into d when the loader has published those
+            // tiles' ids: the ids of a CTA's tiles increase, so a ring entry greater than the pass's last tile is a later
+            // tile's, not a stale one.
+            static_assert(C::STAGES % TP == 0 && C::STAGES >= 2 * TP, "operand stages per pass");
+            float d[TP][16];
+            int s_tile[TP];                                                       // tile whose self terms d[u] holds
+#pragma unroll
+            for (int u = 0; u < TP; ++u) s_tile[u] = -1;
+            for (int64_t tl = 0;; tl += TP) {
+                const int s0 = (int)(tl % C::STAGES);                             // stages s0 .. s0 + TP - 1
+                int tile[TP];
+                tile[0] = wait_full(tl);
+                if (tile[0] < 0) break;                                           // closing entry: end of stream
+                if constexpr (TP == 2) tile[1] = wait_full(tl + 1);               // (-1: the closing entry)
+                if constexpr (C::SELF_SPLIT) {
+#pragma unroll
+                    for (int u = 0; u < TP; ++u) {
+                        if (tile[u] >= 0 && tile[u] != s_tile[u]) {
+#pragma unroll
+                            for (int nb = 0; nb < 4; ++nb)
+#pragma unroll
+                                for (int e = 0; e < 2; ++e) {
+                                    const float2 sv = self_terms(tile[u], nb, e);
+                                    d[u][4 * nb + e] = sv.x; d[u][4 * nb + 2 + e] = sv.y;
+                                }
+                        }
+                    }
+                }
+                auto mma_step = [&](int j, const uint32_t (&a)[NS][4]) {
+                    const uint32_t boff = (uint32_t)((j >> 2) * (TN * 128) + (j & 3) * 32);
+                    wgmma_fence();
+#pragma unroll
+                    for (int u = 0; u < TP; ++u) {
+                        const uint32_t st0 = smem_base + (uint32_t)((s0 + u) * C::STAGE_BYTES);
+                        uint64_t xb[NS];
+#pragma unroll
+                        for (int p = 0; p < NS; ++p) xb[p] = make_b_desc(st0 + (uint32_t)(p * C::PART_BYTES) + boff);   // x term p
+                        wgmma_split_products<NS>(d[u], a, xb, 1u);                  // (the self terms start d)
+                    }
+                    wgmma_commit();
+                };
+                // (registers a running wgmma reads must not be written before it retires, and ptxas serializes the MMAs of a
+                // step when any wgmma input is written while one is in flight: the next fragments are loaded before the step)
+    #pragma unroll 1
+                for (int j = 0; j < C::KSTEPS; ++j) {
+                    uint32_t a_cur[NS][4];
+                    copy_a(a_cur, a_n[0]);
+#pragma unroll
+                    for (int i = 0; i + 1 < AHEAD; ++i) copy_a(a_n[i], a_n[i + 1]);
+                    load_a(j + AHEAD < C::KSTEPS ? j + AHEAD : j + AHEAD - C::KSTEPS, a_n[AHEAD - 1]);   // K >= 64: >= 4 K steps
+                    mma_step(j, a_cur);
+                    wgmma_wait_all();
+                }
+                __syncwarp();
+                if (lane == 0) {
+#pragma unroll
+                    for (int u = 0; u < TP; ++u) mbar_arrive(empty_bar(s0 + u));  // this warp's MMAs no longer read the stages
+                }
+
+                // ---- epilogue, per tile: + bias, ReLU, one 8-byte store per (row, thread)
+                int s_next[TP];
+#pragma unroll
+                for (int u = 0; u < TP; ++u) {
+                    s_next[u] = -1;
+                    if constexpr (C::SELF_SPLIT) {
+                        const int nx = tile_ids[(tl + TP + u) % TILE_RING];
+                        if (tile[TP - 1] >= 0 && nx > tile[TP - 1]) s_next[u] = nx;
+                    }
+                }
+#pragma unroll
+                for (int u = 0; u < TP; ++u) {
+                    if (tile[u] < 0) break;                                       // the closing entry in the second slot
+                    const int64_t row0 = row_begin + (int64_t)tile[u] * TN;
+                    float part[8];
+#pragma unroll
+                    for (int nb = 0; nb < 4; ++nb) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            float2 o = make_float2(d[u][4 * nb + e] + b2.x, d[u][4 * nb + 2 + e] + b2.y);
+                            if (C::SELF_SPLIT && s_next[u] >= 0) {
+                                const float2 sv = self_terms(s_next[u], nb, e);
+                                d[u][4 * nb + e] = sv.x; d[u][4 * nb + 2 + e] = sv.y;
+                            }
+                            if (relu) { o.x = fmaxf(o.x, 0.f); o.y = fmaxf(o.y, 0.f); }
+                            part[2 * nb + e] = o.x * nw2.x + o.y * nw2.y;
+                            const int64_t row = row0 + 8 * nb + 2 * c + e;
+                            if (row < row_end) {
+                                const int64_t off = row * UM + f0;
+                                if (peers.mc) {                                   // NVSwitch multicast: every rank's buffer at once
+                                    multimem_st2(peers.mc + off, o);
+                                } else {
+                                    if constexpr (QUAD) *reinterpret_cast<float2*>(out + off) = o;
+                                    else st_hint(reinterpret_cast<float2*>(out + off), o, pol());
+                                    if (peers.n) {                                // fused exchange over NVLink
+                                        const unsigned need = peers.need ? (unsigned)__ldg(peers.need + row) : 0xFFu;
+#pragma unroll
+                                        for (int pr = 0; pr < MAX_PEERS; ++pr)
+                                            if (pr < peers.n && ((need >> pr) & 1u)) *reinterpret_cast<float2*>(peers.out[pr] + off) = o;
+                                    }
+                                }
+                            }
+                        }
+                    }
+                    s_tile[u] = s_next[u];
+                    if (node_w) {
+                        // fused node head: score[row] = sigmoid(h[row,:] . node_w + node_b); a warp's 16 features summed over g.
+                        // The halves of head_red alternate by tile (the first and second tile of a pass); warp 0 reads a half
+                        // before it reaches the next tile's barrier, which orders that read before the half is written again.
+#pragma unroll
+                        for (int i = 0; i < 8; ++i) {
+                            part[i] += __shfl_xor_sync(0xffffffffu, part[i], 4);
+                            part[i] += __shfl_xor_sync(0xffffffffu, part[i], 8);
+                            part[i] += __shfl_xor_sync(0xffffffffu, part[i], 16);
+                        }
+                        const int half = (int)((tl + u) & 1);
+                        float* hb = head_red + (half * EPI_WARPS + warp) * 32;
+                        if (g == 0) {
+#pragma unroll
+                            for (int nb = 0; nb < 4; ++nb) { hb[8 * nb + 2 * c] = part[2 * nb]; hb[8 * nb + 2 * c + 1] = part[2 * nb + 1]; }
+                        }
+                        named_bar(1, 256);                                       // the eight consumer warps
+                        if (warp == 0) {
+                            const float* hr = head_red + half * EPI_WARPS * 32 + lane;
+                            const float dot = ((hr[0] + hr[32]) + (hr[64] + hr[96])) + ((hr[128] + hr[160]) + (hr[192] + hr[224]));
+                            if (row0 + lane < row_end) score[row0 + lane] = 1.f / (1.f + expf(-(dot + node_b)));
+                        }
+                    }
+                }
+                if (tile[TP - 1] < 0) break;                                      // the pass held the closing entry
+            }
         }
     }
 }
@@ -1152,14 +1244,7 @@ sage_self_prep_kernel(const float* __restrict__ x, const float* __restrict__ W, 
                 uint64_t xb[NS];
 #pragma unroll
                 for (int p = 0; p < NS; ++p) xb[p] = make_b_desc(base + (uint32_t)(sl * P::SLICE_BYTES + p * P::PART_BYTES) + boff);
-                wgmma_rs(d[sl], a[j][0], xb[0], j > 0 ? 1u : 0u);
-                wgmma_rs(d[sl], a[j][0], xb[1], 1u);
-                wgmma_rs(d[sl], a[j][1], xb[0], 1u);
-                if constexpr (NS == 3) {
-                    wgmma_rs(d[sl], a[j][1], xb[1], 1u);
-                    wgmma_rs(d[sl], a[j][0], xb[2], 1u);
-                    wgmma_rs(d[sl], a[j][2], xb[0], 1u);
-                }
+                wgmma_split_products<NS>(d[sl], a[j], xb, j > 0 ? 1u : 0u);
             }
         }
         wgmma_commit();
