@@ -363,6 +363,62 @@ int nerrf_trace_decode(const uint8_t* buf, int64_t len, int64_t n_events,
  * applies to `path`, available for `new_path` (a rename target names the file from then on). */
 int nerrf_trace_path_flags(const int64_t* off, const uint8_t* data, int64_t n, uint8_t* flags_out);
 
+/* Top-level framing of an EventBatch byte stream (HOST code), the walk of nerrf_trace_decode without parsing the
+ * Events: for every Event record (field 1) rec_at = byte offset of its tag, body_off / body_len = its body; any other
+ * top-level field is skipped by its wire type.  The first min(n, max_records) records are written and *n_records = n
+ * (call again with a larger array when n > max_records).  *consumed = bytes covered by whole records.  partial != 0: a
+ * trailing record that is merely cut off is left out of `consumed` (the caller carries it over to the next chunk);
+ * partial == 0 or anything else malformed -> NERRF_ERR_INVALID, "malformed EventBatch at byte offset N", with the
+ * outputs describing the records before N (an Event body is not checked here: nerrf_trace_decode_device does that). */
+int nerrf_trace_frame(const uint8_t* buf, int64_t len, int partial, int64_t max_records, int64_t* rec_at,
+                      int64_t* body_off, int64_t* body_len, int64_t* n_records, int64_t* consumed);
+
+/* ------------------------------------------------------------------ live stream: EventBatch records decoded and
+ * appended ON THE DEVICE (csrc/live_stream.cu; nerrf_b200/stream.py DeviceStream.live).
+ * Columns are passed as a host array `cols` of 17 device pointers in the argument order of nerrf_trace_decode:
+ * ts_sec, ts_nanos, pid, tid, flags, ret_val, bytes, event_slot, path_flags, comm_off, comm_data, syscall_off,
+ * syscall_data, path_off, path_data, new_path_off, new_path_data.
+ *
+ * nerrf_trace_decode_device: the n_records records framed by nerrf_trace_frame (rec_at / body_off / body_len, device
+ * copies; offsets into `buf`, the wire bytes on the device) are parsed by the host decoder's rules and written at rows
+ * n_old .. n_old + n_records - 1; string offsets continue from off[n_old], so every data array needs room for
+ * off[n_old] + the records' body bytes (which must stay below 2^31).  *status (device) = the smallest rec_at of a
+ * malformed record, or all ones when every record parsed: the rows are only valid then.  Asynchronous on `stream`.
+ * workspace: 256-byte aligned, nerrf_trace_decode_device_workspace_bytes. */
+int nerrf_trace_decode_device_workspace_bytes(int64_t n_records, int64_t* bytes);
+int nerrf_trace_decode_device(const uint8_t* buf, const int64_t* rec_at, const int64_t* body_off, const int64_t* body_len,
+                              int64_t n_records, int64_t n_old, void* const* cols, uint64_t* status, void* workspace,
+                              int64_t workspace_bytes, void* stream);
+/* Time order, path resolution and retention of n_events resident events (device arrays):
+ *   ts_out [n] = ts_sec + ts_nanos * 1e-9 in float64 (numpy's two roundings);
+ *   src_out [n] = stored index of the event whose path the event uses: itself when its path is non-empty, else the pid's
+ *     most recent event with a path in stable time order, or -1 (dropped) -- nerrf_b200/ingest.py resolve_columns;
+ *   order_out [n_keep] = the surviving events in stable time order, ts_sorted_out [n_keep] their timestamps;
+ *   res_path_off [n+1] = offsets of the resolved path column (dropped events: empty);
+ *   retain_out [n_retain] (may be NULL) = in stored order, the events with ts > horizon and, per pid, its latest event
+ *     with a path at or before the horizon (a later path-less write still resolves to it).
+ * counts (HOST [3]) = n_keep, n_retain, total bytes of the resolved path column; the call synchronises the stream.
+ * workspace: 256-byte aligned, nerrf_trace_stream_order_workspace_bytes. */
+int nerrf_trace_stream_order_workspace_bytes(int64_t n_events, int64_t* bytes);
+int nerrf_trace_stream_order(int64_t n_events, const int64_t* ts_sec, const int32_t* ts_nanos, const uint32_t* pid,
+                             const int64_t* path_off, double horizon, double* ts_out, int64_t* order_out,
+                             double* ts_sorted_out, int64_t* src_out, int64_t* res_path_off, int64_t* retain_out,
+                             int64_t* counts, void* workspace, int64_t workspace_bytes, void* stream);
+/* The per-event columns the window graph reads, from src_out / res_path_off of nerrf_trace_stream_order: the resolved
+ * path bytes (res_path_data), pf_raw_out = path_flags of the source event, pf_out = the same OR the NERRF_PATH_LOCKBIT bit
+ * of new_path when merge_renames, slot_out = slot_map[event_slot] (slot_map: device uint8 [8], NULL = identity).
+ * Asynchronous on `stream`. */
+int nerrf_trace_stream_columns(int64_t n_events, const int64_t* src, const int64_t* path_off, const uint8_t* path_data,
+                               const uint8_t* path_flags, const int64_t* new_path_off, const uint8_t* new_path_data,
+                               const uint8_t* event_slot, const uint8_t* slot_map, const int64_t* res_path_off,
+                               int merge_renames, uint8_t* res_path_data, uint8_t* pf_out, uint8_t* pf_raw_out,
+                               uint8_t* slot_out, void* stream);
+/* cols_out row k = cols_in row rows[k] (device int64 [n_rows], distinct rows, so every output data array fits in the
+ * input's size); string offsets restart at 0.  Asynchronous; workspace from nerrf_trace_gather_rows_workspace_bytes. */
+int nerrf_trace_gather_rows_workspace_bytes(int64_t n_rows, int64_t* bytes);
+int nerrf_trace_gather_rows(void* const* cols_in, const int64_t* rows, int64_t n_rows, void* const* cols_out,
+                            void* workspace, int64_t workspace_bytes, void* stream);
+
 /* The same interning ON THE DEVICE ("inode/path dedup via hash", SURVEY.md 8f rank 1; architecture.mdx:39-41): identical
  * nodes, numbering and names for the same events in the same processing order, computed by data-parallel passes (64-bit
  * hash + open-addressing table with first-mention atomicMin, rename-alias forest, creating-mention scan).  All array

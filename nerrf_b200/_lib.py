@@ -82,7 +82,16 @@ SIGNATURES = {
     "nerrf_trace_scan": (C.c_int, [vp, C.c_int64, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "nerrf_trace_decode": (C.c_int, [vp, C.c_int64, C.c_int64] + [vp] * 17),
     "nerrf_trace_path_flags": (C.c_int, [vp, vp, C.c_int64, vp]),
-    "nerrf_trace_intern_device_workspace_bytes": (C.c_int, [C.c_int64, C.c_int64, C.POINTER(C.c_int64)]),
+    "nerrf_trace_frame": (C.c_int, [vp, C.c_int64, C.c_int, C.c_int64, vp, vp, vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
+    "nerrf_trace_decode_device_workspace_bytes": (C.c_int, [C.c_int64, C.POINTER(C.c_int64)]),
+    "nerrf_trace_decode_device": (C.c_int, [vp, vp, vp, vp, C.c_int64, C.c_int64, C.POINTER(vp), vp, vp, C.c_int64, vp]),
+    "nerrf_trace_stream_order_workspace_bytes": (C.c_int, [C.c_int64, C.POINTER(C.c_int64)]),
+    "nerrf_trace_stream_order": (C.c_int, [C.c_int64, vp, vp, vp, vp, C.c_double, vp, vp, vp, vp, vp, vp, C.POINTER(C.c_int64),
+                                           vp, C.c_int64, vp]),
+    "nerrf_trace_stream_columns": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]),
+    "nerrf_trace_gather_rows_workspace_bytes": (C.c_int, [C.c_int64, C.POINTER(C.c_int64)]),
+    "nerrf_trace_gather_rows": (C.c_int, [C.POINTER(vp), vp, C.c_int64, C.POINTER(vp), vp, C.c_int64, vp]),
+    "nerrf_trace_intern_device_workspace_bytes":(C.c_int, [C.c_int64, C.c_int64, C.POINTER(C.c_int64)]),
     "nerrf_trace_intern_device": (C.c_int, [C.c_int64, C.c_int64, vp, vp, vp, vp, vp, vp, C.c_int, vp, vp, vp, C.POINTER(C.c_int64),
                                             vp, vp, vp, C.c_int64, vp, C.c_int64, vp]),
     "nerrf_trace_name_hash": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp, vp]),

@@ -15,85 +15,13 @@
 #include <unordered_map>
 #include <vector>
 #include "common.cuh"
+#include "wire.cuh"
 
 namespace nerrf {
 namespace {
 
-struct Reader {
-    const uint8_t* p;
-    const uint8_t* end;
-    bool varint(uint64_t* v) {
-        uint64_t r = 0;
-        for (int shift = 0; shift < 70; shift += 7) {
-            if (p >= end) return false;
-            const uint8_t b = *p++;
-            if (shift < 64) r |= (uint64_t)(b & 0x7f) << shift;
-            if (!(b & 0x80)) { *v = r; return true; }
-        }
-        return false;   // > 10 bytes
-    }
-    bool len_delim(const uint8_t** s, uint64_t* n) {
-        if (!varint(n)) return false;
-        if (*n > (uint64_t)(end - p)) return false;
-        *s = p; p += *n;
-        return true;
-    }
-    bool skip(uint32_t wire) {
-        uint64_t v; const uint8_t* s;
-        switch (wire) {
-            case 0: return varint(&v);
-            case 1: if (end - p < 8) return false; p += 8; return true;
-            case 2: return len_delim(&s, &v);
-            case 5: if (end - p < 4) return false; p += 4; return true;
-            default: return false;   // groups (3, 4) are not used by this schema
-        }
-    }
-};
-
-struct EventView {
-    int64_t ts_sec = 0; int32_t ts_nanos = 0;
-    uint32_t pid = 0, tid = 0; int32_t flags = 0; int64_t ret_val = 0; uint64_t bytes = 0;
-    const uint8_t *comm = nullptr, *syscall = nullptr, *path = nullptr, *new_path = nullptr;
-    uint64_t comm_n = 0, syscall_n = 0, path_n = 0, new_path_n = 0;
-};
-
-bool parse_timestamp(const uint8_t* s, uint64_t n, EventView* e) {
-    Reader r{s, s + n};
-    while (r.p < r.end) {
-        uint64_t tag, v;
-        if (!r.varint(&tag)) return false;
-        const uint32_t field = (uint32_t)(tag >> 3), wire = (uint32_t)(tag & 7);
-        if (field == 1 && wire == 0) { if (!r.varint(&v)) return false; e->ts_sec = (int64_t)v; }
-        else if (field == 2 && wire == 0) { if (!r.varint(&v)) return false; e->ts_nanos = (int32_t)v; }
-        else if (!r.skip(wire)) return false;
-    }
-    return true;
-}
-
-bool parse_event(const uint8_t* s, uint64_t n, EventView* e) {
-    Reader r{s, s + n};
-    while (r.p < r.end) {
-        uint64_t tag, v; const uint8_t* q;
-        if (!r.varint(&tag)) return false;
-        const uint32_t field = (uint32_t)(tag >> 3), wire = (uint32_t)(tag & 7);
-        if (wire == 0 && (field == 2 || field == 3 || field == 8 || field == 9 || field == 10)) {
-            if (!r.varint(&v)) return false;
-            if (field == 2) e->pid = (uint32_t)v;
-            else if (field == 3) e->tid = (uint32_t)v;
-            else if (field == 8) e->flags = (int32_t)v;
-            else if (field == 9) e->ret_val = (int64_t)(v >> 1) ^ -(int64_t)(v & 1);      // zigzag
-            else e->bytes = v;
-        } else if (wire == 2 && (field == 1 || (field >= 4 && field <= 7))) {
-            if (!r.len_delim(&q, &v)) return false;
-            if (field == 1) { if (!parse_timestamp(q, v, e)) return false; }             // repeated occurrence merges
-            else if (field == 4) { e->comm = q; e->comm_n = v; }
-            else if (field == 5) { e->syscall = q; e->syscall_n = v; }
-            else if (field == 6) { e->path = q; e->path_n = v; }
-            else { e->new_path = q; e->new_path_n = v; }
-        } else if (!r.skip(wire)) return false;
-    }
-    return true;
-}
+using wire::EventView;
+using wire::Reader;
 
 // calls f(EventView&) for every Event of the batch; returns the byte offset of the first malformed record or -1
 template <typename Fn>
@@ -101,41 +29,15 @@ int64_t for_each_event(const uint8_t* buf, int64_t len, Fn&& f) {
     Reader r{buf, buf + len};
     while (r.p < r.end) {
         const uint8_t* at = r.p;
-        uint64_t tag, n; const uint8_t* s;
-        if (!r.varint(&tag)) return at - buf;
-        if ((tag >> 3) == 1 && (tag & 7) == 2) {
-            if (!r.len_delim(&s, &n)) return at - buf;
+        bool event; const uint8_t* s; uint64_t n;
+        if (!wire::next_record(&r, &event, &s, &n)) return at - buf;
+        if (event) {
             EventView e;
-            if (!parse_event(s, n, &e)) return at - buf;
+            if (!wire::parse_event(s, n, &e)) return at - buf;
             f(e);
-        } else if (!r.skip((uint32_t)(tag & 7))) return at - buf;
+        }
     }
     return -1;
-}
-
-bool contains(const uint8_t* s, uint64_t n, const char* needle, size_t m) { return n >= m && memmem(s, n, needle, m) != nullptr; }
-
-// "README" or "RANSOM" anywhere in the path, ASCII case-insensitive: both start with R, so one memchr-style scan
-bool has_note_word(const uint8_t* s, uint64_t n) {
-    if (n < 6) return false;
-    for (uint64_t i = 0; i + 6 <= n; ++i) {
-        if ((s[i] | 0x20) != 'r') continue;
-        uint8_t w[5];
-        for (int k = 0; k < 5; ++k) { const uint8_t c = s[i + 1 + k]; w[k] = (c >= 'a' && c <= 'z') ? (uint8_t)(c - 32) : c; }
-        if (memcmp(w, "EADME", 5) == 0 || memcmp(w, "ANSOM", 5) == 0) return true;
-    }
-    return false;
-}
-bool starts_with(const uint8_t* s, uint64_t n, const char* pre) { const size_t m = strlen(pre); return n >= m && memcmp(s, pre, m) == 0; }
-bool ends_with(const uint8_t* s, uint64_t n, const char* suf) { const size_t m = strlen(suf); return n >= m && memcmp(s + n - m, suf, m) == 0; }
-
-// event-kind slots of nerrf_b200/graph.py (_EVENT_SLOT); slot 7 = anything else
-int event_slot(const uint8_t* s, uint64_t n) {
-    static const char* names[7] = {"file_created", "file_encrypt_start", "file_encrypt_complete", "ransom_note_created",
-                                   "openat", "write", "rename"};
-    for (int i = 0; i < 7; ++i)
-        if (strlen(names[i]) == n && memcmp(s, names[i], n) == 0) return i;
-    return 7;
 }
 
 // merge key of a file and its renamed / encrypted twin: the path without its last extension (graph.py _stem)
@@ -173,6 +75,55 @@ extern "C" int nerrf_trace_scan(const uint8_t* buf, int64_t len, int64_t* n_even
     return NERRF_OK;
 }
 
+// top-level varint for the framing walk: 1 = read, 0 = the bytes ran out first (cut off), -1 = more than 10 bytes
+static int frame_varint(const uint8_t** p, const uint8_t* end, uint64_t* v) {
+    uint64_t r = 0;
+    for (int shift = 0; shift < 70; shift += 7) {
+        if (*p >= end) return 0;
+        const uint8_t b = *(*p)++;
+        if (shift < 64) r |= (uint64_t)(b & 0x7f) << shift;
+        if (!(b & 0x80)) { *v = r; return 1; }
+    }
+    return -1;
+}
+
+extern "C" int nerrf_trace_frame(const uint8_t* buf, int64_t len, int partial, int64_t max_records, int64_t* rec_at,
+                                 int64_t* body_off, int64_t* body_len, int64_t* n_records, int64_t* consumed) {
+    NERRF_REQUIRE((buf != nullptr || len == 0) && len >= 0 && max_records >= 0, "bad buffer");
+    NERRF_REQUIRE(n_records && consumed && (max_records == 0 || (rec_at && body_off && body_len)), "null output");
+    // the walk of for_each_event (tag + length per record, unknown fields skipped by wire type) without parsing the Events
+    const uint8_t* p = buf;
+    const uint8_t* end = buf + len;
+    int64_t n = 0;
+    int state = 1;                                          // 1 ok, 0 cut off, -1 malformed
+    const uint8_t* at = p;
+    while (p < end) {
+        at = p;
+        uint64_t tag, m = 0;
+        state = frame_varint(&p, end, &tag);
+        if (state < 1) break;
+        const uint32_t wt = (uint32_t)(tag & 7);
+        const bool event = (tag >> 3) == 1 && wt == 2;
+        if (wt == 0) state = frame_varint(&p, end, &m);
+        else if (wt == 1 || wt == 5) { const int64_t w = wt == 1 ? 8 : 4; state = end - p < w ? 0 : 1; if (state) p += w; }
+        else if (wt == 2) {
+            state = frame_varint(&p, end, &m);
+            if (state == 1 && m > (uint64_t)(end - p)) state = 0;
+        } else state = -1;                                  // groups are malformed
+        if (state < 1) break;
+        if (event) {
+            if (n < max_records) { rec_at[n] = at - buf; body_off[n] = p - buf; body_len[n] = (int64_t)m; }
+            ++n;
+        }
+        if (wt == 2) p += m;
+    }
+    *n_records = n;
+    *consumed = (state == 1 ? p : at) - buf;
+    // a malformed record, or (whole-buffer mode) a cut-off one: the outputs still describe the records before it
+    NERRF_REQUIRE(state == 1 || (state == 0 && partial), "malformed EventBatch at byte offset %lld", (long long)(at - buf));
+    return NERRF_OK;
+}
+
 extern "C" int nerrf_trace_decode(const uint8_t* buf, int64_t len, int64_t n_events, int64_t* ts_sec, int32_t* ts_nanos,
                                   uint32_t* pid, uint32_t* tid, int32_t* flags, int64_t* ret_val, uint64_t* bytes,
                                   uint8_t* event_slot_out, uint8_t* path_flags, int64_t* comm_off, uint8_t* comm_data,
@@ -194,13 +145,8 @@ extern "C" int nerrf_trace_decode(const uint8_t* buf, int64_t len, int64_t n_eve
         if (i >= n_events) { overflow = true; return; }
         ts_sec[i] = e.ts_sec; ts_nanos[i] = e.ts_nanos; pid[i] = e.pid; tid[i] = e.tid; flags[i] = e.flags;
         ret_val[i] = e.ret_val; bytes[i] = e.bytes;
-        event_slot_out[i] = (uint8_t)event_slot(e.syscall, e.syscall_n);
-        uint8_t pf = 0;
-        if (contains(e.path, e.path_n, ".lockbit", 8)) pf |= NERRF_PATH_LOCKBIT;
-        if (has_note_word(e.path, e.path_n)) pf |= NERRF_PATH_NOTE;
-        if (starts_with(e.path, e.path_n, "/tmp") || starts_with(e.path, e.path_n, "/proc")) pf |= NERRF_PATH_TMP;
-        if (ends_with(e.path, e.path_n, ".lockbit3")) pf |= NERRF_PATH_ENCRYPTED;
-        path_flags[i] = pf;
+        event_slot_out[i] = (uint8_t)wire::event_slot(e.syscall, e.syscall_n);
+        path_flags[i] = wire::path_flags(e.path, e.path_n);
         put(comm_data, comm_off, i, &o[0], e.comm, e.comm_n);
         put(syscall_data, syscall_off, i, &o[1], e.syscall, e.syscall_n);
         put(path_data, path_off, i, &o[2], e.path, e.path_n);
@@ -220,12 +166,7 @@ extern "C" int nerrf_trace_path_flags(const int64_t* off, const uint8_t* data, i
         NERRF_REQUIRE(off[i + 1] >= off[i], "offsets must be non-decreasing (string %lld)", (long long)i);
         const uint8_t* s = data + off[i];
         const uint64_t m = (uint64_t)(off[i + 1] - off[i]);
-        uint8_t pf = 0;
-        if (contains(s, m, ".lockbit", 8)) pf |= NERRF_PATH_LOCKBIT;
-        if (has_note_word(s, m)) pf |= NERRF_PATH_NOTE;
-        if (starts_with(s, m, "/tmp") || starts_with(s, m, "/proc")) pf |= NERRF_PATH_TMP;
-        if (ends_with(s, m, ".lockbit3")) pf |= NERRF_PATH_ENCRYPTED;
-        flags_out[i] = pf;
+        flags_out[i] = wire::path_flags(s, m);
     }
     return NERRF_OK;
 }
@@ -275,7 +216,7 @@ extern "C" int nerrf_trace_intern(int64_t n_events, const int64_t* order, const 
             fit = files.emplace(key, id).first;
         }
         node_f[i] = fit->second;
-        if (ends_with(s, n, ".lockbit3")) { node_name_event[fit->second] = i; node_name_which[fit->second] = 0; }   // rollback target
+        if (wire::ends_with(s, n, ".lockbit3", 9)) { node_name_event[fit->second] = i; node_name_which[fit->second] = 0; }   // rollback target
         node_g[i] = -1;
         const uint64_t gn = (uint64_t)(new_path_off[i + 1] - new_path_off[i]);
         if (gn && merge_renames) {
@@ -284,7 +225,7 @@ extern "C" int nerrf_trace_intern(int64_t n_events, const int64_t* order, const 
             const uint8_t* g = new_path_data + new_path_off[i];
             key.assign((const char*)g, stem_len(g, gn));
             files.emplace(key, fit->second);                              // no-op when the key is already known
-            if (ends_with(g, gn, ".lockbit3")) { node_name_event[fit->second] = i; node_name_which[fit->second] = 1; }
+            if (wire::ends_with(g, gn, ".lockbit3", 9)) { node_name_event[fit->second] = i; node_name_which[fit->second] = 1; }
         }
         if (gn && !merge_renames) {
             key.assign((const char*)(new_path_data + new_path_off[i]), gn);

@@ -75,6 +75,35 @@ def decode_event_batch(buf) -> EventColumns:
     return EventColumns(n=n, strings=strings, **cols)
 
 
+def _frame(raw: np.ndarray, partial: bool):
+    """nerrf_trace_frame -> (error offset or None, rec_at, body_off, body_len, consumed).  On a malformed record the
+    arrays still hold the records before it."""
+    h = _lib.lib()
+    cap = raw.size // 16 + 16
+    while True:
+        rec = np.empty((3, cap), np.int64)
+        n, consumed = C.c_int64(), C.c_int64()
+        rc = h.nerrf_trace_frame(_p(raw) if raw.size else None, raw.size, int(bool(partial)), cap, _p(rec[0]), _p(rec[1]),
+                                 _p(rec[2]), C.byref(n), C.byref(consumed))
+        if n.value <= cap:
+            break
+        cap = n.value
+    if rc != 0 and not h.nerrf_last_error().decode().startswith("malformed"):
+        _lib.check(rc, "nerrf_trace_frame")
+    m = n.value
+    return (consumed.value if rc != 0 else None), rec[0, :m], rec[1, :m], rec[2, :m], consumed.value
+
+
+def frame_event_batch(buf, partial=False):
+    """Top-level framing of EventBatch wire bytes (nerrf_trace_frame): -> (rec_at, body_off, body_len, consumed), one
+    entry per Event record.  partial=True: a cut-off trailing record is not an error; `consumed` stops before it."""
+    raw = np.frombuffer(buf, dtype=np.uint8) if not isinstance(buf, np.ndarray) else np.ascontiguousarray(buf, np.uint8)
+    bad, rec_at, body_off, body_len, consumed = _frame(raw, partial)
+    if bad is not None:
+        raise _lib.NerrfError(f"nerrf_trace_frame failed: malformed EventBatch at byte offset {bad}")
+    return rec_at, body_off, body_len, consumed
+
+
 def events_from_columns(cols: EventColumns) -> list:
     """The dict schema of graph.events_from_event_batch / the JSONL traces (for the per-event host loader)."""
     ts = cols.timestamp
@@ -385,3 +414,46 @@ def encode_event_batch(events) -> bytes:
                 + field_varint(10, int(e.get("bytes", e.get("size", 0)) or 0)))
         out += varint(1 << 3 | 2) + varint(len(body)) + body
     return bytes(out)
+
+
+def encode_columns(cols: EventColumns) -> list:
+    """One serialized EventBatch record (field 1 = an Event) per row of `cols`, in stored order: the stream a tracker
+    would send, for replaying column traces through the live path (test / tooling helper)."""
+    from functools import lru_cache
+
+    @lru_cache(maxsize=1 << 16)
+    def varint(v):
+        v &= (1 << 64) - 1
+        out = bytearray()
+        while True:
+            b = v & 0x7f
+            v >>= 7
+            out.append(b | (0x80 if v else 0))
+            if not v:
+                return bytes(out)
+
+    raw = {k: (off.tolist(), data.tobytes()) for k, (off, data) in cols.strings.items()}
+    sec, nan, pid, tid = cols.ts_sec.tolist(), cols.ts_nanos.tolist(), cols.pid.tolist(), cols.tid.tolist()
+    flg, rv, by = cols.flags.tolist(), cols.ret_val.tolist(), cols.bytes.tolist()
+    fields = ((4, "comm"), (5, "syscall"), (6, "path"), (7, "new_path"))
+    recs = []
+    for i in range(cols.n):
+        ts = (varint(8) + varint(sec[i]) if sec[i] else b"") + (varint(16) + varint(nan[i]) if nan[i] else b"")
+        body = [b"\x0a", varint(len(ts)), ts]
+        if pid[i]:
+            body += [b"\x10", varint(pid[i])]
+        if tid[i]:
+            body += [b"\x18", varint(tid[i])]
+        for num, name in fields:
+            off, data = raw[name]
+            if off[i + 1] > off[i]:
+                body += [varint(num << 3 | 2), varint(off[i + 1] - off[i]), data[off[i]:off[i + 1]]]
+        if flg[i]:
+            body += [b"\x40", varint(flg[i])]
+        if rv[i]:
+            body += [b"\x48", varint((rv[i] << 1) ^ (rv[i] >> 63))]
+        if by[i]:
+            body += [b"\x50", varint(by[i])]
+        b = b"".join(body)
+        recs.append(b"\x0a" + varint(len(b)) + b)
+    return recs

@@ -153,6 +153,158 @@ class LazyNames:
         e, w = int(self.name_event[v]), int(self.name_which[v])
         return "pid:%d" % int(self.cols.pid[e]) if w == 2 else self.cols.text("path" if w == 0 else "new_path", e)
 
+    def take(self, nodes):
+        return [self[v] for v in nodes]
+
+
+class DeviceNames:
+    """Node names of a live window graph, read from the device string columns: `take` fetches the names of many nodes
+    with two device-to-host copies, whatever their number."""
+
+    def __init__(self, pid, poff, pdata, goff, gdata, name_event: np.ndarray, name_which: np.ndarray):
+        self.pid, self.poff, self.pdata, self.goff, self.gdata = pid, poff, pdata, goff, gdata
+        self.name_event, self.name_which = name_event, name_which
+
+    def __len__(self):
+        return int(self.name_event.shape[0])
+
+    def __getitem__(self, v):
+        return self.take([v])[0]
+
+    def take(self, nodes):
+        import torch
+        nodes = np.asarray(nodes, np.int64).reshape(-1)
+        if nodes.size == 0:
+            return []
+        ev, which = self.name_event[nodes], self.name_which[nodes]
+        e = torch.from_numpy(ev).to(self.pid.device)
+        meta = torch.stack([self.poff[e], self.poff[e + 1], self.goff[e], self.goff[e + 1],
+                            self.pid[e].to(torch.int64) & 0xffffffff]).cpu().numpy()
+        lo = np.where(which == 1, meta[2], meta[0]); hi = np.where(which == 1, meta[3], meta[1])
+        ln = np.where(which == 2, 0, hi - lo)
+        starts = np.zeros(nodes.size + 1, np.int64); np.cumsum(ln, out=starts[1:])
+        raw = b""
+        if starts[-1]:
+            pos = np.arange(starts[-1], dtype=np.int64) - np.repeat(starts[:-1], ln) + np.repeat(lo, ln)
+            from_g = np.repeat(which == 1, ln)
+            p = torch.from_numpy(pos).to(self.pid.device); g = torch.from_numpy(from_g).to(self.pid.device)
+            pick = torch.where(g, self.gdata[p.clamp(max=self.gdata.numel() - 1)], self.pdata[p.clamp(max=self.pdata.numel() - 1)])
+            raw = pick.cpu().numpy().tobytes()
+        return ["pid:%d" % int(meta[4][k]) if which[k] == 2 else raw[starts[k]:starts[k + 1]].decode("utf-8", "replace")
+                for k in range(nodes.size)]
+
+
+_SCALARS = (("ts_sec", "int64"), ("ts_nanos", "int32"), ("pid", "int32"), ("tid", "int32"), ("flags", "int32"),
+            ("ret_val", "int64"), ("bytes", "int64"), ("event_slot", "uint8"), ("path_flags", "uint8"))
+
+
+class _DeviceColumns:
+    """EventColumns in HBM with room to grow: scalars [rows], string offsets [rows + 1], string bytes; ptrs() = the 17
+    column pointers of the C entry points (nerrf_trace_decode's argument order)."""
+
+    def __init__(self, dev, rows: int, nbytes):
+        import torch
+        self.dev = dev
+        self.s = {k: torch.zeros(max(rows, 1), dtype=getattr(torch, dt), device=dev) for k, dt in _SCALARS}
+        self.off = [torch.zeros(max(rows, 1) + 1, dtype=torch.int64, device=dev) for _ in range(4)]
+        self.data = [torch.zeros(max(int(b), 1), dtype=torch.uint8, device=dev) for b in nbytes]
+
+    @property
+    def rows(self):
+        return int(self.s["ts_sec"].shape[0])
+
+    def ptrs(self):
+        t = [self.s[k] for k, _ in _SCALARS]
+        for q in range(4):
+            t += [self.off[q], self.data[q]]
+        return _lib_ptr_array(t)
+
+    def reserve(self, n_used: int, used_bytes, rows: int, nbytes):
+        """room for `rows` rows and nbytes[q] bytes per string column, keeping the first n_used rows"""
+        import torch
+        if rows > self.rows:
+            new = max(rows, 2 * self.rows)
+            for k, _ in _SCALARS:
+                t = torch.zeros(new, dtype=self.s[k].dtype, device=self.dev); t[:n_used] = self.s[k][:n_used]; self.s[k] = t
+            for q in range(4):
+                t = torch.zeros(new + 1, dtype=torch.int64, device=self.dev); t[:n_used + 1] = self.off[q][:n_used + 1]; self.off[q] = t
+        for q in range(4):
+            if nbytes[q] > self.data[q].numel():
+                t = torch.zeros(max(int(nbytes[q]), 2 * self.data[q].numel()), dtype=torch.uint8, device=self.dev)
+                t[:used_bytes[q]] = self.data[q][:used_bytes[q]]
+                self.data[q] = t
+
+    def host(self, n: int) -> ingest.EventColumns:
+        """the first n rows as host EventColumns"""
+        sc = {k: self.s[k][:n].cpu().numpy() for k, _ in _SCALARS}
+        sc["pid"] = sc["pid"].view(np.uint32); sc["tid"] = sc["tid"].view(np.uint32); sc["bytes"] = sc["bytes"].view(np.uint64)
+        strings = {}
+        for q, name in enumerate(ingest.STRING_COLUMNS):
+            off = self.off[q][:n + 1].cpu().numpy()
+            strings[name] = (off, self.data[q][:int(off[-1])].cpu().numpy())
+        return ingest.EventColumns(n=n, strings=strings, **sc)
+
+
+def _lib_ptr_array(tensors):
+    from . import _lib
+    return _lib.ptr_array(tensors)
+
+
+def _decode_into(dc: _DeviceColumns, n: int, used_bytes, raw: np.ndarray, partial: bool, timings=None):
+    """Frame `raw` on the host, decode its Event records on the device into rows n.. of `dc`.  -> (rows added, bytes
+    consumed, new used_bytes).  Raises (and adds nothing) when a record is malformed: same message and byte offset as
+    ingest.decode_event_batch."""
+    import ctypes as C
+    import time
+    import torch
+    from . import _lib
+    a = time.perf_counter()
+    bad, rec_at, body_off, body_len, consumed = ingest._frame(raw, partial)
+    m = int(rec_at.shape[0])
+    if timings is not None:
+        timings["frame_ms"] = (time.perf_counter() - a) * 1e3
+    dev_bad = None
+    used = list(used_bytes)
+    if m:
+        payload = int(body_len.sum())
+        if payload >= (1 << 31):
+            raise _lib.NerrfError("append of %d event bytes: split it (at most 2^31 - 1 per append)" % payload)
+        end = int(body_off[-1] + body_len[-1])
+        wire_d = torch.from_numpy(raw[:end] if raw.flags.writeable else raw[:end].copy()).to(dc.dev)
+        rec_d = torch.from_numpy(np.stack([rec_at, body_off, body_len])).to(dc.dev)
+        dc.reserve(n, used, n + m, [u + payload for u in used])
+        need = C.c_int64()
+        _lib.check(_lib.lib().nerrf_trace_decode_device_workspace_bytes(m, C.byref(need)), "decode_device_workspace_bytes")
+        ws = torch.empty(need.value + 256, dtype=torch.uint8, device=dc.dev)
+        status = torch.empty(1, dtype=torch.int64, device=dc.dev)
+        ev0 = torch.cuda.Event(enable_timing=True); ev1 = torch.cuda.Event(enable_timing=True)
+        with torch.cuda.device(dc.dev):
+            ev0.record()
+            _lib.check(_lib.lib().nerrf_trace_decode_device(
+                _lib.ptr(wire_d), _lib.ptr(rec_d[0]), _lib.ptr(rec_d[1]), _lib.ptr(rec_d[2]), m, n, dc.ptrs(), _lib.ptr(status),
+                C.c_void_p((ws.data_ptr() + 255) & ~255), need.value, _lib.current_stream_ptr()), "nerrf_trace_decode_device")
+            ev1.record()
+        back = torch.cat([status] + [o[n + m:n + m + 1] for o in dc.off]).cpu().numpy()
+        if timings is not None:
+            timings["decode_ms"] = ev0.elapsed_time(ev1)
+        if back[0] != -1:
+            dev_bad = int(back[0])
+        used = [int(v) for v in back[1:]]
+    worst = min([b for b in (bad, dev_bad) if b is not None], default=None)
+    if worst is not None:
+        raise _lib.NerrfError(f"nerrf_trace_decode_device failed: malformed EventBatch at byte offset {worst}")
+    return m, consumed, used
+
+
+def decode_event_batch_device(buf, device="cuda") -> ingest.EventColumns:
+    """ingest.decode_event_batch with the Event bodies parsed ON THE DEVICE (nerrf_trace_decode_device): the same
+    columns, brought back to the host."""
+    import torch
+    raw = np.frombuffer(buf, dtype=np.uint8) if not isinstance(buf, np.ndarray) else np.ascontiguousarray(buf, np.uint8)
+    dc = _DeviceColumns(torch.device(device), 1, [1, 1, 1, 1])
+    m, _, _ = _decode_into(dc, 0, [0, 0, 0, 0], raw, False)
+    return dc.host(m)
+
 
 class DeviceStream:
     """The event stream resident in HBM (SURVEY.md 8f rank 1: "window, inode/path dedup via hash, sort-by-dst -> CSR,
@@ -201,10 +353,159 @@ class DeviceStream:
         self._ws = torch.empty(need.value + 256, dtype=torch.uint8, device=dev)
         self._ws_bytes = need.value
 
+    @classmethod
+    def live(cls, device="cuda", observable=True, merge_renames=True):
+        """An empty stream that grows as the tracker delivers EventBatch bytes (append) and sheds what no future window
+        can reach (compact).  Decoding, time order, path resolution and retention run on the device."""
+        import torch
+        self = cls.__new__(cls)
+        self.torch = torch
+        self.dev = torch.device(device)
+        self.observable, self.merge = observable, bool(merge_renames)
+        self.cols = None
+        self._dc = _DeviceColumns(self.dev, 1024, [1 << 16] * 4)
+        self._used = [0, 0, 0, 0]
+        self._horizon = -np.inf
+        self._slot_map = torch.tensor(G.OBSERVABLE_SLOT, dtype=torch.uint8, device=self.dev) if observable else None
+        self.n = 0
+        self.n_keep = 0
+        self.timings_ms = {}
+        self._rebuild()
+        return self
+
+    @property
+    def resident_events(self) -> int:
+        """events held in HBM (live stream)"""
+        return self.n
+
+    def append(self, wire_bytes, partial=False) -> int:
+        """Decode whole EventBatch records on the device and append them.  partial=True: a cut-off trailing record is
+        left for the caller to resend with the rest of its bytes.  -> bytes consumed.  A malformed record raises and
+        leaves the stream as it was."""
+        raw = np.frombuffer(wire_bytes, dtype=np.uint8) if not isinstance(wire_bytes, np.ndarray) else np.ascontiguousarray(wire_bytes, np.uint8)
+        self.timings_ms = {}
+        m, consumed, used = _decode_into(self._dc, self.n, self._used, raw, partial, self.timings_ms)
+        if m:
+            self.n += m
+            self._used = used
+            self._rebuild()
+        return consumed
+
+    def compact(self, horizon: float):
+        """Drop the events no window ending after `horizon + window` can hold (ts <= horizon), except each pid's latest
+        event with a path, which a later path-less write of that pid still resolves to.  Stored order is kept."""
+        import ctypes as C
+        from . import _lib
+        torch = self.torch
+        self._horizon = max(self._horizon, float(horizon))
+        ev0 = torch.cuda.Event(enable_timing=True); ev1 = torch.cuda.Event(enable_timing=True)
+        with torch.cuda.device(self.dev):
+            ev0.record()
+        self._rebuild()
+        if self._n_retain < self.n:
+            m = self._n_retain
+            out = _DeviceColumns(self.dev, self._dc.rows, [d.numel() for d in self._dc.data])
+            need = C.c_int64()
+            _lib.check(_lib.lib().nerrf_trace_gather_rows_workspace_bytes(m, C.byref(need)), "gather_rows_workspace_bytes")
+            ws = torch.empty(need.value + 256, dtype=torch.uint8, device=self.dev)
+            with torch.cuda.device(self.dev):
+                _lib.check(_lib.lib().nerrf_trace_gather_rows(self._dc.ptrs(), _lib.ptr(self._retain), m, out.ptrs(),
+                                                              C.c_void_p((ws.data_ptr() + 255) & ~255), need.value,
+                                                              _lib.current_stream_ptr()), "nerrf_trace_gather_rows")
+            self._dc, self.n = out, m
+            self._used = [int(v) for v in torch.cat([o[m:m + 1] for o in out.off]).cpu().numpy()]
+            self._rebuild()
+        with torch.cuda.device(self.dev):
+            ev1.record()
+        ev1.synchronize()
+        self.timings_ms["compact_ms"] = ev0.elapsed_time(ev1)
+
+    def _rebuild(self):
+        """time order, path resolution and the per-event columns of the window graph over the resident events"""
+        import ctypes as C
+        from . import _lib
+        torch = self.torch
+        dev, n, dc = self.dev, self.n, self._dc
+        ev0 = torch.cuda.Event(enable_timing=True); ev1 = torch.cuda.Event(enable_timing=True)
+        with torch.cuda.device(dev):
+            ev0.record()
+        need = C.c_int64()
+        _lib.check(_lib.lib().nerrf_trace_stream_order_workspace_bytes(n, C.byref(need)), "stream_order_workspace_bytes")
+        ws = torch.empty(need.value + 256, dtype=torch.uint8, device=dev)
+        e = lambda dt, k=n: torch.empty(max(k, 1), dtype=dt, device=dev)
+        ts, order, ts_sorted, src, retain = e(torch.float64), e(torch.int64), e(torch.float64), e(torch.int64), e(torch.int64)
+        res_off = torch.zeros(n + 1, dtype=torch.int64, device=dev)
+        counts = (C.c_int64 * 3)()
+        poff, pdata, goff, gdata = dc.off[2], dc.data[2], dc.off[3], dc.data[3]
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().nerrf_trace_stream_order(
+                n, _lib.ptr(dc.s["ts_sec"]), _lib.ptr(dc.s["ts_nanos"]), _lib.ptr(dc.s["pid"]), _lib.ptr(poff), float(self._horizon),
+                _lib.ptr(ts), _lib.ptr(order), _lib.ptr(ts_sorted), _lib.ptr(src), _lib.ptr(res_off), _lib.ptr(retain), counts,
+                C.c_void_p((ws.data_ptr() + 255) & ~255), need.value, _lib.current_stream_ptr()), "nerrf_trace_stream_order")
+        n_keep, n_retain, pbytes = int(counts[0]), int(counts[1]), int(counts[2])
+        res_data = torch.zeros(max(pbytes, 1), dtype=torch.uint8, device=dev)
+        pf, pf_raw, slot = e(torch.uint8), e(torch.uint8), e(torch.uint8)
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().nerrf_trace_stream_columns(
+                n, _lib.ptr(src), _lib.ptr(poff), _lib.ptr(pdata), _lib.ptr(dc.s["path_flags"]), _lib.ptr(goff), _lib.ptr(gdata),
+                _lib.ptr(dc.s["event_slot"]), _lib.ptr(self._slot_map), _lib.ptr(res_off), int(self.merge), _lib.ptr(res_data),
+                _lib.ptr(pf), _lib.ptr(pf_raw), _lib.ptr(slot), _lib.current_stream_ptr()), "nerrf_trace_stream_columns")
+            ev1.record()
+        self.n_keep, self._n_retain, self._retain = n_keep, n_retain, retain[:n_retain]
+        self.d_order, self.d_ts_sorted, self.d_ts = order[:n_keep], ts_sorted[:n_keep], ts
+        self.d_pid, self.d_poff, self.d_pdata, self.d_goff, self.d_gdata = dc.s["pid"], res_off, res_data, goff, gdata
+        self.d_raw_slot, self.d_slot, self.d_bytes, self.d_pf, self.d_pf_raw = dc.s["event_slot"], slot, dc.s["bytes"], pf, pf_raw
+        if n_keep:
+            lohi = torch.stack([ts_sorted[0], ts_sorted[n_keep - 1]]).cpu().numpy()
+            self._span = (float(lohi[0]), float(lohi[1]))
+        else:
+            self._span = (0.0, 0.0)
+        self._alloc_intern(max(n, 1))
+        ev1.synchronize()
+        self.timings_ms["rebuild_ms"] = self.timings_ms.get("rebuild_ms", 0.0) + ev0.elapsed_time(ev1)
+
+    def _alloc_intern(self, n):
+        """node tables and interning workspace for windows of up to n events"""
+        import ctypes as C
+        from . import _lib
+        torch = self.torch
+        if getattr(self, "node_p", None) is not None and self.node_p.shape[0] >= n:
+            return
+        n = max(n, 2 * getattr(self, "node_p", torch.empty(0)).shape[0])
+        self.cap = max((2 if self.merge else 3) * n, 1)
+        self.node_p = torch.empty(n, dtype=torch.int32, device=self.dev)
+        self.node_f = torch.empty_like(self.node_p); self.node_g = torch.empty_like(self.node_p)
+        self.kind = torch.zeros(self.cap, dtype=torch.int8, device=self.dev)
+        self.name_event = torch.zeros(self.cap, dtype=torch.int64, device=self.dev)
+        self.name_which = torch.zeros(self.cap, dtype=torch.int8, device=self.dev)
+        need = C.c_int64()
+        _lib.check(_lib.lib().nerrf_trace_intern_device_workspace_bytes(n, self.cap, C.byref(need)), "intern_device_workspace_bytes")
+        self._ws = torch.empty(need.value + 256, dtype=torch.uint8, device=self.dev)
+        self._ws_bytes = need.value
+
     def span(self):
+        if self.cols is None:                                  # live stream: first and last surviving event
+            return self._span
         if self.n == 0:
             return 0.0, 0.0
         return float(self.ts_sorted[0]), float(self.ts_sorted[-1])
+
+    def _window_ranks(self, t_lo: float, t_hi: float):
+        """-> (lo, hi, ts of rank lo, ts of rank hi - 1): the window's slice of the time-sorted survivors"""
+        if self.cols is not None:
+            lo = int(np.searchsorted(self.ts_sorted, t_lo, "right")); hi = int(np.searchsorted(self.ts_sorted, t_hi, "right"))
+            if hi <= lo:
+                return lo, hi, None, None
+            return lo, hi, float(self.ts_sorted[lo]), float(self.ts_sorted[hi - 1])
+        torch = self.torch
+        if self.n_keep == 0:
+            return 0, 0, None, None
+        b = torch.searchsorted(self.d_ts_sorted, torch.tensor([t_lo, t_hi], dtype=torch.float64, device=self.dev), right=True)
+        lo, hi = (int(v) for v in b.cpu().numpy())
+        if hi <= lo:
+            return lo, hi, None, None
+        v = self.d_ts_sorted[torch.tensor([lo, hi - 1], device=self.dev)].cpu().numpy()
+        return lo, hi, float(v[0]), float(v[1])
 
     def window_graph(self, t_lo: float, t_hi: float, window_s: float):
         """The temporal graph of the events with t_lo < t <= t_hi (device tensors), or None when there are none.
@@ -212,7 +513,7 @@ class DeviceStream:
         import ctypes as C
         from . import _lib
         torch = self.torch
-        lo = int(np.searchsorted(self.ts_sorted, t_lo, "right")); hi = int(np.searchsorted(self.ts_sorted, t_hi, "right"))
+        lo, hi, t_first, t_last = self._window_ranks(t_lo, t_hi)
         nw = hi - lo
         if nw <= 0:
             return None
@@ -226,7 +527,7 @@ class DeviceStream:
                 C.byref(nn), _lib.ptr(self.kind), _lib.ptr(self.name_event), _lib.ptr(self.name_which), self.cap,
                 C.c_void_p(ws_ptr), self._ws_bytes, _lib.current_stream_ptr()), "nerrf_trace_intern_device")
         N = int(nn.value)
-        t0 = float(self.ts_sorted[lo]); span = max(float(self.ts_sorted[hi - 1]) - t0, 1e-6)
+        t0 = t_first; span = max(t_last - t0, 1e-6)
         window = window_s or max(span, G.WINDOW)
         P, F = self.node_p[sel], self.node_f[sel]                   # by rank: the window's events in time order
         t = self.d_ts[sel] - t0
@@ -257,7 +558,10 @@ class DeviceStream:
                                                         _lib.ptr(self.d_poff), _lib.ptr(self.d_pdata), _lib.ptr(self.d_goff),
                                                         _lib.ptr(self.d_gdata), _lib.ptr(nh), _lib.current_stream_ptr()),
                        "nerrf_trace_name_hash")
-        meta = {"kind": "trace", "names": LazyNames(self.cols, self.name_event[:N].cpu().numpy(), self.name_which[:N].cpu().numpy()),
+        ne, nwh = self.name_event[:N].cpu().numpy(), self.name_which[:N].cpu().numpy()
+        names = LazyNames(self.cols, ne, nwh) if self.cols is not None else \
+            DeviceNames(self.d_pid, self.d_poff, self.d_pdata, self.d_goff, self.d_gdata, ne, nwh)
+        meta = {"kind": "trace", "names": names,
                 "node_kind": kind_d.cpu().numpy().astype(np.int64), "t0": t0, "span": span, "merge_renames": self.merge,
                 "label": lab.cpu().numpy().astype(np.int64), "size_mb": size_mb.cpu().numpy(), "device": str(self.dev),
                 "name_hash": nh, "events": nw, "window_ranks": (lo, hi), "perm": perm if Gn is None else None}
@@ -289,6 +593,9 @@ class DeviceStream:
 
     def sequences(self, g: G.TemporalGraph, only_nodes):
         """LSTM sequences of the given file nodes of window graph `g` (ingest.sequences_core on the window's events)."""
+        if self.cols is None:
+            from . import _lib
+            raise _lib.NerrfError("a live stream builds its sequences on the device (sequences_device)")
         lo, hi = g.meta["window_ranks"]
         order = self.order[lo:hi]
         if "_F_host" not in g.meta:
@@ -330,11 +637,61 @@ class StreamingPlanner:
     ingest_ms: float = 0.0         # one-time: stream columns -> HBM (DeviceStream)
     killed: set = field(default_factory=set)
     ticks: list = field(default_factory=list)
+    lateness_s: float = 0.0        # live feed: a tick at t_hi fires once an event with ts > t_hi + lateness_s has arrived
+    live: object = None            # live feed: the DeviceStream the bytes go to
+    _carry: bytes = b""
+    _t0: float = None
+    _t_hi: float = None
+
+    def feed(self, chunk) -> list:
+        """Live form of run(): `chunk` = the next bytes of the tracker's EventBatch stream, cut anywhere (a partial record
+        is carried over to the next call).  The bytes are decoded and appended on the device; every tick that can no
+        longer change fires.  -> the TickResults fired by this call.  Ticks, windows and plans are those run() computes
+        over the whole stream when no event arrives more than lateness_s late."""
+        if self.dist_ctx is not None and self.dist_ctx.world > 1:
+            raise NotImplementedError("live feeding runs on one GPU")
+        if self.live is None:
+            self.live = DeviceStream.live(self.device, observable=True)
+        buf = self._carry + bytes(chunk)
+        used = self.live.append(buf, partial=True)
+        self._carry = buf[used:]
+        return self._fire(final=False)
+
+    def flush(self) -> list:
+        """End of the stream: fire the remaining ticks, the last one at the last event (like run()).  A carried-over
+        partial record is malformed input."""
+        if self.live is None:
+            return []
+        if self._carry:
+            self.live.append(self._carry)                      # raises: the stream ended inside a record
+        return self._fire(final=True)
+
+    def _fire(self, final: bool) -> list:
+        import torch
+        ds, out = self.live, []
+        dev = torch.device(self.device)
+        while ds.n_keep:
+            first, last = ds.span()
+            t0 = self._t0 if self._t0 is not None else first     # fixed by the first tick: earlier events have arrived
+            t_hi = self._t_hi if self._t_hi is not None else t0
+            if final:
+                if not t_hi < last:
+                    break
+                nxt = min(t_hi + self.tick_s, last)
+            else:
+                nxt = t_hi + self.tick_s
+                if not last > nxt + self.lateness_s:
+                    break
+            self._t0, self._t_hi = t0, nxt
+            k = len(self.ticks)
+            self._tick(ds, nxt, t0, dev, True, False, None)
+            out += self.ticks[k:]
+            ds.compact(nxt - self.window_s)                      # no later window reaches back past this tick's
+        return out
 
     def run(self, cols: ingest.EventColumns):
         """cols: the event stream (multi-GPU: only rank 0's copy is read -- rank 0 does the host-side ingest of every tick
         and broadcasts the device graph, the exclusion mask and the candidates' sequences; names stay on rank 0)."""
-        from . import pipeline
         import time
         import torch
         ctx = self.dist_ctx
@@ -370,78 +727,89 @@ class StreamingPlanner:
         t_hi = t0
         while t_hi < t1:
             t_hi = min(t_hi + self.tick_s, t1)
-            tm = {}
-            names, g, n_events = None, None, 0
-            a = time.perf_counter()
-            if lead:
-                # window = a slice of the time-sorted index array; interning (hash table), features, edges, CSR on the GPU
-                g = ds.window_graph(t_hi - self.window_s, t_hi, self.window_s)
-                torch.cuda.synchronize()
-                n_events = g.meta["events"] if g is not None else 0
-            if multi:
-                ne = torch.tensor([n_events], device=dev); dist.broadcast(ne, 0); n_events = int(ne)
-            if n_events == 0:
-                continue
-            if lead:
-                names = g.meta["names"]
-            if multi:                                      # the device graph travels over NVLink; the strings do not
-                x = bcast(g.x if lead else None, dtype=torch.float32)
-                rp = bcast(g.rowptr.to(torch.int64) if lead else None, dtype=torch.int64).to(torch.int32)
-                col = bcast(g.col if lead else None, dtype=torch.int32)
-                ew = bcast(g.ew if lead else None, dtype=torch.float32)
-                kind_t = bcast(torch.from_numpy(np.asarray(g.meta["node_kind"]).astype(np.int64)) if lead else None, dtype=torch.int64)
-                size_t = bcast(torch.from_numpy(np.asarray(g.meta["size_mb"], np.float32)) if lead else None, dtype=torch.float32)
-                if not lead:
-                    g = G.TemporalGraph(rp, col, ew, x, {"kind": "trace", "node_kind": kind_t.cpu().numpy(), "size_mb": size_t.cpu().numpy()})
-            tm["graph_build"] = (time.perf_counter() - a) * 1e3
-            kind = np.asarray(g.meta["node_kind"])
-            nodes = np.nonzero(kind == 0)[0]
-
-            # LSTM sequences are built lazily, for the top-A candidates only (a window holds ~10^6 file nodes)
-            def seq(cand, g=g):
-                if lead and not multi:                      # built on the device from the resident columns, in candidate order
-                    sq_d, ln_d = ds.sequences_device(g, cand)
-                    return sq_d, ln_d, None
-                if lead:
-                    sq, ln, have = ds.sequences(g, cand)
-                if multi:
-                    sq_t = bcast(torch.from_numpy(sq) if lead else None, dtype=torch.float32)
-                    ln_t = bcast(torch.from_numpy(ln) if lead else None, dtype=torch.int32)
-                    hv_t = bcast(torch.from_numpy(have) if lead else None, dtype=torch.int64)
-                    return sq_t.cpu().numpy(), ln_t.cpu().numpy(), hv_t.cpu().numpy()
-                return sq, ln, have
-
-            new, truncated = [], False
-            for rnd in range(4):
-                # a planning pass proposes at most 32 process kills (planner spec v1: guards live in state word 0); a tick
-                # with more suspicious processes than that plans again over what is still unreverted
-                skip = None
-                if lead and self.reverted:               # files already reverted by an earlier tick: matched by name hash on the device
-                    rh = torch.tensor(sorted(self._reverted_hash), dtype=torch.int64, device=dev)
-                    skip = torch.isin(g.meta["name_hash"][torch.from_numpy(nodes).to(dev)], rh).cpu().numpy()
-                if multi:
-                    flag = torch.tensor([1 if (lead and skip is not None) else 0], device=dev); dist.broadcast(flag, 0)
-                    if int(flag):
-                        skip = bcast(torch.from_numpy(skip) if lead else None, shape=[nodes.shape[0]], dtype=torch.bool).cpu().numpy()
-                res = pipeline.run(g, seq, None, nodes, self.model, self.scorer, top_a=self.top_a, n_rollouts=self.n_rollouts,
-                                   depth=self.depth, iterations=self.iterations, device=self.device, exclude=skip,
-                                   commit_per_search=self.commit_per_search, dist_ctx=self.dist_ctx,
-                                   kill_candidates=self.kill_candidates)
-                for k, v in res.timings_ms.items():
-                    tm[k] = tm.get(k, 0.0) + float(v)
-                got = []
-                if lead:
-                    self.killed.update(names[n] for n in res.plan_nodes if kind[n] == 1)
-                    got = [names[n] for n in res.plan_nodes if kind[n] == 0]
-                    got = [nm for nm in dict.fromkeys(got) if nm not in self.reverted]
-                    self.reverted.update(got)
-                    self._reverted_hash.update(name_hash(nm) for nm in got)
-                    new += got
-                more = bool(self.kill_candidates and res.n_kill >= 32 and got)
-                if multi:
-                    flag = torch.tensor([int(more)], device=dev); dist.broadcast(flag, 0); more = bool(int(flag))
-                truncated = truncated or bool(res.plan.truncated)
-                if not more:
-                    break
-            self.ticks.append(TickResult(t_hi - t0, n_events, g.num_nodes, g.num_edges, new, tm, truncated))
+            self._tick(ds, t_hi, t0, dev, lead, multi, bcast if multi else None)
         return self.ticks
+
+    def _tick(self, ds, t_hi, t0, dev, lead, multi, bcast):
+        """One tick: the window (t_hi - window_s, t_hi] becomes a graph, is scored and planned; appends a TickResult
+        (nothing when the window is empty).  Shared by run() and the live loop (feed / flush)."""
+        from . import pipeline
+        import time
+        import torch
+        if multi:
+            import torch.distributed as dist
+        tm = {}
+        names, g, n_events = None, None, 0
+        a = time.perf_counter()
+        if lead:
+            # window = a slice of the time-sorted index array; interning (hash table), features, edges, CSR on the GPU
+            g = ds.window_graph(t_hi - self.window_s, t_hi, self.window_s)
+            torch.cuda.synchronize()
+            n_events = g.meta["events"] if g is not None else 0
+        if multi:
+            ne = torch.tensor([n_events], device=dev); dist.broadcast(ne, 0); n_events = int(ne)
+        if n_events == 0:
+            return
+        if lead:
+            names = g.meta["names"]
+        if multi:                                      # the device graph travels over NVLink; the strings do not
+            x = bcast(g.x if lead else None, dtype=torch.float32)
+            rp = bcast(g.rowptr.to(torch.int64) if lead else None, dtype=torch.int64).to(torch.int32)
+            col = bcast(g.col if lead else None, dtype=torch.int32)
+            ew = bcast(g.ew if lead else None, dtype=torch.float32)
+            kind_t = bcast(torch.from_numpy(np.asarray(g.meta["node_kind"]).astype(np.int64)) if lead else None, dtype=torch.int64)
+            size_t = bcast(torch.from_numpy(np.asarray(g.meta["size_mb"], np.float32)) if lead else None, dtype=torch.float32)
+            if not lead:
+                g = G.TemporalGraph(rp, col, ew, x, {"kind": "trace", "node_kind": kind_t.cpu().numpy(), "size_mb": size_t.cpu().numpy()})
+        tm["graph_build"] = (time.perf_counter() - a) * 1e3
+        kind = np.asarray(g.meta["node_kind"])
+        nodes = np.nonzero(kind == 0)[0]
+
+        # LSTM sequences are built lazily, for the top-A candidates only (a window holds ~10^6 file nodes)
+        def seq(cand, g=g):
+            if lead and not multi:                      # built on the device from the resident columns, in candidate order
+                sq_d, ln_d = ds.sequences_device(g, cand)
+                return sq_d, ln_d, None
+            if lead:
+                sq, ln, have = ds.sequences(g, cand)
+            if multi:
+                sq_t = bcast(torch.from_numpy(sq) if lead else None, dtype=torch.float32)
+                ln_t = bcast(torch.from_numpy(ln) if lead else None, dtype=torch.int32)
+                hv_t = bcast(torch.from_numpy(have) if lead else None, dtype=torch.int64)
+                return sq_t.cpu().numpy(), ln_t.cpu().numpy(), hv_t.cpu().numpy()
+            return sq, ln, have
+
+        new, truncated = [], False
+        for rnd in range(4):
+            # a planning pass proposes at most 32 process kills (planner spec v1: guards live in state word 0); a tick
+            # with more suspicious processes than that plans again over what is still unreverted
+            skip = None
+            if lead and self.reverted:               # files already reverted by an earlier tick: matched by name hash on the device
+                rh = torch.tensor(sorted(self._reverted_hash), dtype=torch.int64, device=dev)
+                skip = torch.isin(g.meta["name_hash"][torch.from_numpy(nodes).to(dev)], rh).cpu().numpy()
+            if multi:
+                flag = torch.tensor([1 if (lead and skip is not None) else 0], device=dev); dist.broadcast(flag, 0)
+                if int(flag):
+                    skip = bcast(torch.from_numpy(skip) if lead else None, shape=[nodes.shape[0]], dtype=torch.bool).cpu().numpy()
+            res = pipeline.run(g, seq, None, nodes, self.model, self.scorer, top_a=self.top_a, n_rollouts=self.n_rollouts,
+                               depth=self.depth, iterations=self.iterations, device=self.device, exclude=skip,
+                               commit_per_search=self.commit_per_search, dist_ctx=self.dist_ctx,
+                               kill_candidates=self.kill_candidates)
+            for k, v in res.timings_ms.items():
+                tm[k] = tm.get(k, 0.0) + float(v)
+            got = []
+            if lead:
+                plan_names = names.take(res.plan_nodes)           # one bulk fetch (device names of a live stream)
+                self.killed.update(nm for n, nm in zip(res.plan_nodes, plan_names) if kind[n] == 1)
+                got = [nm for n, nm in zip(res.plan_nodes, plan_names) if kind[n] == 0]
+                got = [nm for nm in dict.fromkeys(got) if nm not in self.reverted]
+                self.reverted.update(got)
+                self._reverted_hash.update(name_hash(nm) for nm in got)
+                new += got
+            more = bool(self.kill_candidates and res.n_kill >= 32 and got)
+            if multi:
+                flag = torch.tensor([int(more)], device=dev); dist.broadcast(flag, 0); more = bool(int(flag))
+            truncated = truncated or bool(res.plan.truncated)
+            if not more:
+                break
+        self.ticks.append(TickResult(t_hi - t0, n_events, g.num_nodes, g.num_edges, new, tm, truncated))
