@@ -193,6 +193,17 @@ int nerrf_sage_session_destroy(nerrf_sage_session* s);
  * additionally loses p_guard * p_a * size_a (the live process re-encrypts the file).  NULL = spec v0. */
 int nerrf_reward_score(const uint32_t* states, int64_t B, const float* p, const float* size,
                        const float* cost, const int32_t* guard, int A, float* out, nerrf_stream_t stream);
+/* Planner spec v2: cover (int32 [A], or NULL; device pointer here and in the device-pointer entry points below, host
+ * pointer in the *_host_ex ones) -- cover[a] = index (0..31, < A) of the "restore from backup" action
+ * (threat-model.mdx:216-219) of the directory that holds a's file, or -1.  An action that is not applied but whose cover
+ * is applied is restored all the same: its data-loss term is (1-p_a)*size_a (plus the guard penalty while its guard is
+ * not applied) and it adds no downtime.  cover[a] != a; a cover target is not covered itself and is not a guard target
+ * (otherwise NERRF_ERR_INVALID).  The check reads `cover` and `guard` back to the host, so with a cover table a
+ * device-pointer call synchronizes its stream before it launches.  Each *_ex entry point takes `cover` right after
+ * `guard`; the plain symbols are the *_ex ones with cover = NULL (spec v1, bit for bit). */
+int nerrf_reward_score_ex(const uint32_t* states, int64_t B, const float* p, const float* size,
+                          const float* cost, const int32_t* guard, const int32_t* cover, int A, float* out,
+                          nerrf_stream_t stream);
 
 /* ------------------------------------------------------------------ planner.mcts.search (a5)
  * Replaces: ai/planner/mcts.py (README.md:74, ROADMAP.md:84; architecture.mdx:62-72).
@@ -207,12 +218,20 @@ int nerrf_mcts_search(const float* p, const float* size, const float* cost, cons
                       float lo, float inv_range, const float* ln_table, int32_t* root_n,
                       float* root_w, int32_t* num_nodes, void* workspace, size_t workspace_bytes,
                       nerrf_stream_t stream);
+int nerrf_mcts_search_ex(const float* p, const float* size, const float* cost, const int32_t* guard,
+                         const int32_t* cover, int A, const uint32_t* root_state, int R, int D, int T, uint64_t seed,
+                         float c, float lo, float inv_range, const float* ln_table, int32_t* root_n, float* root_w,
+                         int32_t* num_nodes, void* workspace, size_t workspace_bytes, nerrf_stream_t stream);
 /* HOST in / HOST out, one-shot (allocates + frees device memory internally, synchronous).
  * root_state_host and guard may be NULL. */
 int nerrf_mcts_search_host(const float* p, const float* size, const float* cost, const int32_t* guard, int A,
                            const uint32_t* root_state_host, int R, int D, int T, uint64_t seed,
                            float c, float lo, float inv_range, const float* ln_table_host,
                            int32_t* root_n_host, float* root_w_host, int32_t* num_nodes_host);
+int nerrf_mcts_search_host_ex(const float* p, const float* size, const float* cost, const int32_t* guard,
+                              const int32_t* cover, int A, const uint32_t* root_state_host, int R, int D, int T,
+                              uint64_t seed, float c, float lo, float inv_range, const float* ln_table_host,
+                              int32_t* root_n_host, float* root_w_host, int32_t* num_nodes_host);
 /* plan(): validate-and-commit loop on the device (architecture.mdx:81-86 "sandbox validates, then apply"; the commit half of
  * ai/planner/mcts.py plan()).  cand[n_cand] (device int32, ranked root children of a search) are scored as score(state + c)
  * with the exact reward; the highest-ranked improving one is committed, the candidates that still improved stay in the list;
@@ -225,6 +244,10 @@ int nerrf_plan_commit(const float* p, const float* size, const float* cost, cons
                       uint32_t* state, const int32_t* cand, int n_cand, float cur, int max_commits,
                       int allow_tentative, int32_t* actions_out, float* scores_out, int32_t* n_out,
                       void* workspace, size_t workspace_bytes, nerrf_stream_t stream);
+int nerrf_plan_commit_ex(const float* p, const float* size, const float* cost, const int32_t* guard,
+                         const int32_t* cover, int A, uint32_t* state, const int32_t* cand, int n_cand, float cur,
+                         int max_commits, int allow_tentative, int32_t* actions_out, float* scores_out, int32_t* n_out,
+                         void* workspace, size_t workspace_bytes, nerrf_stream_t stream);
 
 /* HOST in / HOST out through a session: the device buffers and a stream live in the handle (create once for the
  * largest A / T / R; a search is then six small H2D copies, one launch and three D2H copies, no allocation).
@@ -235,6 +258,11 @@ int nerrf_mcts_session_search_host(nerrf_mcts_session* s, const float* p, const 
                                    const int32_t* guard, int A, const uint32_t* root_state_host, int R, int D, int T,
                                    uint64_t seed, float c, float lo, float inv_range, const float* ln_table_host,
                                    int32_t* root_n_host, float* root_w_host, int32_t* num_nodes_host);
+int nerrf_mcts_session_search_host_ex(nerrf_mcts_session* s, const float* p, const float* size, const float* cost,
+                                      const int32_t* guard, const int32_t* cover, int A, const uint32_t* root_state_host,
+                                      int R, int D, int T, uint64_t seed, float c, float lo, float inv_range,
+                                      const float* ln_table_host, int32_t* root_n_host, float* root_w_host,
+                                      int32_t* num_nodes_host);
 int nerrf_mcts_session_destroy(nerrf_mcts_session* s);
 
 /* ------------------------------------------------------------------ lstm.forward (row a4)
@@ -440,6 +468,12 @@ int nerrf_trace_intern_device(int64_t n_events, int64_t n_stored, const int64_t*
 int nerrf_trace_name_hash(int64_t n_nodes, const int64_t* node_name_event, const int8_t* node_name_which,
                           const uint32_t* pid, const int64_t* path_off, const uint8_t* path_data,
                           const int64_t* new_path_off, const uint8_t* new_path_data, uint64_t* hash_out, void* stream);
+/* The same hash over each node's parent DIRECTORY: the bytes of its name up to (not including) the last '/' (none: the
+ * empty string); pid nodes hash as in nerrf_trace_name_hash.  Groups file nodes by directory for the planner's
+ * "restore from backup" candidates.  Equals nerrf_b200/stream.py dir_hash bit for bit. */
+int nerrf_trace_dir_hash(int64_t n_nodes, const int64_t* node_name_event, const int8_t* node_name_which,
+                         const uint32_t* pid, const int64_t* path_off, const uint8_t* path_data,
+                         const int64_t* new_path_off, const uint8_t* new_path_data, uint64_t* hash_out, void* stream);
 int nerrf_trace_intern(int64_t n_events, const int64_t* order, const uint32_t* pid,
                        const int64_t* path_off, const uint8_t* path_data,
                        const int64_t* new_path_off, const uint8_t* new_path_data, int merge_renames,

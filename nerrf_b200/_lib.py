@@ -60,6 +60,15 @@ SIGNATURES = {
     "nerrf_mcts_session_search_host": (C.c_int, [vp, vp, vp, vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_uint64,
                                                  C.c_float, C.c_float, C.c_float, vp, vp, vp, vp]),
     "nerrf_mcts_session_destroy": (C.c_int, [vp]),
+    "nerrf_reward_score_ex": (C.c_int, [vp, C.c_int64, vp, vp, vp, vp, vp, C.c_int, vp, vp]),
+    "nerrf_mcts_search_ex": (C.c_int, [vp, vp, vp, vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_float,
+                                       C.c_float, C.c_float, vp, vp, vp, vp, vp, C.c_size_t, vp]),
+    "nerrf_mcts_search_host_ex": (C.c_int, [vp, vp, vp, vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_uint64, C.c_float,
+                                            C.c_float, C.c_float, vp, vp, vp, vp]),
+    "nerrf_plan_commit_ex": (C.c_int, [vp, vp, vp, vp, vp, C.c_int, vp, vp, C.c_int, C.c_float, C.c_int, C.c_int, vp, vp, vp, vp,
+                                       C.c_size_t, vp]),
+    "nerrf_mcts_session_search_host_ex": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_int, C.c_uint64,
+                                                    C.c_float, C.c_float, C.c_float, vp, vp, vp, vp]),
     "nerrf_lstm_workspace_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
     "nerrf_lstm_forward": (C.c_int, [vp, vp, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp),
                                      C.POINTER(vp), C.POINTER(vp), vp, vp, vp, vp, C.c_size_t, vp]),
@@ -95,6 +104,7 @@ SIGNATURES = {
     "nerrf_trace_intern_device": (C.c_int, [C.c_int64, C.c_int64, vp, vp, vp, vp, vp, vp, C.c_int, vp, vp, vp, C.POINTER(C.c_int64),
                                             vp, vp, vp, C.c_int64, vp, C.c_int64, vp]),
     "nerrf_trace_name_hash": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "nerrf_trace_dir_hash": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "nerrf_trace_intern": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, C.c_int, vp, vp, vp, C.POINTER(C.c_int64),
                                      vp, vp, vp, C.c_int64]),
 }

@@ -44,15 +44,37 @@ def reversion_for(path: str) -> dict:
     return r
 
 
+def restore_dir_step(directory: str, covered_paths) -> dict:
+    """One directory restore from the pre-attack snapshot (threat-model.mdx:216-219 "Restore from backup"): brings back
+    every file of `directory`; the sandbox checks each covered file against its pre-attack md5."""
+    r = {"op": "restore_snapshot_dir", "dir": directory, "covers": list(covered_paths),
+         "validate": [{"check": "md5", "path": p_, "against": "pre_attack_snapshot"} for p_ in covered_paths]}
+    if _has_control_chars(directory) or any(_has_control_chars(p_) for p_ in covered_paths):
+        r["hostile_name"] = True
+    return r
+
+
 def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node_score=None, truncated=False,
-              remaining_candidates=0) -> dict:
+              remaining_candidates=0, restores=None) -> dict:
     """names: node id -> path (TemporalGraph.meta['names']); plan_nodes: node ids to revert, in plan order
     (PipelineResult.plan_nodes); scores: Plan.scores (exact reward after each commit, scores[0] = before).
     truncated / remaining_candidates: the planner stopped at its step limit while improving candidates remained --
-    such a plan must not be auto-approved as complete."""
+    such a plan must not be auto-approved as complete.
+    restores: PipelineResult.restores -- directory restores, each at its position in the plan ({"position", "dir",
+    "covers": node ids}); the node steps fill the other positions in order."""
+    at = {int(r["position"]): r for r in (restores or [])}
+    total = len(plan_nodes) + len(at)
+    nodes = iter(plan_nodes)
     steps = []
-    for k, n in enumerate(plan_nodes):
-        n = int(n)
+    for k in range(total):
+        if k in at:
+            r = at[k]
+            step = {"order": k, **restore_dir_step(r["dir"], [names[int(c)] for c in r["covers"]])}
+            if scores is not None and k + 1 < len(scores):
+                step["reward_after"] = float(scores[k + 1])
+            steps.append(step)
+            continue
+        n = int(next(nodes))
         step = {"order": k, "node": n, **reversion_for(names[n]),
                 "validate": {"check": "md5", "against": "pre_attack_snapshot"}}
         if size_mb is not None:
@@ -67,7 +89,7 @@ def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node
            "truncated": bool(truncated), "remaining_candidates": int(remaining_candidates)}
     if scores:
         out["reward_before"] = float(scores[0])
-        out["reward_after"] = float(scores[min(len(plan_nodes), len(scores) - 1)])
+        out["reward_after"] = float(scores[min(total, len(scores) - 1)])
     return out
 
 
@@ -81,6 +103,9 @@ def to_shell(plan: dict) -> str:
     for s in plan["steps"]:
         if s["op"] == "rename":
             lines.append("mv -- %s %s" % (shlex.quote(s["from"]), shlex.quote(s["to"])))
+        elif s["op"] == "restore_snapshot_dir":
+            # the directory is only ever a single-quoted ARGUMENT of the `:` no-op (see below)
+            lines.append(": restore-dir-from-pre-attack-snapshot %s" % shlex.quote(s["dir"]))
         else:
             # never a comment: a newline inside a path would end the comment and start a command.  `:` is the
             # POSIX no-op; the path is only ever a single-quoted ARGUMENT (newlines inside '...' are literal).
@@ -93,4 +118,5 @@ def from_pipeline(g, result, attack_id=None) -> dict:
     score = result.node_score.detach().cpu().numpy() if hasattr(result.node_score, "detach") else result.node_score
     return undo_plan(g.meta["names"], result.plan_nodes, scores=result.plan.scores, attack_id=attack_id,
                      size_mb=g.meta.get("size_mb"), node_score=score, truncated=getattr(result.plan, "truncated", False),
-                     remaining_candidates=getattr(result.plan, "remaining_candidates", 0))
+                     remaining_candidates=getattr(result.plan, "remaining_candidates", 0),
+                     restores=getattr(result, "restores", None))

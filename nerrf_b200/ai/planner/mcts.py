@@ -82,6 +82,7 @@ class SearchContext:
         with torch.cuda.device(self.device):
             self.p, self.size, self.cost = actions.device_arrays(self.device)
             self.guard = actions.device_guard(self.device)
+            self.cover = actions.device_cover(self.device)
             self.d_ln = torch.from_numpy(ln_table(self.T, self.R)).to(self.device)
             self.d_root = torch.empty(self.nw, device=self.device, dtype=torch.int32)
             # root_n | root_w | num_nodes in one buffer -> one D2H
@@ -101,11 +102,12 @@ class SearchContext:
         self.h_root.copy_(torch.from_numpy(root.view(np.int32)))
         self.d_root.copy_(self.h_root, non_blocking=True)
         o = self.d_out
-        L.check(L.lib().nerrf_mcts_search(L.ptr(self.p), L.ptr(self.size), L.ptr(self.cost), L.ptr(self.guard), A, L.ptr(self.d_root), self.R,
+        L.check(L.lib().nerrf_mcts_search_ex(L.ptr(self.p), L.ptr(self.size), L.ptr(self.cost), L.ptr(self.guard), L.ptr(self.cover),
+                                             A, L.ptr(self.d_root), self.R,
                                           self.D if depth is None else int(depth), self.T, C.c_uint64(seed), self.c,
                                           float(lo), float(inv), L.ptr(self.d_ln), C.c_void_p(o.data_ptr()),
                                           C.c_void_p(o.data_ptr() + 4 * self.A_pad), C.c_void_p(o.data_ptr() + 8 * self.A_pad),
-                                          L.ptr(self.ws), self.ws_bytes, L.current_stream_ptr()), "nerrf_mcts_search")
+                                          L.ptr(self.ws), self.ws_bytes, L.current_stream_ptr()), "nerrf_mcts_search_ex")
         return float(lo), float(inv)
 
     def fetch(self, lo, inv) -> "SearchResult":
@@ -167,15 +169,16 @@ def search(actions: Actions, scorer=None, n_rollouts: int = 4096, depth: int = 5
         root_n = np.zeros(A_pad, np.int32); root_w = np.zeros(A_pad, np.float32); nn = np.zeros(1, np.int32)
         as_p = lambda a: a.ctypes.data_as(C.c_void_p)
         gp = as_p(actions.guard) if actions.guard is not None else None
+        cp = as_p(actions.cover) if actions.cover is not None else None
         if isinstance(host_call, HostSession):
-            L.check(L.lib().nerrf_mcts_session_search_host(host_call.handle, as_p(actions.p), as_p(actions.size), as_p(actions.cost), gp,
-                                                           A, as_p(root), R, D, T, C.c_uint64(seed), float(c), float(lo), float(inv),
-                                                           as_p(lnN), as_p(root_n), as_p(root_w), as_p(nn)),
-                    "nerrf_mcts_session_search_host")
+            L.check(L.lib().nerrf_mcts_session_search_host_ex(host_call.handle, as_p(actions.p), as_p(actions.size), as_p(actions.cost),
+                                                              gp, cp, A, as_p(root), R, D, T, C.c_uint64(seed), float(c), float(lo),
+                                                              float(inv), as_p(lnN), as_p(root_n), as_p(root_w), as_p(nn)),
+                    "nerrf_mcts_session_search_host_ex")
         else:
-            L.check(L.lib().nerrf_mcts_search_host(as_p(actions.p), as_p(actions.size), as_p(actions.cost), gp, A, as_p(root), R, D, T,
-                                                   C.c_uint64(seed), float(c), float(lo), float(inv), as_p(lnN), as_p(root_n),
-                                                   as_p(root_w), as_p(nn)), "nerrf_mcts_search_host")
+            L.check(L.lib().nerrf_mcts_search_host_ex(as_p(actions.p), as_p(actions.size), as_p(actions.cost), gp, cp, A, as_p(root), R,
+                                                      D, T, C.c_uint64(seed), float(c), float(lo), float(inv), as_p(lnN), as_p(root_n),
+                                                      as_p(root_w), as_p(nn)), "nerrf_mcts_search_host_ex")
         return SearchResult(root_n[:A].copy(), root_w[:A].copy(), best_child(root_n[:A], root_w[:A]), int(nn[0]),
                             float(lo), float(inv), R * T)
     ctx = context or SearchContext(actions, R, D, T, c, device)
@@ -227,17 +230,64 @@ class _DeviceCommit:
             o = self.d_out
             st = o[2 * self.cap + 2:]
             st.copy_(torch.from_numpy(np.ascontiguousarray(state, np.uint32).view(np.int32)))
-            L.check(L.lib().nerrf_plan_commit(L.ptr(ctx.p), L.ptr(ctx.size), L.ptr(ctx.cost), L.ptr(ctx.guard), ctx.actions.A,
+            L.check(L.lib().nerrf_plan_commit_ex(L.ptr(ctx.p), L.ptr(ctx.size), L.ptr(ctx.cost), L.ptr(ctx.guard), L.ptr(ctx.cover),
+                                                 ctx.actions.A,
                                               C.c_void_p(st.data_ptr()), L.ptr(self.d_cand), n, C.c_float(cur), max_commits,
                                               int(bool(allow_tentative)), C.c_void_p(o.data_ptr()),
                                               C.c_void_p(o.data_ptr() + 4 * self.cap), C.c_void_p(o.data_ptr() + 8 * self.cap),
-                                              L.ptr(self.ws), self.ws_bytes, L.current_stream_ptr()), "nerrf_plan_commit")
+                                              L.ptr(self.ws), self.ws_bytes, L.current_stream_ptr()), "nerrf_plan_commit_ex")
             self.h_out.copy_(o, non_blocking=True)
             torch.cuda.current_stream().synchronize()
         h = self.h_out.numpy()
         k = int(h[2 * self.cap])
         return (h[:k].tolist(), h[self.cap:self.cap + k].view(np.float32).copy(), h[2 * self.cap + 2:].view(np.uint32).copy(),
                 int(h[2 * self.cap + 1]))
+
+
+def _states_with(actions: Actions, rows) -> np.ndarray:
+    st = np.repeat(RW.empty_state(actions.A)[None, :], len(rows), axis=0)
+    for i, acts in enumerate(rows):
+        for a_ in acts:
+            st[i, a_ >> 5] |= np.uint32(1) << np.uint32(a_ & 31)
+    return st
+
+
+def _refine_restores(actions: Actions, out: "Plan", device):
+    """Spec v2 clean-up of a finished plan (exact reward throughout; the plan order is kept, additions go last).
+    (1) The commit loop is greedy: a restore that beats "nothing reverted" is committed even when reverting its files one by
+    one would be better, and after it no reversion of those files can improve.  So each applied restore is compared with
+    its alternative -- the plan without it plus every reversion it covers that improves that plan on its own -- and the
+    better one is kept.  (2) A restore makes the reversions it covers pure downtime, but a reversion may have been
+    committed before its restore: committed actions whose removal improves the reward are dropped (all at once when that
+    is better still, else the best single one) until none is.  -> (final state, final score)."""
+    score = lambda rows: RW.score(_states_with(actions, rows), actions, device=device).cpu().numpy()
+    acts, cur = list(out.actions), np.float32(out.scores[-1])
+    for r in [a_ for a_ in acts if (actions.cover == a_).any()]:
+        base = [a_ for a_ in acts if a_ != r]
+        cov = [int(a_) for a_ in np.nonzero(actions.cover == r)[0] if int(a_) not in base]
+        if not cov:
+            continue
+        sc = score([base] + [base + [a_] for a_ in cov])
+        alt = base + [a_ for a_, v in zip(cov, sc[1:]) if v > sc[0]]
+        s_alt = score([alt])[0]
+        if s_alt > cur:
+            acts, cur = alt, s_alt
+    while len(acts) > 1:
+        sc = score([acts[:i] + acts[i + 1:] for i in range(len(acts))])
+        better = sc > cur
+        if not better.any():
+            break
+        rest = [a_ for a_, b in zip(acts, better) if not b]
+        s_all = score([rest])[0]
+        k = int(np.argmax(sc))
+        if s_all >= sc[k]:
+            acts, cur = rest, s_all
+        else:
+            acts, cur = acts[:k] + acts[k + 1:], sc[k]
+    if acts != list(out.actions):
+        pref = score([acts[:i] for i in range(1, len(acts) + 1)])
+        out.actions, out.scores = acts, out.scores[:1] + [float(v) for v in pref]
+    return _states_with(actions, [out.actions])[0], float(out.scores[-1])
 
 
 def plan(actions: Actions, max_steps: int | None = None, n_rollouts: int = 4096, depth: int = 50, seed: int = 0,
@@ -254,11 +304,15 @@ def plan(actions: Actions, max_steps: int | None = None, n_rollouts: int = 4096,
     would otherwise need one tree search per file).
     merge: root parallelism over several GPUs -- a callable (root_n, root_w) -> (root_n, root_w) that sums the root
     statistics of all ranks in rank order (nerrf_b200.dist); every rank then takes identical decisions.
-    lookahead (default: on when the actions carry guards, spec v1): the reward is then not separable -- killing a process
-    costs downtime and only pays off through the reversions it makes durable -- so a step that no single action improves
+    lookahead (default: on when the actions carry guards (spec v1) or covers (spec v2)): the reward is then not separable --
+    killing a process costs downtime and only pays off through the reversions it makes durable, a restore costs downtime
+    and makes the reversions it covers redundant -- so a step that no single action improves
     is not the end: the search's recommended child is committed TENTATIVELY, planning continues from there for at most
     `patience` steps below the best reward seen, and the plan is finally cut back to its best prefix (what the sandbox
     would approve).
+    With covers (spec v2) the finished plan is refined with the exact reward (_refine_restores): each applied restore is
+    weighed against reverting its files one by one, and committed actions whose removal improves the reward (a reversion
+    committed before the restore that covers it) are dropped.
     device_commit (default): the validate-and-commit loop runs on the device in one launch per search (nerrf_plan_commit);
     False keeps it as a host loop over rewards.score calls -- the same decisions bit for bit (tests compare the two)."""
     A = actions.A
@@ -269,7 +323,7 @@ def plan(actions: Actions, max_steps: int | None = None, n_rollouts: int = 4096,
     ctx = SearchContext(actions, n_rollouts, depth, iterations, c, device)
     dc = None
     step = 0
-    lookahead = (actions.guard is not None) if lookahead is None else lookahead
+    lookahead = (actions.guard is not None or actions.cover is not None) if lookahead is None else lookahead
     best_score, best_len = cur, 0
     while len(out.actions) < max_steps:
         # one-commit-per-search plans keep a total horizon of `depth` moves; batch-committing plans (large incidents)
@@ -321,6 +375,8 @@ def plan(actions: Actions, max_steps: int | None = None, n_rollouts: int = 4096,
         for a_ in out.actions:
             state[a_ >> 5] |= np.uint32(1) << np.uint32(a_ & 31)
         cur = best_score
+    if actions.cover is not None and out.actions:
+        state, cur = _refine_restores(actions, out, device)
     if len(out.actions) >= max_steps and len(out.actions) < A:
         # step limit hit: say so instead of handing back a silently incomplete plan (one batched exact-reward call)
         rest = np.array([a for a in range(A) if not (state[a >> 5] >> np.uint32(a & 31)) & np.uint32(1)], np.int64)

@@ -13,6 +13,12 @@ Spec v1 (DESIGN.md 1.3) adds the one non-separable term the reference's own cand
 -- the index (< 32) of the "kill process" action of the process that wrote its file.  An applied action whose guard
 is NOT applied additionally loses w_a = p_guard * p_a * size_a: the live process re-encrypts the reverted file.
 
+Spec v2 (DESIGN.md 1.3) gives the third candidate kind, "Restore from backup" (threat-model.mdx:216-219), its meaning:
+every action may name a COVER -- the index (< 32) of the restore action of the directory that holds its file.  An
+action that is not applied but whose cover is applied is restored all the same: it loses (1-p_a) size_a (plus w_a while
+its guard lives), like an applied action, but adds no downtime.  A restore action itself has p = 0 and size = the
+collateral it destroys (u = 0, v = collateral).
+
 States are bitsets: uint32 [B, n_words], action a = bit (a & 31) of word (a >> 5),
 n_words = 32*NW with NW = 1/2/4 for A <= 1024/2048/4096.
 """
@@ -40,6 +46,7 @@ class Actions:
     kind: np.ndarray | None = None
     names: list = field(default_factory=list)
     guard: np.ndarray | None = None      # int32 [A]: index (< 32) of the kill action guarding a, or -1 (spec v1)
+    cover: np.ndarray | None = None      # int32 [A]: index (< 32) of the restore action covering a, or -1 (spec v2)
 
     def __post_init__(self):
         self.p = np.ascontiguousarray(_np(self.p), dtype=np.float32)
@@ -54,6 +61,8 @@ class Actions:
             if g.shape != self.p.shape or (g < -1).any() or (g >= 32).any() or (g >= self.p.shape[0]).any():
                 raise ValueError("guard must be -1 or the index (< 32, < A) of the kill action, one per action")
             self.guard = g if (g >= 0).any() else None
+        if self.cover is not None:
+            self.cover = check_cover(self.cover, self.guard, self.p.shape[0])
 
     @property
     def A(self):
@@ -72,6 +81,27 @@ class Actions:
 
     def device_guard(self, device):
         return None if self.guard is None else torch.from_numpy(self.guard).to(device)
+
+    def device_cover(self, device):
+        return None if self.cover is None else torch.from_numpy(self.cover).to(device)
+
+
+def check_cover(cover, guard, A):
+    """Validated int32 [A] cover table, or None when no action is covered.  cover[a] is -1 or the index of a restore action
+    in state word 0 (< 32, < A), never a itself; a restore action is not covered itself (one level) and is no guard target."""
+    c = np.ascontiguousarray(_np(cover), dtype=np.int32)
+    if c.shape != (A,):
+        raise ValueError("cover must hold one entry per action")
+    if (c < -1).any() or (c >= min(32, A)).any():
+        raise ValueError("cover must be -1 or the index (< 32, < A) of the restore action, one per action")
+    if (c == np.arange(A)).any():
+        raise ValueError("an action cannot cover itself")
+    targets = np.unique(c[c >= 0])
+    if (c[targets] >= 0).any():
+        raise ValueError("a restore action cannot itself be covered (covers do not chain)")
+    if guard is not None and np.isin(targets, guard[guard >= 0]).any():
+        raise ValueError("an action cannot be both a guard and a cover target")
+    return c if targets.size else None
 
 
 def _np(a):
@@ -128,17 +158,19 @@ def score(states, actions: Actions, device=None) -> torch.Tensor:
     B = st.shape[0]
     p, size, cost = actions.device_arrays(device)
     guard = actions.device_guard(device)
+    cover = actions.device_cover(device)
     out = torch.empty(B, device=device, dtype=torch.float32)
     with torch.cuda.device(device):
-        L.check(L.lib().nerrf_reward_score(L.ptr(st), B, L.ptr(p), L.ptr(size), L.ptr(cost), L.ptr(guard), actions.A, L.ptr(out),
-                                           L.current_stream_ptr()), "nerrf_reward_score")
+        L.check(L.lib().nerrf_reward_score_ex(L.ptr(st), B, L.ptr(p), L.ptr(size), L.ptr(cost), L.ptr(guard), L.ptr(cover),
+                                              actions.A, L.ptr(out), L.current_stream_ptr()), "nerrf_reward_score_ex")
     return out
 
 
 def reward_bounds(actions: Actions, root_state=None):
     """(lo, inv_range): worst score over supersets of root_state and 1/(best - worst), so that
     value = (score - lo) * inv_range is in ~[0,1] for UCT.  float64 with exactly-rounded
-    summation (math.fsum), then rounded to fp32."""
+    summation (math.fsum), then rounded to fp32.  With covers (spec v2) an action that is not applied may still be
+    restored by its cover: its best case is then min(u, v, v + 0.1 cost), its worst case still includes vw."""
     A = actions.A
     p = actions.p; one = np.float32(1.0)
     u = (p * actions.size).astype(np.float32).astype(np.float64)
@@ -158,6 +190,8 @@ def reward_bounds(actions: Actions, root_state=None):
         fixed = ((rs[idx >> 5] >> (idx & 31).astype(np.uint32)) & np.uint32(1)) != 0
     worst = np.where(fixed, applied_worst, np.maximum(u, applied_worst))
     best = np.where(fixed, applied_cost, np.minimum(u, applied_cost))
+    if actions.cover is not None:              # a covered action may be restored without being applied: loss v, no downtime
+        best = np.where(~fixed & (actions.cover >= 0), np.minimum(best, v), best)
     lo = np.float32(-math.fsum(worst.tolist()))
     hi = -math.fsum(best.tolist())
     rng = hi - float(lo)

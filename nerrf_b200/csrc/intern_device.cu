@@ -228,6 +228,35 @@ __global__ void __launch_bounds__(256) name_hash_kernel(int64_t n_nodes, const i
     }
 }
 
+// 64-bit hash of every node's parent DIRECTORY: the name hash of the bytes of its name up to (not including) the last
+// '/' (no '/': the empty string); pid nodes hash their pid as in name_hash_kernel.  Groups file nodes by directory for the
+// planner's "restore from backup" candidates.  Same function as nerrf_b200/stream.py dir_hash.
+__device__ __forceinline__ int64_t dir_len_dev(const uint8_t* __restrict__ s, int64_t n) {
+    for (int64_t i = n - 1; i >= 0; --i)
+        if (s[i] == '/') return i;
+    return 0;
+}
+__global__ void __launch_bounds__(256) dir_hash_kernel(int64_t n_nodes, const int64_t* __restrict__ name_event,
+                                                       const int8_t* __restrict__ name_which, const uint32_t* __restrict__ pid,
+                                                       const int64_t* __restrict__ path_off, const uint8_t* __restrict__ path_data,
+                                                       const int64_t* __restrict__ gpath_off, const uint8_t* __restrict__ gpath_data,
+                                                       unsigned long long* __restrict__ out) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < n_nodes; v += stride) {
+        const int64_t e = name_event[v];
+        const int w = name_which[v];
+        unsigned long long h;
+        if (w == 2) {
+            h = mix64((uint64_t)pid[e] + 0x9E3779B97F4A7C15ull);
+        } else {
+            const uint8_t* s = w == 1 ? gpath_data + gpath_off[e] : path_data + path_off[e];
+            const int64_t n = w == 1 ? gpath_off[e + 1] - gpath_off[e] : path_off[e + 1] - path_off[e];
+            h = hash_bytes(s, dir_len_dev(s, n));
+        }
+        out[v] = h;
+    }
+}
+
 struct InternWs {
     size_t fkey, ffirst, pkey, pfirst, slot_p, slot_f, slot_g, flags, sums, total, err, name_code, bytes;
     uint32_t fcap, pcap;
@@ -337,4 +366,16 @@ extern "C" int nerrf_trace_name_hash(int64_t n_nodes, const int64_t* node_name_e
     name_hash_kernel<<<sm_count() * 8, 256, 0, (cudaStream_t)stream>>>(n_nodes, node_name_event, node_name_which, pid, path_off, path_data,
                                                                         new_path_off, new_path_data, (unsigned long long*)hash_out);
     return launch_status("name_hash_kernel");
+}
+
+extern "C" int nerrf_trace_dir_hash(int64_t n_nodes, const int64_t* node_name_event, const int8_t* node_name_which,
+                                    const uint32_t* pid, const int64_t* path_off, const uint8_t* path_data,
+                                    const int64_t* new_path_off, const uint8_t* new_path_data, uint64_t* hash_out, void* stream) {
+    NERRF_REQUIRE(n_nodes >= 0, "negative node count");
+    if (n_nodes == 0) return NERRF_OK;
+    NERRF_REQUIRE(node_name_event && node_name_which && pid && path_off && path_data && new_path_off && new_path_data && hash_out,
+                  "null pointer");
+    dir_hash_kernel<<<sm_count() * 8, 256, 0, (cudaStream_t)stream>>>(n_nodes, node_name_event, node_name_which, pid, path_off, path_data,
+                                                                       new_path_off, new_path_data, (unsigned long long*)hash_out);
+    return launch_status("dir_hash_kernel");
 }

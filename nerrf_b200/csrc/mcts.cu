@@ -21,7 +21,12 @@
 //            statistics of the leaf (fixed ascending-r order)
 // Reward spec v1 (oracle/rewards_ref.py): an applied action whose GUARD (a "kill process" action, index < 32, i.e. a
 // bit of state word 0) is not applied contributes vw_a = fl(v_a + fl(p_g * u_a)) instead of v_a.
+// Reward spec v2 (oracle/restore_ref.py): an action may also name a COVER -- the "restore from snapshot" action (index
+// < 32, state word 0) of its directory.  An action that is not applied but whose cover is applied is restored all the
+// same: its data-loss term is v_a (vw_a while its guard lives) and its downtime term is 0.
 #include "common.cuh"
+
+#include <vector>
 
 namespace nerrf {
 
@@ -48,28 +53,40 @@ __device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t
 // downtime term) PAIRS -- tab[0] = (u, 0) for an action that is NOT applied, tab[1] = (v, cost) applied, tab[2] = (vw, cost)
 // applied while its guard (kill) action is not -- so evaluating one action is one 8-byte shared load from the table the
 // state selects, + two rounded adds (r1/r2: five loads and three selects per action, ~600 instructions per state).
-struct TermsS { float2* tab; uint8_t* g; bool has_guard; };
+// Spec v2 (covers) adds two more tables -- ctab[0] = (v, 0) restored by its cover, ctab[1] = (vw, 0) restored while its
+// guard lives -- and the cover byte table.  They live in a separate region the caller places AFTER everything else the
+// kernel keeps in dynamic shared memory, and are only allocated when covers are passed: without covers every offset, the
+// shared-memory size and the occupancy are what they were in spec v1.
+struct TermsS { float2* tab; uint8_t* g; bool has_guard; float2* ctab; uint8_t* cv; bool has_cover; };
 template <int NW>
-__device__ __forceinline__ TermsS carve_terms(unsigned char* smem) {
+__device__ __forceinline__ TermsS carve_terms(unsigned char* smem, unsigned char* cover_smem) {
     constexpr int A_PAD = 1024 * NW;
     TermsS t;
     t.tab = reinterpret_cast<float2*>(smem);
     t.g = reinterpret_cast<uint8_t*>(t.tab + 3 * A_PAD);
     t.has_guard = false;
+    t.ctab = reinterpret_cast<float2*>(cover_smem);
+    t.cv = reinterpret_cast<uint8_t*>(t.ctab + 2 * A_PAD);
+    t.has_cover = false;
     return t;
 }
 template <int NW>
 constexpr size_t terms_smem_bytes() { return (size_t)1024 * NW * (3 * 8 + 1); }
+// the cover region (spec v2), appended only when covers are passed
+template <int NW>
+constexpr size_t cover_smem_bytes() { return (size_t)1024 * NW * (2 * 8 + 1); }
 // the search kernel appends one scratch bitset (32*NW words) per warp: the rank-space rollouts scatter their picks into it
 template <int NW>
 constexpr size_t mcts_smem_bytes() { return terms_smem_bytes<NW>() + (size_t)(896 / 32) * 32 * NW * 4; }
 
-// block-wide (contains a __syncthreads): fills the tables and reports whether any action has a guard
+// block-wide (contains __syncthreads): fills the tables and reports whether any action has a guard / a cover.  `cover` is
+// non-null only when the cover region was allocated.
 template <int NW>
 __device__ __forceinline__ void stage_terms(const float* __restrict__ p, const float* __restrict__ size,
-                                            const float* __restrict__ cost, const int32_t* __restrict__ guard, int A, TermsS& t) {
+                                            const float* __restrict__ cost, const int32_t* __restrict__ guard,
+                                            const int32_t* __restrict__ cover, int A, TermsS& t) {
     constexpr int CHUNK = 32 * NW, A_PAD = 1024 * NW;
-    int any = 0;
+    int any = 0, any_cover = 0;
     for (int a = threadIdx.x; a < A_PAD; a += blockDim.x) {
         float u = 0.f, v = 0.f, vw = 0.f, c = 0.f;
         int g = 255;
@@ -87,8 +104,17 @@ __device__ __forceinline__ void stage_terms(const float* __restrict__ p, const f
         t.tab[A_PAD + i * 32 + lane] = make_float2(v, c);
         t.tab[2 * A_PAD + i * 32 + lane] = make_float2(vw, c);
         t.g[i * 32 + lane] = (uint8_t)g;
+        if (cover) {                                                      // (uniform) spec v2
+            const int cd = a < A ? cover[a] : -1;
+            const bool on = cd >= 0 && cd < 32 && cd < A;
+            any_cover |= on ? 1 : 0;
+            t.ctab[i * 32 + lane] = make_float2(v, 0.f);
+            t.ctab[A_PAD + i * 32 + lane] = make_float2(vw, 0.f);
+            t.cv[i * 32 + lane] = (uint8_t)(on ? cd : 255);
+        }
     }
     t.has_guard = __syncthreads_or(any) != 0;
+    if (cover) t.has_cover = __syncthreads_or(any_cover) != 0;
 }
 
 // score of the state held across a warp (lane holds words w[0..NW)), spec'd order.  All lanes return it.
@@ -97,7 +123,26 @@ __device__ __forceinline__ float warp_score(const uint32_t (&w)[NW], const Terms
     constexpr int A_PAD = 1024 * NW;
     float dl = 0.f, dt = 0.f;
     const float2* tab = t.tab + lane;
-    if (!t.has_guard) {                                                   // (uniform) no guards: two tables
+    if (t.has_cover) {                                                    // (uniform) spec v2: guards and covers
+        const uint32_t w0 = __shfl_sync(0xffffffffu, w[0], 0);          // state word 0 holds the kill and restore actions
+        const float2* ctab = t.ctab + lane;
+#pragma unroll
+        for (int k = 0; k < NW; ++k) {
+#pragma unroll 8
+            for (int b = 0; b < 32; ++b) {
+                const int i = k * 32 + b;
+                const unsigned ap = (w[k] >> b) & 1u;
+                const unsigned gd = t.g[i * 32 + lane], cd = t.cv[i * 32 + lane];
+                const unsigned guard_alive = (gd < 32u && !((w0 >> (gd & 31u)) & 1u)) ? 1u : 0u;
+                const bool covered = cd < 32u && ((w0 >> (cd & 31u)) & 1u);
+                // applied: (v|vw, cost); restored by its cover only: (v|vw, 0); neither: (u, 0)
+                const float2* src = ap ? tab + (1u + guard_alive) * A_PAD : (covered ? ctab + guard_alive * A_PAD : tab);
+                const float2 e = src[i * 32];
+                dl = __fadd_rn(dl, e.x);
+                dt = __fadd_rn(dt, e.y);
+            }
+        }
+    } else if (!t.has_guard) {                                                   // (uniform) no guards: two tables
 #pragma unroll
         for (int k = 0; k < NW; ++k) {
 #pragma unroll 8
@@ -222,6 +267,7 @@ __device__ __forceinline__ void grid_barrier(unsigned* counter, unsigned& target
 struct MctsArgs {
     const float *p, *size, *cost;
     const int32_t* guard;   // [A] guard (kill action) index per action, or nullptr
+    const int32_t* cover;   // [A] cover (restore action) index per action, or nullptr (then no cover region in smem)
     int A;
     const uint32_t* root_state;
     int R, D, T;
@@ -246,7 +292,7 @@ __global__ void __launch_bounds__(MCTS_THREADS) mcts_search_kernel(MctsArgs P) {
     constexpr int A_PAD = 1024 * NW, NWORDS = 32 * NW;
     unsigned bar_target = 0;
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    TermsS terms = carve_terms<NW>(smem_raw);
+    TermsS terms = carve_terms<NW>(smem_raw, smem_raw + mcts_smem_bytes<NW>());
     uint32_t* const s_scratch = reinterpret_cast<uint32_t*>(smem_raw + terms_smem_bytes<NW>()) + (threadIdx.x >> 5) * NWORDS;
     __shared__ uint32_t s_state[NWORDS];
     __shared__ int2 s_path[MAXD];
@@ -262,7 +308,7 @@ __global__ void __launch_bounds__(MCTS_THREADS) mcts_search_kernel(MctsArgs P) {
     int32_t* const child_n = P.child_n + (size_t)blockIdx.x * P.node_stride * A_PAD;
     float* const child_w = P.child_w + (size_t)blockIdx.x * P.node_stride * A_PAD;
     int32_t* const child_id = P.child_id + (size_t)blockIdx.x * P.node_stride * A_PAD;
-    stage_terms<NW>(P.p, P.size, P.cost, P.guard, P.A, terms);
+    stage_terms<NW>(P.p, P.size, P.cost, P.guard, P.cover, P.A, terms);
     // the replica is initialised here, by its own CTA (no host memsets): T+1 node rows
     for (size_t i = tid; i < (size_t)(P.T + 1) * A_PAD; i += MCTS_THREADS) { child_n[i] = 0; child_w[i] = 0.f; child_id[i] = -1; }
     for (int i = tid; i <= P.T; i += MCTS_THREADS) visits[i] = 0;
@@ -605,10 +651,10 @@ template <int NW>
 __global__ void __launch_bounds__(256) reward_score_kernel(const uint32_t* __restrict__ states, int64_t B,
                                                            const float* __restrict__ p, const float* __restrict__ size,
                                                            const float* __restrict__ cost, const int32_t* __restrict__ guard,
-                                                           int A, float* __restrict__ out) {
+                                                           const int32_t* __restrict__ cover, int A, float* __restrict__ out) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    TermsS terms = carve_terms<NW>(smem_raw);
-    stage_terms<NW>(p, size, cost, guard, A, terms);
+    TermsS terms = carve_terms<NW>(smem_raw, smem_raw + terms_smem_bytes<NW>());
+    stage_terms<NW>(p, size, cost, guard, cover, A, terms);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int64_t s = (int64_t)blockIdx.x * 8 + warp; s < B; s += (int64_t)gridDim.x * 8) {
         uint32_t w[NW];
@@ -631,6 +677,7 @@ __global__ void __launch_bounds__(256) reward_score_kernel(const uint32_t* __res
 struct CommitArgs {
     const float *p, *size, *cost;
     const int32_t* guard;
+    const int32_t* cover;       // nullptr, or [A] (then the cover region follows the candidate list in smem)
     int A;
     uint32_t* state;            // [32*NW] in: the current state, out: the state after the commits
     const int32_t* cand;        // [n_cand] ranked candidates
@@ -649,14 +696,14 @@ template <int NW>
 __global__ void __launch_bounds__(256) plan_commit_kernel(CommitArgs P) {
     constexpr int NWORDS = 32 * NW;
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    TermsS terms = carve_terms<NW>(smem_raw);
+    TermsS terms = carve_terms<NW>(smem_raw, smem_raw + terms_smem_bytes<NW>() + 4096 * 4);
     int32_t* s_cand = reinterpret_cast<int32_t*>(smem_raw + terms_smem_bytes<NW>());          // [cap]
     __shared__ uint32_t s_state[NWORDS];
     __shared__ int s_first, s_cnt[8];
     __shared__ float s_cur;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     unsigned bar_target = 0;
-    stage_terms<NW>(P.p, P.size, P.cost, P.guard, P.A, terms);
+    stage_terms<NW>(P.p, P.size, P.cost, P.guard, P.cover, P.A, terms);
     for (int i = tid; i < P.n_cand; i += 256) s_cand[i] = P.cand[i];
     for (int k = tid; k < NWORDS; k += 256) s_state[k] = P.state[k];
     if (tid == 0) s_cur = P.cur;
@@ -765,7 +812,7 @@ static MctsLayout mcts_layout(int A, int T, int R) {
 
 template <int NW>
 static int launch_mcts(MctsArgs& args, int grid, cudaStream_t st) {
-    const size_t smem = mcts_smem_bytes<NW>();
+    const size_t smem = mcts_smem_bytes<NW>() + (args.cover ? cover_smem_bytes<NW>() : 0);
     const int rc = set_max_dynamic_smem((const void*)mcts_search_kernel<NW>, smem);
     if (rc) return rc;
     int per_sm = 0;
@@ -780,28 +827,61 @@ static int launch_mcts(MctsArgs& args, int grid, cudaStream_t st) {
 
 using namespace nerrf;
 
-extern "C" int nerrf_reward_score(const uint32_t* states, int64_t B, const float* p, const float* size,
-                                  const float* cost, const int32_t* guard, int A, float* out, nerrf_stream_t stream) {
+// Spec v2 cover table check (host side; `cover` / `guard` may be host or device pointers).  cover[a] is -1 or the index
+// of a restore action in word 0 (< 32, < A), never a itself; a restore action is not covered itself (one level), and no
+// index is both a guard and a cover target.
+static int check_cover(const int32_t* cover, const int32_t* guard, int A, cudaStream_t st) {
+    if (!cover) return NERRF_OK;
+    std::vector<int32_t> c((size_t)A), g((size_t)A, -1);
+    NERRF_CHECK_CUDA(cudaMemcpyAsync(c.data(), cover, (size_t)A * 4, cudaMemcpyDefault, st));
+    if (guard) NERRF_CHECK_CUDA(cudaMemcpyAsync(g.data(), guard, (size_t)A * 4, cudaMemcpyDefault, st));
+    NERRF_CHECK_CUDA(cudaStreamSynchronize(st));
+    const int lim = A < 32 ? A : 32;
+    bool target[32] = {false}, guard_target[32] = {false};
+    for (int a = 0; a < A; ++a) {
+        NERRF_REQUIRE(c[a] == -1 || (c[a] >= 0 && c[a] < lim), "cover[%d] = %d: must be -1 or a restore action index in 0..%d",
+                      a, c[a], lim - 1);
+        NERRF_REQUIRE(c[a] != a, "cover[%d] names the action itself", a);
+        if (c[a] >= 0) target[c[a]] = true;
+        if (g[a] >= 0 && g[a] < 32) guard_target[g[a]] = true;
+    }
+    for (int r = 0; r < lim; ++r) {
+        NERRF_REQUIRE(!target[r] || c[r] == -1, "restore action %d is itself covered (covers do not chain)", r);
+        NERRF_REQUIRE(!(target[r] && guard_target[r]), "action %d is both a guard and a cover target", r);
+    }
+    return NERRF_OK;
+}
+
+extern "C" int nerrf_reward_score_ex(const uint32_t* states, int64_t B, const float* p, const float* size,
+                                     const float* cost, const int32_t* guard, const int32_t* cover, int A, float* out,
+                                     nerrf_stream_t stream) {
     NERRF_REQUIRE(states && p && size && cost && out, "null pointer");
     NERRF_REQUIRE(A >= 1 && A <= 4096, "number of actions must be in 1..4096 (got %d)", A);
     NERRF_REQUIRE(B >= 0, "negative batch");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int rc0 = check_cover(cover, guard, A, st);
+    if (rc0) return rc0;
     if (B == 0) return NERRF_OK;
     const int NW = nw_for(A);
     int64_t g = (B + 7) / 8;
     const int64_t cap = (int64_t)sm_count() * 8;
     if (g > cap) g = cap;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (NW == 1) reward_score_kernel<1><<<(unsigned)g, 256, terms_smem_bytes<1>(), st>>>(states, B, p, size, cost, guard, A, out);
-    else if (NW == 2) {                                                   // 50 / 100 KB of staged terms: above the 48 KB default
-        const int rc = set_max_dynamic_smem((const void*)reward_score_kernel<2>, terms_smem_bytes<2>());
-        if (rc) return rc;
-        reward_score_kernel<2><<<(unsigned)g, 256, terms_smem_bytes<2>(), st>>>(states, B, p, size, cost, guard, A, out);
-    } else {
-        const int rc = set_max_dynamic_smem((const void*)reward_score_kernel<4>, terms_smem_bytes<4>());
-        if (rc) return rc;
-        reward_score_kernel<4><<<(unsigned)g, 256, terms_smem_bytes<4>(), st>>>(states, B, p, size, cost, guard, A, out);
-    }
-    return launch_status("reward_score_kernel");
+    auto go = [&](auto kern, size_t smem) -> int {
+        if (smem > 48 * 1024) {                                           // staged terms above the 48 KB default
+            const int rc = set_max_dynamic_smem((const void*)kern, smem);
+            if (rc) return rc;
+        }
+        kern<<<(unsigned)g, 256, smem, st>>>(states, B, p, size, cost, guard, cover, A, out);
+        return launch_status("reward_score_kernel");
+    };
+    if (NW == 1) return go(reward_score_kernel<1>, terms_smem_bytes<1>() + (cover ? cover_smem_bytes<1>() : 0));
+    if (NW == 2) return go(reward_score_kernel<2>, terms_smem_bytes<2>() + (cover ? cover_smem_bytes<2>() : 0));
+    return go(reward_score_kernel<4>, terms_smem_bytes<4>() + (cover ? cover_smem_bytes<4>() : 0));
+}
+
+extern "C" int nerrf_reward_score(const uint32_t* states, int64_t B, const float* p, const float* size,
+                                  const float* cost, const int32_t* guard, int A, float* out, nerrf_stream_t stream) {
+    return nerrf_reward_score_ex(states, B, p, size, cost, guard, nullptr, A, out, stream);
 }
 
 extern "C" int nerrf_mcts_workspace_bytes(int A, int T, int R, size_t* bytes) {
@@ -813,10 +893,10 @@ extern "C" int nerrf_mcts_workspace_bytes(int A, int T, int R, size_t* bytes) {
     return NERRF_OK;
 }
 
-extern "C" int nerrf_mcts_search(const float* p, const float* size, const float* cost, const int32_t* guard, int A,
-                                 const uint32_t* root_state, int R, int D, int T, uint64_t seed, float c, float lo,
-                                 float inv_range, const float* ln_table, int32_t* root_n, float* root_w, int32_t* num_nodes,
-                                 void* workspace, size_t workspace_bytes, nerrf_stream_t stream) {
+extern "C" int nerrf_mcts_search_ex(const float* p, const float* size, const float* cost, const int32_t* guard,
+                                    const int32_t* cover, int A, const uint32_t* root_state, int R, int D, int T, uint64_t seed,
+                                    float c, float lo, float inv_range, const float* ln_table, int32_t* root_n, float* root_w,
+                                    int32_t* num_nodes, void* workspace, size_t workspace_bytes, nerrf_stream_t stream) {
     size_t need = 0;
     int rc = nerrf_mcts_workspace_bytes(A, T, R, &need);
     if (rc) return rc;
@@ -827,11 +907,13 @@ extern "C" int nerrf_mcts_search(const float* p, const float* size, const float*
         return NERRF_ERR_WORKSPACE;
     }
     cudaStream_t st = (cudaStream_t)stream;
+    rc = check_cover(cover, guard, A, st);
+    if (rc) return rc;
     const MctsLayout L = mcts_layout(A, T, R);
     unsigned char* ws = (unsigned char*)workspace;
     NERRF_CHECK_CUDA(cudaMemsetAsync(ws + L.barrier, 0, 4, st));       // the tree replicas are initialised by the kernel itself
     MctsArgs a;
-    a.p = p; a.size = size; a.cost = cost; a.guard = guard; a.A = A; a.root_state = root_state; a.R = R; a.D = D; a.T = T;
+    a.p = p; a.size = size; a.cost = cost; a.guard = guard; a.cover = cover; a.A = A; a.root_state = root_state; a.R = R; a.D = D; a.T = T;
     a.k0 = (uint32_t)(seed & 0xffffffffu); a.k1 = (uint32_t)(seed >> 32);
     a.c = c; a.lo = lo; a.inv_range = inv_range; a.lnN = ln_table;
     a.root_n = root_n; a.root_w = root_w; a.num_nodes_out = num_nodes;
@@ -844,13 +926,21 @@ extern "C" int nerrf_mcts_search(const float* p, const float* size, const float*
     return launch_mcts<4>(a, L.grid, st);
 }
 
+extern "C" int nerrf_mcts_search(const float* p, const float* size, const float* cost, const int32_t* guard, int A,
+                                 const uint32_t* root_state, int R, int D, int T, uint64_t seed, float c, float lo,
+                                 float inv_range, const float* ln_table, int32_t* root_n, float* root_w, int32_t* num_nodes,
+                                 void* workspace, size_t workspace_bytes, nerrf_stream_t stream) {
+    return nerrf_mcts_search_ex(p, size, cost, guard, nullptr, A, root_state, R, D, T, seed, c, lo, inv_range, ln_table, root_n,
+                                root_w, num_nodes, workspace, workspace_bytes, stream);
+}
+
 // ---- host-buffer session: device memory + a stream live in the handle, so a host-side search is copies + one launch
 struct nerrf_mcts_session {
     unsigned char* d = nullptr;
     size_t bytes = 0;
     int A_max = 0, T_max = 0, R_max = 0;
     cudaStream_t st = nullptr;
-    size_t o_p, o_s, o_c, o_g, o_rs, o_ln, o_rn, o_rw, o_nn, o_ws, ws_bytes;
+    size_t o_p, o_s, o_c, o_g, o_cv, o_rs, o_ln, o_rn, o_rw, o_nn, o_ws, ws_bytes;
 };
 
 extern "C" int nerrf_mcts_session_create(int A_max, int T_max, int R_max, nerrf_mcts_session** out) {
@@ -863,7 +953,7 @@ extern "C" int nerrf_mcts_session_create(int A_max, int T_max, int R_max, nerrf_
     const size_t A_pad = 1024 * (size_t)nw_for(A_max), nwords = 32 * (size_t)nw_for(A_max);
     auto al = [](size_t v) { return (v + 255) & ~(size_t)255; };
     s->o_p = 0; s->o_s = al(s->o_p + A_pad * 4); s->o_c = al(s->o_s + A_pad * 4); s->o_g = al(s->o_c + A_pad * 4);
-    s->o_rs = al(s->o_g + A_pad * 4); s->o_ln = al(s->o_rs + nwords * 4); s->o_rn = al(s->o_ln + (size_t)(T_max + 2) * 4);
+    s->o_cv = al(s->o_g + A_pad * 4); s->o_rs = al(s->o_cv + A_pad * 4); s->o_ln = al(s->o_rs + nwords * 4); s->o_rn = al(s->o_ln + (size_t)(T_max + 2) * 4);
     s->o_rw = al(s->o_rn + A_pad * 4); s->o_nn = al(s->o_rw + A_pad * 4); s->o_ws = al(s->o_nn + 4);
     s->ws_bytes = need; s->bytes = s->o_ws + need;
     cudaError_t e = cudaMalloc((void**)&s->d, s->bytes);
@@ -886,10 +976,11 @@ extern "C" int nerrf_mcts_session_destroy(nerrf_mcts_session* s) {
     return NERRF_OK;
 }
 
-extern "C" int nerrf_mcts_session_search_host(nerrf_mcts_session* s, const float* p, const float* size, const float* cost,
-                                              const int32_t* guard, int A, const uint32_t* root_state_host, int R, int D, int T,
-                                              uint64_t seed, float c, float lo, float inv_range, const float* ln_table_host,
-                                              int32_t* root_n_host, float* root_w_host, int32_t* num_nodes_host) {
+extern "C" int nerrf_mcts_session_search_host_ex(nerrf_mcts_session* s, const float* p, const float* size, const float* cost,
+                                                 const int32_t* guard, const int32_t* cover, int A,
+                                                 const uint32_t* root_state_host, int R, int D, int T, uint64_t seed, float c,
+                                                 float lo, float inv_range, const float* ln_table_host, int32_t* root_n_host,
+                                                 float* root_w_host, int32_t* num_nodes_host) {
     NERRF_REQUIRE(s && p && size && cost && ln_table_host && root_n_host && root_w_host && num_nodes_host, "null pointer");
     NERRF_REQUIRE(A >= 1 && A <= s->A_max && nw_for(A) == nw_for(s->A_max) && T >= 1 && T <= s->T_max && R >= 1 && R <= s->R_max,
                   "search (A=%d, T=%d, R=%d) exceeds the session (A_max=%d with the same word count, T_max=%d, R_max=%d)", A, T, R,
@@ -901,10 +992,11 @@ extern "C" int nerrf_mcts_session_search_host(nerrf_mcts_session* s, const float
     NERRF_CHECK_CUDA(cudaMemcpyAsync(d + s->o_s, size, (size_t)A * 4, cudaMemcpyHostToDevice, st));
     NERRF_CHECK_CUDA(cudaMemcpyAsync(d + s->o_c, cost, (size_t)A * 4, cudaMemcpyHostToDevice, st));
     if (guard) NERRF_CHECK_CUDA(cudaMemcpyAsync(d + s->o_g, guard, (size_t)A * 4, cudaMemcpyHostToDevice, st));
+    if (cover) NERRF_CHECK_CUDA(cudaMemcpyAsync(d + s->o_cv, cover, (size_t)A * 4, cudaMemcpyHostToDevice, st));
     if (root_state_host) NERRF_CHECK_CUDA(cudaMemcpyAsync(d + s->o_rs, root_state_host, nwords * 4, cudaMemcpyHostToDevice, st));
     NERRF_CHECK_CUDA(cudaMemcpyAsync(d + s->o_ln, ln_table_host, (size_t)(T + 2) * 4, cudaMemcpyHostToDevice, st));
-    int rc = nerrf_mcts_search((const float*)(d + s->o_p), (const float*)(d + s->o_s), (const float*)(d + s->o_c),
-                               guard ? (const int32_t*)(d + s->o_g) : nullptr, A,
+    int rc = nerrf_mcts_search_ex((const float*)(d + s->o_p), (const float*)(d + s->o_s), (const float*)(d + s->o_c),
+                               guard ? (const int32_t*)(d + s->o_g) : nullptr, cover ? (const int32_t*)(d + s->o_cv) : nullptr, A,
                                root_state_host ? (const uint32_t*)(d + s->o_rs) : nullptr, R, D, T, seed, c, lo, inv_range,
                                (const float*)(d + s->o_ln), (int32_t*)(d + s->o_rn), (float*)(d + s->o_rw), (int32_t*)(d + s->o_nn),
                                d + s->o_ws, s->ws_bytes, st);
@@ -916,18 +1008,34 @@ extern "C" int nerrf_mcts_session_search_host(nerrf_mcts_session* s, const float
     return launch_status("mcts session search");
 }
 
+extern "C" int nerrf_mcts_session_search_host(nerrf_mcts_session* s, const float* p, const float* size, const float* cost,
+                                              const int32_t* guard, int A, const uint32_t* root_state_host, int R, int D, int T,
+                                              uint64_t seed, float c, float lo, float inv_range, const float* ln_table_host,
+                                              int32_t* root_n_host, float* root_w_host, int32_t* num_nodes_host) {
+    return nerrf_mcts_session_search_host_ex(s, p, size, cost, guard, nullptr, A, root_state_host, R, D, T, seed, c, lo, inv_range,
+                                             ln_table_host, root_n_host, root_w_host, num_nodes_host);
+}
+
 // one-shot convenience: a temporary session (allocates and frees device memory inside the call)
+extern "C" int nerrf_mcts_search_host_ex(const float* p, const float* size, const float* cost, const int32_t* guard,
+                                         const int32_t* cover, int A, const uint32_t* root_state_host, int R, int D, int T,
+                                         uint64_t seed, float c, float lo, float inv_range, const float* ln_table_host,
+                                         int32_t* root_n_host, float* root_w_host, int32_t* num_nodes_host) {
+    nerrf_mcts_session* s = nullptr;
+    int rc = nerrf_mcts_session_create(A, T, R, &s);
+    if (rc) return rc;
+    rc = nerrf_mcts_session_search_host_ex(s, p, size, cost, guard, cover, A, root_state_host, R, D, T, seed, c, lo, inv_range,
+                                           ln_table_host, root_n_host, root_w_host, num_nodes_host);
+    nerrf_mcts_session_destroy(s);
+    return rc;
+}
+
 extern "C" int nerrf_mcts_search_host(const float* p, const float* size, const float* cost, const int32_t* guard, int A,
                                       const uint32_t* root_state_host, int R, int D, int T, uint64_t seed, float c,
                                       float lo, float inv_range, const float* ln_table_host, int32_t* root_n_host,
                                       float* root_w_host, int32_t* num_nodes_host) {
-    nerrf_mcts_session* s = nullptr;
-    int rc = nerrf_mcts_session_create(A, T, R, &s);
-    if (rc) return rc;
-    rc = nerrf_mcts_session_search_host(s, p, size, cost, guard, A, root_state_host, R, D, T, seed, c, lo, inv_range, ln_table_host,
-                                        root_n_host, root_w_host, num_nodes_host);
-    nerrf_mcts_session_destroy(s);
-    return rc;
+    return nerrf_mcts_search_host_ex(p, size, cost, guard, nullptr, A, root_state_host, R, D, T, seed, c, lo, inv_range,
+                                     ln_table_host, root_n_host, root_w_host, num_nodes_host);
 }
 
 extern "C" int nerrf_plan_commit_workspace_bytes(int n_cand_max, size_t* bytes) {
@@ -936,10 +1044,10 @@ extern "C" int nerrf_plan_commit_workspace_bytes(int n_cand_max, size_t* bytes) 
     return NERRF_OK;
 }
 
-extern "C" int nerrf_plan_commit(const float* p, const float* size, const float* cost, const int32_t* guard, int A,
-                                 uint32_t* state, const int32_t* cand, int n_cand, float cur, int max_commits,
-                                 int allow_tentative, int32_t* actions_out, float* scores_out, int32_t* n_out,
-                                 void* workspace, size_t workspace_bytes, nerrf_stream_t stream) {
+extern "C" int nerrf_plan_commit_ex(const float* p, const float* size, const float* cost, const int32_t* guard,
+                                    const int32_t* cover, int A, uint32_t* state, const int32_t* cand, int n_cand, float cur,
+                                    int max_commits, int allow_tentative, int32_t* actions_out, float* scores_out, int32_t* n_out,
+                                    void* workspace, size_t workspace_bytes, nerrf_stream_t stream) {
     NERRF_REQUIRE(p && size && cost && state && actions_out && scores_out && n_out && workspace, "null pointer");
     NERRF_REQUIRE(A >= 1 && A <= 4096, "number of actions must be in 1..4096 (got %d)", A);
     NERRF_REQUIRE(n_cand >= 0 && n_cand <= 4096 && (n_cand == 0 || cand), "n_cand must be in 0..4096");
@@ -948,10 +1056,12 @@ extern "C" int nerrf_plan_commit(const float* p, const float* size, const float*
     nerrf_plan_commit_workspace_bytes(4096, &need);
     NERRF_REQUIRE(workspace_bytes >= need && ((uintptr_t)workspace & 15) == 0, "plan-commit workspace too small or misaligned");
     cudaStream_t st = (cudaStream_t)stream;
+    const int rc0 = check_cover(cover, guard, A, st);
+    if (rc0) return rc0;
     unsigned char* ws = (unsigned char*)workspace;
     NERRF_CHECK_CUDA(cudaMemsetAsync(ws, 0, 256, st));
     CommitArgs a;
-    a.p = p; a.size = size; a.cost = cost; a.guard = guard; a.A = A; a.state = state; a.cand = cand; a.n_cand = n_cand;
+    a.p = p; a.size = size; a.cost = cost; a.guard = guard; a.cover = cover; a.A = A; a.state = state; a.cand = cand; a.n_cand = n_cand;
     a.max_commits = max_commits; a.allow_tentative = allow_tentative; a.cur = cur; a.cap = 4096;
     a.barrier = (unsigned*)ws;
     a.sc_buf = (float*)(ws + 256); a.flag_buf = (int32_t*)(ws + 256 + (size_t)2 * 4096 * 4);
@@ -967,7 +1077,15 @@ extern "C" int nerrf_plan_commit(const float* p, const float* size, const float*
         NERRF_CHECK_CUDA(cudaLaunchCooperativeKernel((void*)kern, dim3(grid), dim3(256), kargs, smem, st));
         return NERRF_OK;
     };
-    if (NW == 1) return go(plan_commit_kernel<1>, terms_smem_bytes<1>() + 4096 * 4);
-    if (NW == 2) return go(plan_commit_kernel<2>, terms_smem_bytes<2>() + 4096 * 4);
-    return go(plan_commit_kernel<4>, terms_smem_bytes<4>() + 4096 * 4);
+    if (NW == 1) return go(plan_commit_kernel<1>, terms_smem_bytes<1>() + 4096 * 4 + (cover ? cover_smem_bytes<1>() : 0));
+    if (NW == 2) return go(plan_commit_kernel<2>, terms_smem_bytes<2>() + 4096 * 4 + (cover ? cover_smem_bytes<2>() : 0));
+    return go(plan_commit_kernel<4>, terms_smem_bytes<4>() + 4096 * 4 + (cover ? cover_smem_bytes<4>() : 0));
+}
+
+extern "C" int nerrf_plan_commit(const float* p, const float* size, const float* cost, const int32_t* guard, int A,
+                                 uint32_t* state, const int32_t* cand, int n_cand, float cur, int max_commits,
+                                 int allow_tentative, int32_t* actions_out, float* scores_out, int32_t* n_out,
+                                 void* workspace, size_t workspace_bytes, nerrf_stream_t stream) {
+    return nerrf_plan_commit_ex(p, size, cost, guard, nullptr, A, state, cand, n_cand, cur, max_commits, allow_tentative,
+                                actions_out, scores_out, n_out, workspace, workspace_bytes, stream);
 }

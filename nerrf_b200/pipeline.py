@@ -18,7 +18,7 @@ import torch
 from . import graph as G
 from .ai.models import GraphSAGE_T, lstm
 from .ai.planner import mcts
-from .ai.planner.rewards import Actions, KIND_KILL as RW_KIND_KILL
+from .ai.planner.rewards import Actions, KIND_KILL as RW_KIND_KILL, KIND_RESTORE as RW_KIND_RESTORE, KIND_COST
 
 _SEQ_EVENT_SLOT = {"file_created": 0, "file_encrypt_start": 1, "file_encrypt_complete": 2, "ransom_note_created": 3,
                    "openat": 4, "write": 5, "rename": 6}
@@ -66,7 +66,7 @@ def file_sequences(events, g: G.TemporalGraph, t_max=lstm.T_MAX, observable=Fals
 @dataclass
 class PipelineResult:
     node_score: torch.Tensor
-    candidates: np.ndarray            # node ids of the A candidate files
+    candidates: np.ndarray            # node id of each action (the A candidate files; kills: pid nodes; restores: -1)
     probs: torch.Tensor               # [A, 2] encrypt_probability, ransomware_score
     plan: mcts.Plan
     plan_nodes: list                  # node ids to revert, in plan order
@@ -74,6 +74,10 @@ class PipelineResult:
     n_kill: int = 0                   # the first n_kill candidates are process nodes ("kill process" actions)
     kill_attribution: str | None = None   # how files were attributed to processes: "writer" (last process in-edge) or
                                           # "edges" (the trained edge head); None when no kill actions were proposed
+    n_restore: int = 0                # "restore from backup" actions proposed (state word 0, after the kills)
+    restores: list = field(default_factory=list)   # per APPLIED restore, in plan order: {"position": index in plan.actions,
+                                                   # "dir": directory, "dir_hash": int, "covers": covered node ids}
+    actions: Actions | None = None    # the action set the plan was made over (cand[i] is the node of action i)
 
 
 @dataclass
@@ -199,9 +203,53 @@ def edge_kill_confidence(g: G.TemporalGraph, candidates: np.ndarray, pids: np.nd
     return out
 
 
+def node_dir_hashes(g: G.TemporalGraph, nodes=None):
+    """int64 parent-directory hash (stream.dir_hash) of the given nodes (all when None): on the device for graphs of a
+    device-resident stream (nerrf_trace_dir_hash), from the name strings for host graphs."""
+    from .stream import dir_hash
+    fn = g.meta.get("dir_hash")
+    if callable(fn):
+        dh = fn()
+        return dh if nodes is None else dh[torch.as_tensor(np.asarray(nodes, np.int64)).to(dh.device)]
+    names = g.meta["names"]
+    idx = range(len(names)) if nodes is None else np.asarray(nodes, np.int64).tolist()
+    return torch.tensor([dir_hash(names[int(i)]) for i in idx], dtype=torch.int64)
+
+
+def propose_restores(cand_dir, file_dir, file_size, file_is_cand, max_restores: int = 4, min_files: int = 8):
+    """"Restore from backup" candidates (threat-model.mdx:216-219, cost 100): the directories holding the most candidate
+    files (at least `min_files`), at most `max_restores`, most candidates first (ties: lower hash).
+    cand_dir int64 [A]: directory hash of each candidate file; file_dir / file_size / file_is_cand [F]: every file node of
+    the window.  A restore's collateral is the summed size of the directory's files that are NOT candidates: it assumes
+    the snapshot clobbers every other file the window saw there (conservative).
+    -> (dir hashes int64 [k], collateral fp32 [k], slot of each candidate int64 [A]: index into the k restores or -1)."""
+    cand_dir = torch.as_tensor(cand_dir).cpu()
+    dirs, counts = torch.unique(cand_dir, return_counts=True)
+    ok = counts >= min_files
+    dirs, counts = dirs[ok].numpy(), counts[ok].numpy()
+    chosen = dirs[np.lexsort((dirs, -counts))[:max_restores]]
+    slot = np.full(cand_dir.shape[0], -1, np.int64)
+    if chosen.size == 0:
+        return chosen, np.zeros(0, np.float32), slot
+    slot_of = {int(d): k for k, d in enumerate(chosen.tolist())}
+    slot = np.array([slot_of.get(int(d), -1) for d in cand_dir.tolist()], np.int64)
+    file_dir = torch.as_tensor(file_dir)
+    ch = torch.from_numpy(chosen).to(file_dir.device)
+    other = ~torch.as_tensor(file_is_cand).to(file_dir.device)
+    size = torch.as_tensor(file_size).to(file_dir.device).to(torch.float64)
+    coll = np.zeros(chosen.shape[0], np.float64)
+    hit = other & torch.isin(file_dir, ch)
+    if bool(hit.any()):
+        d_hit, s_hit = file_dir[hit].cpu().numpy(), size[hit].cpu().numpy()
+        for k, d in enumerate(chosen.tolist()):
+            coll[k] = s_hit[d_hit == d].sum()
+    return chosen, coll.astype(np.float32), slot
+
+
 def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_model, top_a=1024, confidence=None,
         plan_steps=None, n_rollouts=4096, depth=50, iterations=16, device="cuda", exclude=None, commit_per_search=1,
-        dist_ctx: DistContext | None = None, kill_candidates: bool = False) -> PipelineResult:
+        dist_ctx: DistContext | None = None, kill_candidates: bool = False, restore_candidates: bool = False,
+        max_restores: int = 4, min_restore_files: int = 8) -> PipelineResult:
     """seq/lengths/seq_nodes: LSTM inputs for (a superset of) the candidate file nodes (file_sequences()).
     seq may instead be a CALLABLE nodes -> (seq, lengths, nodes_with_sequences): the sequences are then built only for
     the top-A candidates (large windows: a million file nodes, a few thousand candidates); seq_nodes = the file nodes.
@@ -210,7 +258,14 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
     kill_candidates: also propose "kill process" actions (cost 10) for the processes that wrote the candidate files;
     a file reversion only sticks once its writer is gone (planner spec v1, DESIGN.md 1.3).  A model marked
     `edge_head_trained` (ai.train with edge_weight > 0) attributes files to processes by its edge head instead of the
-    last-writer rule, on one GPU; res.kill_attribution records which rule ran."""
+    last-writer rule, on one GPU; res.kill_attribution records which rule ran.
+    restore_candidates: also propose "restore from backup" actions (cost 100) for the (at most `max_restores`) parent
+    directories holding the most candidate files (at least `min_restore_files`); a restore covers every candidate file of
+    its directory and costs the directory's other files as collateral (planner spec v2, DESIGN.md 1.3).  Restores take
+    the state-word-0 slots after the kills (kill budget 32 - restores).  res.plan_nodes lists node actions only;
+    res.restores lists the applied restores."""
+    if restore_candidates and dist_ctx is not None and dist_ctx.world > 1:
+        raise NotImplementedError("restore candidates are planned on one GPU (dist_ctx.world > 1 is not supported)")
     dev = torch.device(device)
     tm = {}
     sync = torch.cuda.synchronize
@@ -257,8 +312,17 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
 
     t0 = time.perf_counter()
     cand = candidates.cpu().numpy()
-    size_mb = np.maximum(g.meta.get("size_mb", np.ones(g.num_nodes, np.float32))[cand], 0.01)
+    size_all_nodes = g.meta.get("size_mb", np.ones(g.num_nodes, np.float32))
+    size_mb = np.maximum(size_all_nodes[cand], 0.01)
     n_kill = 0
+    r_dirs, r_slot = np.zeros(0, np.int64), None
+    if restore_candidates:
+        files = np.nonzero(np.asarray(g.meta["node_kind"]) == 0)[0]
+        file_dir = node_dir_hashes(g, files)
+        is_cand = torch.from_numpy(np.isin(files, cand))
+        r_dirs, r_coll, r_slot = propose_restores(node_dir_hashes(g, cand), file_dir, np.asarray(size_all_nodes, np.float32)[files],
+                                                  is_cand, min(max_restores, 32), min_restore_files)
+    n_restore = int(r_dirs.shape[0])
     if confidence is not None:
         p = np.asarray(confidence, np.float32)[cand]
         actions = Actions(p, size_mb, np.ones(a, np.float32))
@@ -268,9 +332,9 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
             # files are attributed to processes by the trained edge head (P(attack) of each CSR edge)
             _, el = model.heads(h_final, rp, col, return_edge_logits=True)
             edge_attack = torch.softmax(el, 1)[:, 0].cpu().numpy()
-        pids, guard = process_kill_candidates(g, cand, edge_attack=edge_attack)
+        pids, guard = process_kill_candidates(g, cand, max_kills=32 - n_restore, edge_attack=edge_attack)
         n_kill = int(pids.shape[0])
-        a_rev = min(a, 4096 - n_kill)                                  # kill actions occupy the first slots (spec v1: guards < 32)
+        a_rev = min(a, 4096 - n_kill - n_restore)                      # kill actions occupy the first slots (spec v1: guards < 32)
         p_rev = 0.5 * (score[candidates[:a_rev]].cpu().numpy() + probs[:a_rev, 0].cpu().numpy())
         gr = guard[:a_rev]
         if edge_attack is not None:
@@ -288,6 +352,21 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
         cand = np.concatenate([pids, cand[:a_rev]])
     else:
         actions = Actions.from_scores(score[candidates], probs[:, 0], size_mb, np.zeros(a, np.int64))
+    if n_restore:
+        # restore actions take the word-0 slots after the kills: p = 0, size = collateral (u = 0, v = collateral), cost 100;
+        # every candidate file of a restored directory names its restore as its cover.  Kill (guard) slots stay below nk.
+        nk = n_kill
+        a_rev = min(actions.A - nk, 4096 - nk - n_restore)
+        ins = lambda x, mid: np.concatenate([x[:nk], mid, x[nk:nk + a_rev]])
+        kind = actions.kind if actions.kind is not None else np.zeros(actions.A, np.int64)
+        guard = actions.guard if actions.guard is not None else np.full(actions.A, -1, np.int32)
+        cover = np.where(r_slot[:a_rev] >= 0, nk + r_slot[:a_rev], -1)
+        actions = Actions(ins(actions.p, np.zeros(n_restore, np.float32)), ins(actions.size, r_coll),
+                          ins(actions.cost, np.full(n_restore, KIND_COST[RW_KIND_RESTORE], np.float32)),
+                          ins(kind, np.full(n_restore, RW_KIND_RESTORE, np.int64)),
+                          guard=ins(guard, np.full(n_restore, -1, np.int32)),
+                          cover=np.concatenate([np.full(nk + n_restore, -1, np.int64), cover]))
+        cand = ins(cand, np.full(n_restore, -1, np.int64))
     merge = None
     if dist_ctx is not None and dist_ctx.world > 1:
         from . import dist as ND
@@ -296,8 +375,21 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
                    iterations=iterations, device=dev, commit_per_search=commit_per_search, merge=merge)
     sync(); tm["mcts_plan"] = (time.perf_counter() - t0) * 1e3
     tm["total"] = sum(tm.values())
-    res = PipelineResult(score, cand, probs, pl, [int(cand[i]) for i in pl.actions], tm)
+    is_restore = lambda i: n_kill <= i < n_kill + n_restore
+    res = PipelineResult(score, cand, probs, pl, [int(cand[i]) for i in pl.actions if not is_restore(i)], tm)
     res.n_kill = n_kill
+    res.n_restore = n_restore
+    res.actions = actions
+    if n_restore:
+        names = g.meta.get("names")
+        for k, i in enumerate(pl.actions):
+            if is_restore(i):
+                covers = cand[np.nonzero(actions.cover == i)[0]].tolist() if actions.cover is not None else []
+                d = ""
+                if names is not None and covers:
+                    from .stream import parent_dir
+                    d = parent_dir(names.take([covers[0]])[0] if hasattr(names, "take") else names[covers[0]])
+                res.restores.append({"position": k, "dir": d, "dir_hash": int(r_dirs[i - n_kill]), "covers": [int(c) for c in covers]})
     if confidence is None and kill_candidates:
         res.kill_attribution = "writer" if edge_attack is None else "edges"
     return res

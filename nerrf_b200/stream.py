@@ -140,6 +140,23 @@ def name_hash(name) -> int:
     return h - (1 << 64) if h >= (1 << 63) else h
 
 
+def dir_hash(name) -> int:
+    """The 64-bit hash of a node's parent directory (csrc/intern_device.cu nerrf_trace_dir_hash) on the host, as a SIGNED
+    int64: name_hash of the bytes up to (not including) the last '/' -- the empty string when there is none; "pid:<n>"
+    names hash as in name_hash."""
+    if isinstance(name, str) and name.startswith("pid:") and name[4:].isdigit():
+        return name_hash(name)
+    b = name.encode("utf-8") if isinstance(name, str) else bytes(name)
+    k = b.rfind(b"/")
+    return name_hash(b[:k] if k >= 0 else b"")
+
+
+def parent_dir(name) -> str:
+    """The directory dir_hash hashes (the name up to its last '/')."""
+    k = name.rfind("/")
+    return name[:k] if k >= 0 else ""
+
+
 class LazyNames:
     """Node names of a window graph, decoded on demand (a window holds ~10^6 nodes, a plan names a few thousand)."""
 
@@ -558,13 +575,22 @@ class DeviceStream:
                                                         _lib.ptr(self.d_poff), _lib.ptr(self.d_pdata), _lib.ptr(self.d_goff),
                                                         _lib.ptr(self.d_gdata), _lib.ptr(nh), _lib.current_stream_ptr()),
                        "nerrf_trace_name_hash")
+        bufs = (self.name_event, self.name_which, self.d_pid, self.d_poff, self.d_pdata, self.d_goff, self.d_gdata)
+
+        def dir_hash_device(bufs=bufs):
+            """int64 [N] parent-directory hash of every node (nerrf_trace_dir_hash); valid until the stream changes."""
+            dh = torch.empty(N, dtype=torch.int64, device=self.dev)
+            with torch.cuda.device(self.dev):
+                _lib.check(_lib.lib().nerrf_trace_dir_hash(N, *(_lib.ptr(b) for b in bufs), _lib.ptr(dh), _lib.current_stream_ptr()),
+                           "nerrf_trace_dir_hash")
+            return dh
         ne, nwh = self.name_event[:N].cpu().numpy(), self.name_which[:N].cpu().numpy()
         names = LazyNames(self.cols, ne, nwh) if self.cols is not None else \
             DeviceNames(self.d_pid, self.d_poff, self.d_pdata, self.d_goff, self.d_gdata, ne, nwh)
         meta = {"kind": "trace", "names": names,
                 "node_kind": kind_d.cpu().numpy().astype(np.int64), "t0": t0, "span": span, "merge_renames": self.merge,
                 "label": lab.cpu().numpy().astype(np.int64), "size_mb": size_mb.cpu().numpy(), "device": str(self.dev),
-                "name_hash": nh, "events": nw, "window_ranks": (lo, hi), "perm": perm if Gn is None else None}
+                "name_hash": nh, "dir_hash": dir_hash_device, "events": nw, "window_ranks": (lo, hi), "perm": perm if Gn is None else None}
         return G.TemporalGraph(rowptr, col, ew, x, meta)
 
     def sequences_device(self, g: G.TemporalGraph, only_nodes):
@@ -613,6 +639,7 @@ class TickResult:
     planned: list                  # paths this tick's plan reverts (new ones only)
     timings_ms: dict
     truncated: bool = False
+    restored: list = field(default_factory=list)   # directories this tick's plan restores from the snapshot
 
 
 @dataclass
@@ -630,12 +657,16 @@ class StreamingPlanner:
     iterations: int = 8
     commit_per_search: int = 64
     kill_candidates: bool = False  # also propose "kill process" actions (planner spec v1: reversions need their writer gone)
+    restore_candidates: bool = False   # also propose directory restores (planner spec v2, one GPU); covered files count as reverted
+    max_restores: int = 4
+    min_restore_files: int = 8
     device: str = "cuda"
     dist_ctx: object = None        # pipeline.DistContext for the multi-GPU form
     reverted: set = field(default_factory=set)
     _reverted_hash: set = field(default_factory=set)
     ingest_ms: float = 0.0         # one-time: stream columns -> HBM (DeviceStream)
     killed: set = field(default_factory=set)
+    restored_dirs: list = field(default_factory=list)
     ticks: list = field(default_factory=list)
     lateness_s: float = 0.0        # live feed: a tick at t_hi fires once an event with ts > t_hi + lateness_s has arrived
     live: object = None            # live feed: the DeviceStream the bytes go to
@@ -696,6 +727,8 @@ class StreamingPlanner:
         import torch
         ctx = self.dist_ctx
         multi = ctx is not None and ctx.world > 1
+        if multi and self.restore_candidates:
+            raise NotImplementedError("restore candidates are planned on one GPU (dist_ctx.world > 1 is not supported)")
         lead = not multi or ctx.rank == 0
         dev = torch.device(self.device)
         if multi:
@@ -779,7 +812,7 @@ class StreamingPlanner:
                 return sq_t.cpu().numpy(), ln_t.cpu().numpy(), hv_t.cpu().numpy()
             return sq, ln, have
 
-        new, truncated = [], False
+        new, truncated, restored = [], False, []
         for rnd in range(4):
             # a planning pass proposes at most 32 process kills (planner spec v1: guards live in state word 0); a tick
             # with more suspicious processes than that plans again over what is still unreverted
@@ -794,7 +827,8 @@ class StreamingPlanner:
             res = pipeline.run(g, seq, None, nodes, self.model, self.scorer, top_a=self.top_a, n_rollouts=self.n_rollouts,
                                depth=self.depth, iterations=self.iterations, device=self.device, exclude=skip,
                                commit_per_search=self.commit_per_search, dist_ctx=self.dist_ctx,
-                               kill_candidates=self.kill_candidates)
+                               kill_candidates=self.kill_candidates, restore_candidates=self.restore_candidates,
+                               max_restores=self.max_restores, min_restore_files=self.min_restore_files)
             for k, v in res.timings_ms.items():
                 tm[k] = tm.get(k, 0.0) + float(v)
             got = []
@@ -806,10 +840,17 @@ class StreamingPlanner:
                 self.reverted.update(got)
                 self._reverted_hash.update(name_hash(nm) for nm in got)
                 new += got
-            more = bool(self.kill_candidates and res.n_kill >= 32 and got)
+                for r in res.restores:                         # a restored directory brings back every file it covers
+                    cov = [nm for nm in dict.fromkeys(names.take(r["covers"])) if nm not in self.reverted]
+                    self.reverted.update(cov)
+                    self._reverted_hash.update(name_hash(nm) for nm in cov)
+                    restored.append(r["dir"]); self.restored_dirs.append(r["dir"])
+                    got = got + cov
+            # a pass proposes at most 32 - (restores) kills (word 0 holds both): plan again while the budget was used up
+            more = bool(self.kill_candidates and res.n_kill >= 32 - res.n_restore and got)
             if multi:
                 flag = torch.tensor([int(more)], device=dev); dist.broadcast(flag, 0); more = bool(int(flag))
             truncated = truncated or bool(res.plan.truncated)
             if not more:
                 break
-        self.ticks.append(TickResult(t_hi - t0, n_events, g.num_nodes, g.num_edges, new, tm, truncated))
+        self.ticks.append(TickResult(t_hi - t0, n_events, g.num_nodes, g.num_edges, new, tm, truncated, restored))
