@@ -5,10 +5,10 @@
 // computed TRANSPOSED so that the gathered tile is the shared-memory operand and the weights travel in registers:
 //
 //   D^T[H=128 features, rows] = W^T[128, K=2F] . X^T[K, rows]      (one m64n32k16 wgmma half per consumer warpgroup)
-//     A operand = W^T, register fragments split into bf16 terms once per launch and read from L2 by the consumer
-//                 warpgroups: the split W^T of an F=128 layer (192 KB) does not fit in shared memory next to the gather
-//                 rings and operand stages, and Hopper has no tensor memory to hold it.  F = 32: all of the split W^T
-//                 (48 registers per thread at NS = 3) is loaded once per CTA and stays in the consumers' registers
+//     A operand = W^T, register fragments split into bf16 terms once per launch.  F = 32, and F = 128 without hub rows:
+//                 loaded once per CTA by the consumer warpgroups and kept in their registers (KSTEPS x NS x 4 per thread,
+//                 NS = 3: 48 at F = 32, 96 at F = 128, whose layer kernel runs only the mean half, below).  F = 64, and
+//                 F = 128 with hub rows: read from L2 one K step ahead of the MMAs
 //     F = 64 / 128: the self half x_v . W[0:F] needs no gather; a prep kernel (sage_self_prep_kernel) computes it over
 //                 contiguous rows of x with W resident in registers and stores the raw accumulators in out, and the
 //                 layer kernel starts from them and runs only the mean half (K = F), which halves its weight traffic.
@@ -25,17 +25,18 @@
 // Warp roles in one CTA per SM:
 //   warps 0-7   two consumer warpgroups (output features 0-63 and 64-127): wgmma (A in registers, B from shared
 //               memory), then the epilogue from the accumulator registers: + bias, ReLU, row stores, fused node head.
-//               At F = 64 / 128 they take the tiles two at a time, both tiles' MMAs from one load of the A fragments
+//               At F = 64 / 128 they take the tiles two at a time (F = 128 without hub rows: both tiles' MMAs in
+//               one commit group)
 //   warp  8     edge-block loader: stages each tile's rowptr words and its col / ew slices into shared memory --
 //               the slices as two bulk async copies (cp.async.bulk, byte count on the stage's mbarrier) --
 //               running up to IDX_STAGES tiles ahead; the next tile's rowptr words are prefetched before it
 //               waits for a free stage
 //   warps 9-..  gather: one CSR row per warp at a time (four at F=32), rows round-robin; source rows are copied into the
 //               warp's shared-memory ring with cp.async (LDGSTS, 16 B per lane), NQ-1 sub-batches in flight;
-//               indices come from shared memory, so the only global latency a row exposes is its x rows
-//   warp  23    F = 64 / 128: spare, completes the sixth warpgroup, so that setmaxnreg can give the consumer warpgroups
-//               128 registers per thread and the four producer warpgroups (loader, gather, spare) 56.  F = 32: the 15th
-//               gather warp; the consumers get 112 registers per thread, the producers 64
+//               indices come from shared memory, so the only global latency a row exposes is its x rows.
+//               F = 32: warps 9-23 (six warpgroups; consumers 112 registers per thread, producers 64).  F = 128 without
+//               hub rows: warps 9-19 (five warpgroups; consumers 168, producers 48).  Otherwise warps 9-22 and a spare
+//               warp 23 (six warpgroups; consumers 128, producers 56)
 // Pipelines: idx stages full/empty (loader <-> gather), smem operand stages full/empty (gather <-> consumer).
 #include <map>
 #include <mutex>
@@ -58,24 +59,35 @@ constexpr int EPAD = EMAX + 4;         // a slice is copied as its 16-byte align
 constexpr int IDX_STAGE_BYTES = EPAD * 8 + 512;      // col[EPAD] | ew[EPAD] | rp[TN+1] (relative) | e_lo (int64) | col_off, ew_off
 // items (source rows) per sub-batch (= one cp.async group): 4 warp-wide copy instructions, i.e. 4 * (32 / (F/4))
 template <int F> constexpr int qs_for() { return 4 * (32 / (F / 4)); }
-constexpr int NQ = 4;                  // sub-batch slots in a warp's ring; NQ-1 groups are in flight
 
 // NS = number of bf16 terms each fp32 value is split into (v = p0 + p1 [+ p2], p_i = bf16 of the
 // running residual).  NS = 3 with the six products (x0w0, x1w0, x0w1, x1w1, x2w0, x0w2) drops only
 // terms below 2^-24: fp32-equivalent.  NS = 2 with three products is ~1e-5 relative.
-template <int F, int NS>
+// LONG: the launch has hub-row scratch (the kernel's pre-aggregated partial items); it picks the CTA shape at F = 128.
+template <int F, int NS, bool LONG = false>
 struct UmmaCfg {
-    static constexpr int GATHER_WARPS = (F == 32) ? 15 : 14;  // F=32 leaves room for more rings (and needs more TLP)
-    // The CTA is six whole warpgroups (F = 64 / 128: one spare warp after the gather warps), so that setmaxnreg can move
-    // registers from the four producer warpgroups (loader, gather, spare) to the two consumer warpgroups: 768 threads x 80
-    // = 2 x 128 x CONSUMER_REGS + 4 x 128 x PRODUCER_REGS.  F = 64 / 128: the consumers hold two tiles' accumulators;
-    // F = 32: all of the split W^T (KSTEPS x NS x 4 = 48 registers at NS = 3)
-    static constexpr int WARPS = 24;
+    // RESIDENT: the consumers keep all of the split W^T of the K steps they run in registers (KSTEPS x NS x 4: 48 at F = 32
+    // (K = 2F), 96 at F = 128, NS = 3).  At F = 128 that takes a CTA of five warpgroups with 11 gather warps, which
+    // measured faster without hub rows but slower on the hub-destination graph, whose gather (hub-row partial items) sets
+    // the pace with fewer warps, and slower at F = 64, where there is less weight traffic to save: there the layer keeps
+    // 14 gather warps and reads the fragments from L2 one K step ahead of the MMAs (DESIGN 2.1, 5).
+    static constexpr bool RESIDENT = F == 32 || (F == 128 && !LONG);
+    // F = 32: 15 gather warps (the quad gather needs the TLP).  F = 64 / 128 resident: 11 gather warps with deeper rings
+    // (NQ = 5: 4 sub-batches in flight per warp, ~the bytes in flight of 14 warps x 3); otherwise 14 and NQ = 4
+    static constexpr int GATHER_WARPS = (F == 32) ? 15 : RESIDENT ? 11 : 14;
+    static constexpr int NQ = (F != 32 && RESIDENT) ? 5 : 4; // sub-batch slots in a warp's ring; NQ-1 groups are in flight
+    // The CTA is whole warpgroups (14 gather warps: one spare warp after them), so that setmaxnreg can
+    // move registers from the producer warpgroups (loader, gather) to the two consumer warpgroups: THREADS x LAUNCH_REGS
+    // >= 2 x 128 x CONSUMER_REGS + (WARPS / 4 - 2) x 128 x PRODUCER_REGS.  768 x 80 = 2 x 128 x 112 + 4 x 128 x 64 (F = 32),
+    // 640 x 96 = 2 x 128 x 168 + 3 x 128 x 48 (F = 128 resident: W^T and two tiles' accumulators),
+    // 768 x 80 = 2 x 128 x 128 + 4 x 128 x 56 (F = 64, F = 128 with hub rows: two tiles' accumulators, two fragment sets)
+    static constexpr int WARPS = (GATHER_WARP0 + GATHER_WARPS + 3) / 4 * 4;
     static constexpr int THREADS = WARPS * 32;
-    static constexpr int CONSUMER_REGS = (F == 32) ? 112 : 128, PRODUCER_REGS = (F == 32) ? 64 : 56;
-    static_assert(WARPS % 4 == 0 && WARPS >= GATHER_WARP0 + GATHER_WARPS &&
-                  (EPI_WARPS * CONSUMER_REGS + (WARPS - EPI_WARPS) * PRODUCER_REGS) * 32 <= THREADS * 80,
-                  "register budget: 80 registers per thread at launch");
+    static constexpr int LAUNCH_REGS = (65536 / THREADS) & ~7;   // one CTA per SM, allocated in 8-register steps
+    static constexpr int CONSUMER_REGS = (F == 32) ? 112 : RESIDENT ? 168 : 128;
+    static constexpr int PRODUCER_REGS = (F == 32) ? 64 : RESIDENT ? 48 : 56;
+    static_assert((EPI_WARPS * CONSUMER_REGS + (WARPS - EPI_WARPS) * PRODUCER_REGS) * 32 <= THREADS * LAUNCH_REGS,
+                  "register budget at launch");
     // F = 32 (quad-mode gather): a warp runs up to 3 units = ~7 tiles ahead of what it has consumed and holds a tile's edge
     // block from issue to completion, so the look-ahead is bounded by the number of edge-block stages, not by the rings
     // (with 4 stages most issue-side polls find the next tile not yet staged)
@@ -90,7 +102,7 @@ struct UmmaCfg {
     static constexpr int PART_BYTES = KB * TN * 128;         // one bf16 term of one stage
     static constexpr int STAGE_BYTES = NS * PART_BYTES;
     static constexpr int QS = qs_for<F>();                    // 4 (F=128), 8 (F=64), 16 (F=32): always 2 KB per sub-batch
-    static constexpr int RING_BYTES = NQ * QS * F * 4;       // per gather warp: NQ sub-batches x QS source rows
+    static constexpr int RING_BYTES = NQ * QS * F * 4;       // per gather warp: NQ sub-batches x QS source rows (8 / 10 KB)
     static constexpr int STAGES = 4;
     static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + IDX_STAGES * IDX_STAGE_BYTES +
                                    (size_t)GATHER_WARPS * RING_BYTES + 2048 /*head reduce*/ + 1024 /*align*/ + 1024 /*barriers*/;
@@ -258,20 +270,20 @@ __global__ void __launch_bounds__(256) long_chunk_kernel(const float* __restrict
 // LONG: compiled with the hub-row (pre-aggregated partial items) paths; the plain variant is used when the
 // launch has no hub-row scratch, so graphs without hub rows pay nothing for the feature.
 template <int F, int NS, typename RP, bool LONG>
-__global__ void __launch_bounds__((UmmaCfg<F, NS>::THREADS), 1)
+__global__ void __launch_bounds__((UmmaCfg<F, NS, LONG>::THREADS), 1)
 sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowptr, const int32_t* __restrict__ col,
                        const float* __restrict__ ew, const float* __restrict__ W, const float* __restrict__ bias,
                        float* __restrict__ out, int64_t row_begin, int64_t row_end, int relu,
                        const float* __restrict__ node_w, float node_b, float* __restrict__ score, const LongWs lw,
                        const Peers peers, unsigned* __restrict__ tile_ctr, const uint4* __restrict__ wsplit,
                        int l2_policy) {
-    using C = UmmaCfg<F, NS>;
+    using C = UmmaCfg<F, NS, LONG>;
     constexpr int LPR = F / 4;
     // L2 policy, F = 64 / 128 (l2_policy == 0: every access at normal priority): the gathered source rows, S, the output rows
     // and the col / ew slices are evict-first; the F = 32 layer (QUAD below) gives no hints (measured, DESIGN 2.1).
     // Created where it is used, so that it holds no register across the roles.
     auto pol = [l2_policy]() { return l2_policy ? l2_policy_evict_first() : l2_policy_evict_normal(); };
-    constexpr int GATHER_WARPS = C::GATHER_WARPS, IDX_STAGES = C::IDX_STAGES;
+    constexpr int GATHER_WARPS = C::GATHER_WARPS, IDX_STAGES = C::IDX_STAGES, NQ = C::NQ;
     extern __shared__ unsigned char smem_dyn[];
     const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;          // SWIZZLE_128B needs 1024-B alignment
     unsigned char* smem_gen = smem_dyn + (smem_base - smem_u32(smem_dyn));
@@ -326,7 +338,6 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
         constexpr int UPT = TN / 4;                                       // units (4 rows) per tile
         constexpr int SLOT_BYTES = 4 * 4 * F * 4;                         // a sub-batch = 4 steps x 4 rows x 128 B = 2 KB
         static_assert(SLOT_BYTES * NQ == C::RING_BYTES, "ring layout");
-        static_assert(C::WARPS == GATHER_WARP0 + GATHER_WARPS, "every warp after the loader gathers");
         setmaxnreg_dec<C::PRODUCER_REGS>();
         const int g = warp - GATHER_WARP0;
         const int grp = lane >> 3, sub = lane & 7;
@@ -556,7 +567,8 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
         // bounded by the ring, not by registers, and no load ever stalls a scoreboard.
         static_assert(C::SELF_SPLIT, "the row-per-warp gather writes only the mean columns");
         setmaxnreg_dec<C::PRODUCER_REGS>();
-        if (warp >= GATHER_WARP0 + GATHER_WARPS) return;                 // the spare warp: no ring, nothing to do
+        if constexpr (C::WARPS > GATHER_WARP0 + GATHER_WARPS)           // 14 gather warps: the spare warp has no ring
+            if (warp >= GATHER_WARP0 + GATHER_WARPS) return;
         constexpr int G = 32 / LPR;                                     // items consumed by one warp-wide LDS.128
         constexpr int QS = C::QS;
         constexpr int SLOT_FLOATS = QS * F;
@@ -964,30 +976,25 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                 }
             }
         } else {
-            // F = 64 / 128: the fragments are re-read from L2 for every pass (the split W^T of an F = 128 layer would take 96
-            // registers per thread).  They are the same for every tile, so their loads run AHEAD K steps ahead of the MMAs
-            // across tile boundaries: an L2 round trip under the gather's load is longer than one K step of one tile.  With
-            // tile pairs (below) a K step issues twice the MMAs, so one step ahead covers as long as two did for a single
-            // tile, and the 12 registers of a second fragment set (NS = 3) go to the second tile's accumulators.
-            constexpr int TP = C::SELF_SPLIT ? 2 : 1;                             // tiles per pass
-            constexpr int AHEAD = 3 - TP;                                         // K steps the fragment loads run ahead
-            auto copy_a = [](uint32_t (&dst)[NS][4], const uint32_t (&src)[NS][4]) {
+            // F = 128 without hub rows (RESIDENT): the split W^T of the mean half (K = F: KSTEPS x NS fragments, 96 registers
+            // at NS = 3) is loaded once and stays in registers, as at F = 32: no fragment register is
+            // redefined while a wgmma runs, so a pass is all its products in ONE commit group with one wait.
+            // F = 64, and F = 128 with hub rows: the fragments are re-read from L2 for every pass, one K step ahead of the MMAs across tile
+            // boundaries (an L2 round trip under the gather's load is longer than one K step of one tile, and a K step issues
+            // both tiles' MMAs); a step's MMAs are waited for before the next fragments are written, because ptxas serializes
+            // the MMAs when a wgmma input register is redefined while one is in flight.
+            constexpr int TP = 2;                                                 // tiles per pass
+            uint32_t a[C::RESIDENT ? C::KSTEPS : 1][NS][4];                       // (with hub rows: the next K step's)
 #pragma unroll
-                for (int p = 0; p < NS; ++p)
-#pragma unroll
-                    for (int r = 0; r < 4; ++r) dst[p][r] = src[p][r];
-            };
-            uint32_t a_n[AHEAD][NS][4];                                           // fragments of the next AHEAD K steps
-#pragma unroll
-            for (int i = 0; i < AHEAD; ++i) load_a(i, a_n[i]);
+            for (int j = 0; j < (C::RESIDENT ? C::KSTEPS : 1); ++j) load_a(j, a[j]);
             // The accumulators start from the prep kernel's self terms (the first F/16 K steps), stored raw in out -- the
             // local buffer: peers and the multicast address never hold this rank's self terms.
             // TILE PAIRS: a warpgroup takes the CTA's tiles two at a time (operand stages tl and tl + 1) and issues each K
-            // step's products for both tiles from ONE fragment load into two independent accumulator sets: half the fragment
-            // traffic and half the K-step waits per row, and two MMA chains the tensor pipe can overlap.  Each tile runs the
-            // same wgmma sequence as it would alone, so its outputs do not depend on its partner.  A closing entry (-1) in the
-            // second slot ends the stream: that pass stores only the first tile (the products over the closing stage are
-            // discarded).
+            // step's products for both tiles into two independent accumulator sets: two MMA chains the tensor pipe can
+            // overlap, and one wait per 64 rows.  Each tile runs the same wgmma sequence as it would alone (same fragments,
+            // same product order, scale-d 1 from its self terms), so its outputs do not depend on its partner.  A closing
+            // entry (-1) in the second slot ends the stream: that pass stores only the first tile (the products over the
+            // closing stage are discarded).
             // The epilogue of a pass already loads the next pass's self terms into d when the loader has published those
             // tiles' ids: the ids of a CTA's tiles increase, so a ring entry greater than the pass's last tile is a later
             // tile's, not a stale one.
@@ -1001,7 +1008,7 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                 int tile[TP];
                 tile[0] = wait_full(tl);
                 if (tile[0] < 0) break;                                           // closing entry: end of stream
-                if constexpr (TP == 2) tile[1] = wait_full(tl + 1);               // (-1: the closing entry)
+                tile[1] = wait_full(tl + 1);                                      // (-1: the closing entry)
                 if constexpr (C::SELF_SPLIT) {
 #pragma unroll
                     for (int u = 0; u < TP; ++u) {
@@ -1016,30 +1023,37 @@ sage_layer_umma_kernel(const float* __restrict__ x, const RP* __restrict__ rowpt
                         }
                     }
                 }
-                auto mma_step = [&](int j, const uint32_t (&a)[NS][4]) {
+                auto pair_products = [&](int j, const uint32_t (&aj)[NS][4]) {      // K step j of both tiles
                     const uint32_t boff = (uint32_t)((j >> 2) * (TN * 128) + (j & 3) * 32);
-                    wgmma_fence();
 #pragma unroll
                     for (int u = 0; u < TP; ++u) {
                         const uint32_t st0 = smem_base + (uint32_t)((s0 + u) * C::STAGE_BYTES);
                         uint64_t xb[NS];
 #pragma unroll
                         for (int p = 0; p < NS; ++p) xb[p] = make_b_desc(st0 + (uint32_t)(p * C::PART_BYTES) + boff);   // x term p
-                        wgmma_split_products<NS>(d[u], a, xb, 1u);                  // (the self terms start d)
+                        wgmma_split_products<NS>(d[u], aj, xb, 1u);                 // (the self terms start d)
                     }
-                    wgmma_commit();
                 };
-                // (registers a running wgmma reads must not be written before it retires, and ptxas serializes the MMAs of a
-                // step when any wgmma input is written while one is in flight: the next fragments are loaded before the step)
-    #pragma unroll 1
-                for (int j = 0; j < C::KSTEPS; ++j) {
-                    uint32_t a_cur[NS][4];
-                    copy_a(a_cur, a_n[0]);
+                if constexpr (C::RESIDENT) {
+                    wgmma_fence();
 #pragma unroll
-                    for (int i = 0; i + 1 < AHEAD; ++i) copy_a(a_n[i], a_n[i + 1]);
-                    load_a(j + AHEAD < C::KSTEPS ? j + AHEAD : j + AHEAD - C::KSTEPS, a_n[AHEAD - 1]);   // K >= 64: >= 4 K steps
-                    mma_step(j, a_cur);
+                    for (int j = 0; j < C::KSTEPS; ++j) pair_products(j, a[j]);
+                    wgmma_commit();
                     wgmma_wait_all();
+                } else {
+    #pragma unroll 1
+                    for (int j = 0; j < C::KSTEPS; ++j) {
+                        uint32_t a_cur[NS][4];
+#pragma unroll
+                        for (int p = 0; p < NS; ++p)
+#pragma unroll
+                            for (int r = 0; r < 4; ++r) a_cur[p][r] = a[0][p][r];
+                        load_a(j + 1 < C::KSTEPS ? j + 1 : j + 1 - C::KSTEPS, a[0]);
+                        wgmma_fence();
+                        pair_products(j, a_cur);
+                        wgmma_commit();
+                        wgmma_wait_all();
+                    }
                 }
                 __syncwarp();
                 if (lane == 0) {
@@ -1297,9 +1311,10 @@ template <int F, int NS, typename RP>
 int launch_umma(const float* x, const RP* rowptr, const int32_t* col, const float* ew, const float* W, const float* b,
                 float* out, int64_t row_begin, int64_t row_end, int relu, const float* node_w, float node_b, float* score,
                 void* long_ws, size_t long_ws_bytes, bool reuse_scan, const Peers& peers, int l2_policy, cudaStream_t st) {
-    using C = UmmaCfg<F, NS>;
+    using C = UmmaCfg<F, NS, false>;
+    using CL = UmmaCfg<F, NS, true>;                                     // with hub-row scratch
     int rc = set_max_dynamic_smem((const void*)sage_layer_umma_kernel<F, NS, RP, false>, C::SMEM);
-    if (!rc) rc = set_max_dynamic_smem((const void*)sage_layer_umma_kernel<F, NS, RP, true>, C::SMEM);
+    if (!rc) rc = set_max_dynamic_smem((const void*)sage_layer_umma_kernel<F, NS, RP, true>, CL::SMEM);
     if (rc) return rc;
     const int64_t rows = row_end - row_begin;
     const int64_t tiles = (rows + TN - 1) / TN;
@@ -1338,7 +1353,7 @@ int launch_umma(const float* x, const RP* rowptr, const int32_t* col, const floa
     }
     // the col / ew slices are staged with bulk copies, which only need 4-byte aligned slices (the aligned superset is copied)
     if (lw.cap > 0)
-        sage_layer_umma_kernel<F, NS, RP, true><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit, l2_policy);
+        sage_layer_umma_kernel<F, NS, RP, true><<<(unsigned)grid, CL::THREADS, CL::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit, l2_policy);
     else
         sage_layer_umma_kernel<F, NS, RP, false><<<(unsigned)grid, C::THREADS, C::SMEM, st>>>(x, rowptr, col, ew, W, b, out, row_begin, row_end, relu, node_w, node_b, score, lw, peers, tile_ctr, wsplit, l2_policy);
     return launch_status("sage_layer_umma_kernel");
