@@ -339,6 +339,18 @@ int nerrf_trace_sequences(const int64_t* cand_nodes, int n_cand, const void* row
                           const uint8_t* path_flags, double t0, double span, int t_max, float* seq_out,
                           int32_t* len_out, void* stream);
 
+/* Per-pair edge labels of a trace graph on the device (the training target of the edge head; spec = nerrf_b200/graph.py
+ * graph_from_events meta['edge_label']).  node_p / node_f [n_events] = the graph's events mapped to node ids (as handed
+ * to nerrf_graph_node_features), raw_slot [n_events] = their ANNOTATION event slots (not the observable fold);
+ * rowptr / col = the graph's CSR by destination (n_edges = rowptr[n_nodes]).  label_out uint8 [n_edges], CSR order: 1 iff
+ * one end of the edge is a process p, the other a file f, and p has an event of raw slot 1..3 (encrypt start, encrypt
+ * complete, ransom note) on f; 0 elsewhere, file <-> file rename links included.  Event ids outside [0, n_nodes) match
+ * nothing.  Sort + binary search: deterministic, no atomics, does not wait for `stream`.  All pointers device. */
+int nerrf_trace_edge_labels_workspace_bytes(int64_t n_events, int64_t* bytes);
+int nerrf_trace_edge_labels(const int32_t* node_p, const int32_t* node_f, const uint8_t* raw_slot, int64_t n_events,
+                            const void* rowptr, int rowptr_is64, const int32_t* col, int64_t n_edges, int64_t n_nodes,
+                            uint8_t* label_out, void* workspace, int64_t workspace_bytes, nerrf_stream_t stream);
+
 /* Per-node features on the device (rest of SURVEY.md 8f rank 1): event columns already mapped to node
  * ids (nerrf_trace_intern, events in time order) -> x [n_nodes, 32] in the layout GraphSAGE_T.forward
  * reads (node schema docs/content/docs/architecture.mdx:144-160, threat-model.mdx:154-184; column

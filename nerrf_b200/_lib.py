@@ -85,6 +85,8 @@ SIGNATURES = {
     "nerrf_trace_sequences": (C.c_int, [vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, C.c_double, C.c_double, C.c_int, vp, vp, vp]),
     "nerrf_graph_build_csr": (C.c_int, [vp, vp, vp, vp, C.c_int64, C.c_int64, C.c_float, C.c_float, vp, C.c_int,
                                         vp, vp, vp, C.c_int64, vp]),
+    "nerrf_trace_edge_labels_workspace_bytes": (C.c_int, [C.c_int64, C.POINTER(C.c_int64)]),
+    "nerrf_trace_edge_labels": (C.c_int, [vp, vp, vp, C.c_int64, vp, C.c_int, vp, C.c_int64, C.c_int64, vp, vp, C.c_int64, vp]),
     "nerrf_graph_node_features_workspace_bytes": (C.c_int, [C.c_int64, C.POINTER(C.c_int64)]),
     "nerrf_graph_node_features": (C.c_int, [vp, vp, vp, vp, vp, vp, vp, C.c_int64, vp, C.c_int64, C.c_double, vp, vp, vp,
                                             vp, C.c_int64, vp]),

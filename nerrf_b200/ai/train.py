@@ -16,6 +16,11 @@ node_b; LSTMScorer.lstm / head).  Inference never calls anything in this file, a
 GraphSAGE_T.forward / LSTMScorer.forward still refuse CPU tensors.
 
     python -m nerrf_b200.ai.train --traces 8 --epochs 200 --out weights.pt
+    python -m nerrf_b200.ai.train --device cuda --fleet 400,8 --bystanders 2 --windows 16 --edge-loss 1.0 --out w.pt
+    python -m nerrf_b200.ai.train --device cuda --stream trace.pb --windows 16 --edge-loss 1.0 --out w.pt
+
+The last two train on sliding windows of a trace stream built on the GPU (stream_examples): graph, node and edge labels
+and sequences come from the device constructor, so a window can have the size of a fleet window (~10^6 nodes).
 """
 from __future__ import annotations
 
@@ -172,6 +177,52 @@ def toy_set(seeds, windows: int = 2, **kw):
     return out
 
 
+# ------------------------------------------------------------------ stream windows (built on the device)
+def stream_examples(source, n_windows: int, window_s: float = 60.0, seed: int = 0, files_per_window: int = 512,
+                    device="cuda") -> list:
+    """`n_windows` labelled examples from random sliding windows of an annotated trace stream, each built on the device:
+    the window graph with its node and per-pair edge labels (stream.DeviceStream.window_graph(..., edge_labels=True)),
+    and the LSTM sequences (DeviceStream.sequences_device) of a class-balanced sample of at most `files_per_window` file
+    nodes -- half encrypted files as far as the window has them, the rest benign.  source: ingest.EventColumns (made
+    device resident here, observable-only features like make_example) or a merge-mode stream.DeviceStream.
+    Same dict schema as make_example, tensors on the device, so train() / evaluate() take these unchanged; except:
+      "events": None (no host event list exists; nothing in train / evaluate reads it),
+      "seq" / "lengths" / "seq_label" / "seq_nodes" cover the sampled files only, not every file of the window,
+    plus "window": (t_lo, t_hi), the window's bounds in the stream's clock.  Windows with no file node are redrawn."""
+    import torch
+    from .. import stream
+    ds = source if isinstance(source, stream.DeviceStream) else stream.DeviceStream(source, device, observable=True)
+    if not ds.merge:
+        raise ValueError("stream_examples needs a merge-mode DeviceStream (sequences_device)")
+    t_first, t_last = ds.span()
+    rng = np.random.default_rng(seed)
+    out, draws = [], 0
+    while len(out) < n_windows:
+        draws += 1
+        if draws > 20 * n_windows + 20:
+            raise ValueError(f"stream_examples: only {len(out)} of {n_windows} windows hold a file node")
+        hi = float(rng.uniform(min(t_first + 0.25 * window_s, t_last), t_last))      # windows end a quarter window in, or later
+        g = ds.window_graph(hi - window_s, hi, window_s, edge_labels=True)
+        if g is None:
+            continue
+        lab = g.meta["label"]
+        files = np.nonzero(g.meta["node_kind"] == 0)[0]
+        if files.size == 0:
+            continue
+        pos, neg = files[lab[files] > 0], files[lab[files] == 0]
+        k_pos = min(pos.size, files_per_window // 2)
+        k_neg = min(neg.size, files_per_window - k_pos)
+        nodes = np.sort(np.concatenate([rng.choice(pos, k_pos, replace=False), rng.choice(neg, k_neg, replace=False)]))
+        seq, lengths = ds.sequences_device(g, nodes)
+        dev = g.x.device
+        label = torch.from_numpy(lab.astype(np.float32)).to(dev)
+        out.append({"x": g.x, "rowptr": g.rowptr, "col": g.col, "ew": g.ew, "label": label,
+                    "is_file": torch.from_numpy(g.meta["node_kind"] == 0).to(dev), "seq": seq, "lengths": lengths,
+                    "seq_label": label[torch.from_numpy(nodes).to(dev)], "edge_label": g.meta["edge_label"], "graph": g,
+                    "events": None, "seq_nodes": nodes, "window": (hi - window_s, hi)})
+    return out
+
+
 def _to(ex, device):
     return {k: (v.to(device) if torch.is_tensor(v) else v) for k, v in ex.items()}
 
@@ -267,8 +318,19 @@ def evaluate(model: GraphSAGE_T, scorer: LSTMScorer | None, examples, device="cp
     return out
 
 
-def main(argv=None):
-    ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
+def _fleet_arg(s: str):
+    try:
+        procs, attacked = (int(v) for v in s.split(","))
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"--fleet takes PROCS,ATTACKED (two integers), got {s!r}")
+    if not 0 <= attacked <= procs or procs < 1:
+        raise argparse.ArgumentTypeError(f"--fleet needs 0 <= ATTACKED <= PROCS and PROCS >= 1, got {s!r}")
+    return procs, attacked
+
+
+def parser() -> argparse.ArgumentParser:
+    """The command line of `python -m nerrf_b200.ai.train`."""
+    ap = argparse.ArgumentParser(prog="python -m nerrf_b200.ai.train", description=__doc__.split("\n")[0])
     ap.add_argument("--traces", type=int, default=8); ap.add_argument("--epochs", type=int, default=150)
     ap.add_argument("--layers", type=int, default=2); ap.add_argument("--lr", type=float, default=3e-3)
     ap.add_argument("--device", default="cpu"); ap.add_argument("--out", default=None)
@@ -278,10 +340,46 @@ def main(argv=None):
     ap.add_argument("--edge-loss", type=float, default=0.0, metavar="W",
                     help="also train the attack/normal edge head with this loss weight (toy traces get 2 bystander "
                          "processes, so the edge labels differ from the file labels)")
+    src = ap.add_mutually_exclusive_group()
+    src.add_argument("--fleet", type=_fleet_arg, default=None, metavar="PROCS,ATTACKED",
+                     help="train on device-built windows of a simulated fleet trace (stream.fleet_columns, seed --seed) and "
+                          "report on windows of a held-out fleet (seed --seed + 1); needs a CUDA device")
+    src.add_argument("--stream", default=None, metavar="TRACE_PB",
+                     help="train on device-built windows of an annotated EventBatch trace (wire bytes) and report on another "
+                          "draw of its windows; needs a CUDA device")
+    ap.add_argument("--bystanders", type=int, default=0, metavar="K",
+                    help="--fleet: K benign processes per attacked process touching its files after it")
+    ap.add_argument("--windows", type=int, default=16, help="--fleet / --stream: training windows")
+    ap.add_argument("--window-s", type=float, default=60.0, help="--fleet / --stream: window length in seconds")
+    ap.add_argument("--files-per-window", type=int, default=512,
+                    help="--fleet / --stream: class-balanced file nodes per window whose sequences train the BiLSTM")
+    ap.add_argument("--seed", type=int, default=0, help="--fleet / --stream: fleet seed and window draw")
+    return ap
+
+
+def main(argv=None):
+    ap = parser()
     a = ap.parse_args(argv)
     edges = a.edge_loss > 0
-    kw = {"bystanders": 2} if edges else {}
-    train_set = toy_set(range(100, 100 + a.traces), **kw); test_set = toy_set(range(900, 903), **kw)
+    if a.fleet is not None or a.stream is not None:
+        if not a.device.startswith("cuda"):
+            ap.error("--fleet / --stream build their windows on the GPU: pass --device cuda")
+        from .. import ingest, stream
+        skw = dict(window_s=a.window_s, files_per_window=a.files_per_window, device=a.device)
+        n_test = max(a.windows // 4, 2)
+        if a.fleet is not None:
+            procs, attacked = a.fleet
+            fleet = lambda s: stream.fleet_columns(procs, attacked, seed=s, bystanders=a.bystanders)[0]
+            train_set = stream_examples(fleet(a.seed), a.windows, seed=a.seed, **skw)
+            test_set = stream_examples(fleet(a.seed + 1), n_test, seed=a.seed + 1, **skw)
+        else:
+            with open(a.stream, "rb") as f:
+                ds = stream.DeviceStream(ingest.decode_event_batch(f.read()), a.device, observable=True)
+            train_set = stream_examples(ds, a.windows, seed=a.seed, **skw)
+            test_set = stream_examples(ds, n_test, seed=a.seed + 1, **skw)
+    else:
+        kw = {"bystanders": 2} if edges else {}
+        train_set = toy_set(range(100, 100 + a.traces), **kw); test_set = toy_set(range(900, 903), **kw)
     model = GraphSAGE_T(G.F_IN, 128, a.layers); scorer = None if a.no_lstm else LSTMScorer()
     print("before:", evaluate(model, scorer, test_set, a.device, edges=edges))
     train(model, scorer, train_set, a.epochs, a.lr, a.device, log=print, lstm_backward=a.lstm_backward,

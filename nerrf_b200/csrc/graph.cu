@@ -231,6 +231,62 @@ __global__ void __launch_bounds__(256) trace_sequences_kernel(const int64_t* __r
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Per-pair edge labels (spec = nerrf_b200/graph.py graph_from_events meta['edge_label']): an edge of the CSR is 1 iff one
+// end is a process p, the other a file f, and p emitted an attack event (raw annotation slot 1..3: encrypt start / complete,
+// ransom note) on f.  Keys p * N + f of the attack events are radix-sorted (radix_sort.cuh); every other event gets the
+// sentinel N * N, which sorts last and equals no pair.  Then one thread per CSR edge finds its row by a binary search of
+// rowptr and looks both orientations of (src, dst) up in the sorted keys: the attack pair is stored process-first, so at
+// most one orientation can hit, and a file <-> file rename link never does.  Duplicate keys are harmless to the search, so
+// no unique pass is needed.  No atomics, no host round trip.
+__global__ void __launch_bounds__(256) attack_keys_kernel(const int32_t* __restrict__ node_p, const int32_t* __restrict__ node_f,
+                                                          const uint8_t* __restrict__ raw_slot, int64_t n, int64_t N,
+                                                          uint64_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    const uint64_t none = (uint64_t)N * (uint64_t)N;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
+        const int32_t p = node_p[i], f = node_f[i];
+        const int s = raw_slot[i];
+        const bool attack = s >= 1 && s <= 3 && (uint32_t)p < (uint64_t)N && (uint32_t)f < (uint64_t)N;   // ids outside [0, N) match nothing
+        keys[i] = attack ? (uint64_t)p * (uint64_t)N + (uint64_t)f : none;
+        vals[i] = (uint32_t)i;
+    }
+}
+
+__device__ __forceinline__ bool sorted_contains(const uint64_t* __restrict__ keys, int64_t n, uint64_t k) {
+    int64_t lo = 0, hi = n;                                          // lower bound
+    while (lo < hi) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (__ldg(keys + mid) < k) lo = mid + 1; else hi = mid;
+    }
+    return lo < n && __ldg(keys + lo) == k;
+}
+
+template <typename RP>
+__global__ void __launch_bounds__(256) edge_label_kernel(const RP* __restrict__ rowptr, const int32_t* __restrict__ col, int64_t E,
+                                                         int64_t N, const uint64_t* __restrict__ keys, int64_t n,
+                                                         uint8_t* __restrict__ label) {
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < E; i += stride) {
+        int64_t lo = 0, hi = N;                                      // row d = the last row with rowptr[d] <= i
+        while (hi - lo > 1) {
+            const int64_t mid = (lo + hi) >> 1;
+            if ((int64_t)__ldg(rowptr + mid) <= i) lo = mid; else hi = mid;
+        }
+        const uint64_t d = (uint64_t)lo, s = (uint32_t)col[i];
+        bool hit = false;
+        if (s < (uint64_t)N) hit = sorted_contains(keys, n, s * N + d) || sorted_contains(keys, n, d * N + s);
+        label[i] = hit ? 1 : 0;
+    }
+}
+
+static int pair_key_bits(int64_t N) {                                // bits of N * N, the largest key (the sentinel)
+    const uint64_t top = (uint64_t)N * (uint64_t)N;
+    int b = 1;
+    while (b < 64 && (top >> b)) ++b;
+    return b;
+}
+
 struct CsrWs {
     size_t keys_a, keys_b, vals_a, vals_b, bad, temp, total, temp_bytes;
 };
@@ -397,6 +453,60 @@ extern "C" int nerrf_graph_node_features(const int32_t* node_p, const int32_t* n
     NERRF_CHECK_CUDA(cudaStreamSynchronize(st));
     NERRF_REQUIRE(h_bad == 0, "event columns hold a node id outside [0, n_nodes), a negative time or an event slot > 7");
     return NERRF_OK;
+}
+
+static size_t edge_label_layout(int64_t n, size_t* keys_b, size_t* vals_a, size_t* vals_b, size_t* scratch) {
+    size_t o = up256((size_t)n * 8);
+    *keys_b = o;  o += up256((size_t)n * 8);
+    *vals_a = o;  o += up256((size_t)n * 4);
+    *vals_b = o;  o += up256((size_t)n * 4);
+    *scratch = o; o += up256(rs_scratch_bytes(n > 0 ? n : 1));
+    return o;
+}
+
+extern "C" int nerrf_trace_edge_labels_workspace_bytes(int64_t n_events, int64_t* bytes) {
+    NERRF_REQUIRE(bytes != nullptr, "null bytes pointer");
+    NERRF_REQUIRE(n_events >= 0 && n_events < ((int64_t)1 << 31), "n_events=%lld out of range [0, 2^31)", (long long)n_events);
+    size_t kb, va, vb, sc;
+    *bytes = (int64_t)edge_label_layout(n_events, &kb, &va, &vb, &sc);
+    return NERRF_OK;
+}
+
+extern "C" int nerrf_trace_edge_labels(const int32_t* node_p, const int32_t* node_f, const uint8_t* raw_slot, int64_t n_events,
+                                       const void* rowptr, int rowptr_is64, const int32_t* col, int64_t n_edges, int64_t n_nodes,
+                                       uint8_t* label_out, void* workspace, int64_t workspace_bytes, void* stream) {
+    NERRF_REQUIRE(n_events >= 0 && n_events < ((int64_t)1 << 31), "n_events=%lld out of range [0, 2^31)", (long long)n_events);
+    NERRF_REQUIRE(n_edges >= 0 && n_nodes >= 1 && n_nodes < ((int64_t)1 << 31), "bad sizes");
+    if (n_edges == 0) return NERRF_OK;
+    NERRF_REQUIRE(rowptr && col && label_out, "null CSR / label pointer");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (n_events == 0) {                                             // no event, no attack pair
+        NERRF_CHECK_CUDA(cudaMemsetAsync(label_out, 0, (size_t)n_edges, st));
+        return NERRF_OK;
+    }
+    NERRF_REQUIRE(node_p && node_f && raw_slot, "null event column");
+    size_t kb, va, vb, sc;
+    const size_t need = edge_label_layout(n_events, &kb, &va, &vb, &sc);
+    NERRF_REQUIRE(workspace != nullptr && workspace_bytes >= (int64_t)need,
+                  "workspace too small: %lld < %lld bytes (nerrf_trace_edge_labels_workspace_bytes)", (long long)workspace_bytes,
+                  (long long)need);
+    NERRF_REQUIRE(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
+    char* ws = (char*)workspace;
+    uint64_t* ka = (uint64_t*)ws; uint64_t* kbp = (uint64_t*)(ws + kb);
+    uint32_t* vap = (uint32_t*)(ws + va); uint32_t* vbp = (uint32_t*)(ws + vb);
+    const int grid = sm_count() * 8;
+    attack_keys_kernel<<<grid, 256, 0, st>>>(node_p, node_f, raw_slot, n_events, n_nodes, ka, vap);
+    int rc = launch_status("attack_keys_kernel");
+    if (rc != NERRF_OK) return rc;
+    const int which = radix_sort_pairs(ka, kbp, vap, vbp, n_events, 0, pair_key_bits(n_nodes), ws + sc, st);
+    rc = launch_status("radix sort");
+    if (rc != NERRF_OK) return rc;
+    const uint64_t* keys = which ? kbp : ka;
+    if (rowptr_is64)
+        edge_label_kernel<int64_t><<<grid, 256, 0, st>>>((const int64_t*)rowptr, col, n_edges, n_nodes, keys, n_events, label_out);
+    else
+        edge_label_kernel<int32_t><<<grid, 256, 0, st>>>((const int32_t*)rowptr, col, n_edges, n_nodes, keys, n_events, label_out);
+    return launch_status("edge_label_kernel");
 }
 
 extern "C" int nerrf_trace_sequences(const int64_t* cand_nodes, int n_cand, const void* rowptr, int rowptr_is64, const uint32_t* perm,

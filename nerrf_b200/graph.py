@@ -92,6 +92,35 @@ def build_csr_device(src, dst, t, conf, N, t_ref=WINDOW, tau=TAU, rowptr_dtype=N
     return rowptr, col, ew
 
 
+def edge_labels_device(node_p, node_f, raw_slot, rowptr, col, n_nodes):
+    """Device per-pair edge labels (include/nerrf_b200.h nerrf_trace_edge_labels): CUDA int32 node ids per event, uint8
+    ANNOTATION event slots, and the graph's CSR -> uint8 [E] in CSR order, the rule of graph_from_events
+    meta['edge_label'].  No CPU fallback."""
+    import ctypes as C
+    import torch
+    from . import _lib
+    _lib.require_cuda(node_p, node_f, raw_slot, rowptr, col)
+    for a, dt in ((node_p, torch.int32), (node_f, torch.int32), (raw_slot, torch.uint8), (col, torch.int32)):
+        if a.dtype != dt or not a.is_contiguous():
+            raise TypeError(f"edge_labels_device: expected contiguous {dt}, got {a.dtype}")
+    if rowptr.dtype not in (torch.int32, torch.int64) or not rowptr.is_contiguous():
+        raise TypeError("rowptr must be contiguous int32 / int64")
+    n, E, dev = int(node_p.shape[0]), int(col.shape[0]), col.device
+    if not (node_f.shape[0] == raw_slot.shape[0] == n and rowptr.shape[0] == int(n_nodes) + 1):
+        raise ValueError("node_p / node_f / raw_slot must have one entry per event and rowptr n_nodes + 1")
+    h = _lib.lib()
+    with torch.cuda.device(dev):
+        need = C.c_int64()
+        _lib.check(h.nerrf_trace_edge_labels_workspace_bytes(n, C.byref(need)), "nerrf_trace_edge_labels_workspace_bytes")
+        ws = torch.empty(need.value + 256, dtype=torch.uint8, device=dev)
+        out = torch.empty(E, dtype=torch.uint8, device=dev)
+        _lib.check(h.nerrf_trace_edge_labels(_lib.ptr(node_p), _lib.ptr(node_f), _lib.ptr(raw_slot), n, _lib.ptr(rowptr),
+                                             int(rowptr.dtype == torch.int64), _lib.ptr(col), E, int(n_nodes), _lib.ptr(out),
+                                             C.c_void_p((ws.data_ptr() + 255) & ~255), need.value, _lib.current_stream_ptr()),
+                   "nerrf_trace_edge_labels")
+    return out
+
+
 def node_features_device(node_p, node_f, node_g, t, event_slot, nbytes, path_flags, node_kind, window):
     """Device per-node features (include/nerrf_b200.h nerrf_graph_node_features).  CUDA tensors: int32 node ids per
     event (node_g may be None), float64 t (seconds since the first event), uint8 event_slot / path_flags, int64|uint64

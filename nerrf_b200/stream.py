@@ -22,10 +22,17 @@ _PLACEHOLDER = b"p0000000_"          # fixed width: 7 decimal digits patched per
 _DIGITS = 7
 
 
-def _base_columns(attacked: bool, n_files: int, benign_files: int, seed: int) -> ingest.EventColumns:
-    ev = trace_sim.lockbit_trace(n_files=n_files if attacked else 0, seed=seed, benign_files=benign_files + (0 if attacked else n_files))
+def _base_columns(attacked: bool, n_files: int, benign_files: int, seed: int, bystanders: int = 0,
+                  pid_stride: int = 0) -> ingest.EventColumns:
+    ev = trace_sim.lockbit_trace(n_files=n_files if attacked else 0, seed=seed, benign_files=benign_files + (0 if attacked else n_files),
+                                 bystanders=bystanders)
     if not attacked:                      # a benign process: no encryption phase, no ransom note
         ev = [e for e in ev if e["phase"] not in ("attack",) and e["event"] not in ("encryption_start", "encryption_complete")]
+    if bystanders:                        # bystander k: pid + (k + 1) * pid_stride, clear of every replica's attacker pid
+        pid0 = ev[0]["pid"]
+        for e in ev:
+            if e["pid"] != pid0:
+                e["pid"] = pid0 + (e["pid"] - pid0) * pid_stride
     for e in ev:
         slash = e["path"].rfind("/")
         if e["path"].startswith("/app/uploads/") and slash >= 0 and "." in e["path"][slash:]:
@@ -81,12 +88,15 @@ def concat_columns(parts) -> ingest.EventColumns:
 
 
 def fleet_columns(n_procs: int, n_attacked: int, seed: int = 0, n_files: int = 45, benign_files: int = 50, jitter_s: float = 5.0,
-                  return_pids: bool = False):
+                  return_pids: bool = False, bystanders: int = 0):
     """A fleet of `n_procs` processes, each with its own n_files + benign_files files under /app/uploads (the m1
     simulator's layout); `n_attacked` of them run the LockBit encryption phase on n_files of their files.
+    bystanders: k benign processes per attacked process that open and write its files, some of the encrypted ones after
+    the attacker under their .lockbit3 name (trace_sim.lockbit_trace), each with a pid of its own; without them the
+    per-pair edge labels of a window only repeat its file labels.  bystanders=0 emits exactly the events it always did.
     -> (EventColumns, encrypted_paths: set of the .lockbit3 names a correct plan must rename back)."""
     rng = np.random.default_rng(seed)
-    att = _base_columns(True, n_files, benign_files, seed)
+    att = _base_columns(True, n_files, benign_files, seed, bystanders, pid_stride=n_procs + 1000)
     ben = _base_columns(False, n_files, benign_files, seed + 1)
     ids = rng.permutation(n_procs).astype(np.int64) + 1000
     shift = rng.random(n_procs) * jitter_s
@@ -104,7 +114,7 @@ def fleet_columns(n_procs: int, n_attacked: int, seed: int = 0, n_files: int = 4
         raw = data.tobytes()
         enc = {raw[off[i]:off[i + 1]].decode() for i in idx.tolist()}
     if return_pids:                       # the ransomware processes, by the node name the graph constructor gives them
-        return cols, enc, {"pid:%d" % p_ for p_ in np.unique(parts[0].pid).tolist()} if n_attacked else set()
+        return cols, enc, {"pid:%d" % (int(att.pid[0]) + int(i)) for i in ids[:n_attacked].tolist()}
     return cols, enc
 
 
@@ -524,9 +534,11 @@ class DeviceStream:
         v = self.d_ts_sorted[torch.tensor([lo, hi - 1], device=self.dev)].cpu().numpy()
         return lo, hi, float(v[0]), float(v[1])
 
-    def window_graph(self, t_lo: float, t_hi: float, window_s: float):
+    def window_graph(self, t_lo: float, t_hi: float, window_s: float, edge_labels: bool = False):
         """The temporal graph of the events with t_lo < t <= t_hi (device tensors), or None when there are none.
-        Same construction as ingest.graph_from_columns(stream.window(cols, t_lo, t_hi), device=...)."""
+        Same construction as ingest.graph_from_columns(stream.window(cols, t_lo, t_hi), device=...).
+        edge_labels=True also attaches meta['edge_label'] (uint8 [E] CUDA tensor, CSR order: graph_from_events' per-pair
+        rule, from the annotation slots; graph.edge_labels_device) -- the edge head's training target."""
         import ctypes as C
         from . import _lib
         torch = self.torch
@@ -591,6 +603,8 @@ class DeviceStream:
                 "node_kind": kind_d.cpu().numpy().astype(np.int64), "t0": t0, "span": span, "merge_renames": self.merge,
                 "label": lab.cpu().numpy().astype(np.int64), "size_mb": size_mb.cpu().numpy(), "device": str(self.dev),
                 "name_hash": nh, "dir_hash": dir_hash_device, "events": nw, "window_ranks": (lo, hi), "perm": perm if Gn is None else None}
+        if edge_labels:
+            meta["edge_label"] = G.edge_labels_device(P, F, self.d_raw_slot[sel], rowptr, col, N)
         return G.TemporalGraph(rowptr, col, ew, x, meta)
 
     def sequences_device(self, g: G.TemporalGraph, only_nodes):
