@@ -109,7 +109,8 @@ int nerrf_sage_layer_fwd_ex(const float* x, const void* rowptr, int rowptr_is64,
 int nerrf_sage_node_head(const float* h, const float* node_w, float node_b, float* score,
                          const float* edge_W, float* proj, int64_t row_begin, int64_t row_end,
                          int H, nerrf_stream_t stream);
-/* edge_logit[e] = proj[col_e][0:2] + proj[dst_e][2:4] + edge_b   (== [h_src||h_dst] @ We + be) */
+/* edge_logit[e] = proj[col_e][0:2] + proj[dst_e][2:4] + edge_b   (== [h_src||h_dst] @ We + be); col and edge_logit
+ * may be NULL when the graph has no edges. */
 int nerrf_sage_edge_head(const float* proj, const void* rowptr, int rowptr_is64, const int32_t* col,
                          const float* edge_b, float* edge_logit, int64_t row_begin,
                          int64_t row_end, nerrf_stream_t stream);
@@ -132,13 +133,21 @@ int nerrf_sage_forward(const float* x, const void* rowptr, int rowptr_is64, cons
  *     dZ = dP W^T;   dh = dZ[:, :F] + A^T dZ[:, F:]
  * A^T is a gather over the TRANSPOSED graph, CSR by source: t_rowptr [n+1], t_col [E] = destination of each out-edge,
  * t_w [E] = ew_e / max(weight sum of that destination, 1e-12).  dh == NULL skips the input gradient (first layer),
- * dW == NULL (with db) skips the weight gradient.  fp32, no atomics: bit-reproducible.  All pointers device,
+ * dW == NULL (with db) skips the weight gradient; t_col / t_w may be NULL when the graph has no edges.  fp32, no atomics,
+ * the chunking of the dW reduction a function of n_nodes only: bit-reproducible on every card.  All pointers device,
  * 16-byte aligned; workspace from nerrf_sage_layer_bwd_workspace_bytes. */
 int nerrf_sage_layer_bwd_workspace_bytes(int64_t n_nodes, int F, size_t* bytes);
 int nerrf_sage_layer_bwd(const float* h_in, const float* m, const float* y, const float* dy, const float* W,
                          const void* t_rowptr, int t_rowptr_is64, const int32_t* t_col, const float* t_w,
                          float* dh, float* dW, float* db, float* workspace, size_t workspace_bytes,
                          int64_t n_nodes, int F, int H, int relu, nerrf_stream_t stream);
+
+/* The normalised edge weights of the graph, for t_w above: a[e] = ew[e] * (1 / max(weight sum of e's destination row,
+ * 1e-12)), edges in CSR-by-destination order (rowptr [n+1], int32 or int64 when rowptr_is64; ew, a [E]).  The weight sum
+ * is taken in the order nerrf_sage_aggregate takes it, so the entries are the forward's to the bit.  No atomics:
+ * bit-reproducible.  ew and a may be NULL when the graph has no edges. */
+int nerrf_sage_norm_weights(const void* rowptr, int rowptr_is64, const float* ew, float* a, int64_t n_nodes,
+                            nerrf_stream_t stream);
 
 /* Edge head backward (training the attack / normal edge classifier).  Forward = nerrf_sage_node_head (proj) +
  * nerrf_sage_edge_head.  Given d_logit [E,2] = d loss / d edge_logit in CSR-by-destination order:

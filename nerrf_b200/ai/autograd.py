@@ -23,7 +23,9 @@ from .. import _lib as L
 class TrainGraph:
     """A graph prepared for training: CSR by destination (what the forward reads) + its transpose, CSR by source with the
     edge weights pre-normalised by the destination's weight sum (what the backward of the aggregate gathers over).
-    Built once per graph with device-wide torch primitives (sort / bincount / cumsum): preparation, not the hot path."""
+    Built once per graph with device-wide torch primitives (sort / bincount / cumsum) and `nerrf_sage_norm_weights` for
+    the normalised weights (no float atomics, so two constructions of one graph give the same bits): preparation, not
+    the hot path."""
 
     def __init__(self, rowptr, col, edge_w):
         L.require_cuda(rowptr, col, edge_w)
@@ -32,8 +34,10 @@ class TrainGraph:
         self.n = n
         deg = (rowptr[1:] - rowptr[:-1]).long()
         dst = torch.repeat_interleave(torch.arange(n, device=rowptr.device), deg)
-        wsum = torch.zeros(n, device=rowptr.device, dtype=torch.float32).index_add_(0, dst, edge_w)
-        a = edge_w / wsum.clamp_min(1e-12)[dst]
+        a = torch.empty_like(self.edge_w)
+        with torch.cuda.device(rowptr.device):
+            L.check(L.lib().nerrf_sage_norm_weights(L.ptr(self.rowptr), int(rowptr.dtype == torch.int64), L.ptr(self.edge_w),
+                                                    L.ptr(a), n, L.current_stream_ptr()), "nerrf_sage_norm_weights")
         src = col.long()
         order = torch.sort(src, stable=True).indices
         t_rowptr = torch.zeros(n + 1, device=rowptr.device, dtype=torch.int64)

@@ -356,7 +356,7 @@ extern "C" int nerrf_sage_node_head(const float* h, const float* node_w, float n
 extern "C" int nerrf_sage_edge_head(const float* proj, const void* rowptr, int rowptr_is64, const int32_t* col,
                                     const float* edge_b, float* edge_logit, int64_t row_begin, int64_t row_end,
                                     nerrf_stream_t stream) {
-    NERRF_REQUIRE(proj && rowptr && col && edge_b && edge_logit, "null pointer");
+    NERRF_REQUIRE(proj && rowptr && edge_b, "null pointer");     // col / edge_logit may be null when the graph has no edges
     NERRF_REQUIRE(row_begin >= 0 && row_begin <= row_end, "bad row range");
     const int64_t rows = row_end - row_begin;
     if (rows == 0) return NERRF_OK;

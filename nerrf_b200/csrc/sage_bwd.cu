@@ -1,5 +1,6 @@
 // GraphSAGE-T layer BACKWARD (SURVEY.md 8f rank 3: "backward for K1/K2"; reference surface: ai/train.py, README.md:75,
-// ROADMAP.md:62-69 -- named, never written).  fp32, deterministic (no atomics: every reduction has a fixed order).
+// ROADMAP.md:62-69 -- named, never written).  fp32, deterministic (no atomics: every reduction has a fixed order, and the
+// row chunking of the weight gradient depends on n only, so every card gives the same bits).
 //
 //   forward   Z = [h || m],  m = A h (A = row-normalised weighted adjacency, CSR by destination),  Y = act(Z W + b)
 //   backward  dP = dY * [Y > 0]                      (ReLU mask from the saved output)
@@ -17,6 +18,8 @@
 //                        (4 x 8 per thread) and writes a partial; slab 0 also accumulates db
 //   sage_bwd_reduce_kernel  partials -> dW / db, chunk order fixed
 //   sage_bwd_dh_kernel   one warp per source row: dZ[u, :F] + gather of dZ[dst, F:] over the transposed row
+//   sage_norm_weights_kernel  one warp per destination row: a_e = w_e / max(row weight sum, 1e-12), the weight sum taken in
+//                        gather_row's lane order and warp_sum, so A^T holds the forward aggregate's A entries to the bit
 #include "common.cuh"
 #include "sage_gather.cuh"
 
@@ -34,6 +37,7 @@ constexpr int DW_BR = 32;            // rows per dW tile
 constexpr int DW_KS = 64;            // k rows of dW per CTA slab
 constexpr int DW_LDZ = DW_KS + 4;
 constexpr int DW_LDP = HB + 4;
+constexpr int MAX_CHUNKS = 264;      // dW row chunks at most (2 per SM of a 132-SM H100, fixed so the bits do not depend on the card)
 
 // dZ[r, k] = sum_j dP[r, j] W[k, j],  dP = dY * [Y > 0] (relu) or dY
 template <int F>
@@ -198,6 +202,21 @@ __global__ void __launch_bounds__(256) sage_bwd_dh_kernel(const float* __restric
     }
 }
 
+// a[e] = ew[e] * (1 / max(sum of the row's weights, 1e-12)) over the CSR-by-destination rows: lane l sums edges e0 + l,
+// e0 + l + 32, ... then warp_sum, exactly as gather_row sums the weights it normalises by
+template <typename RP>
+__global__ void __launch_bounds__(256) sage_norm_weights_kernel(const RP* __restrict__ rowptr, const float* __restrict__ ew,
+                                                                float* __restrict__ a, int64_t n) {
+    const int lane = threadIdx.x & 31;
+    const int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (row >= n) return;
+    const int64_t e0 = rowptr[row], e1 = rowptr[row + 1];
+    float wpart = 0.f;
+    for (int64_t e = e0 + lane; e < e1; e += 32) wpart += __ldg(ew + e);
+    const float inv = 1.0f / fmaxf(warp_sum(wpart), 1e-12f);
+    for (int64_t e = e0 + lane; e < e1; e += 32) a[e] = __ldg(ew + e) * inv;
+}
+
 struct BwdPlan {
     int chunks;
     int64_t rows_per_chunk;
@@ -206,9 +225,8 @@ struct BwdPlan {
 BwdPlan bwd_plan(int64_t n, int F) {
     BwdPlan p;
     int64_t tiles = (n + DW_BR - 1) / DW_BR;
-    int64_t c = 2 * (int64_t)sm_count();
-    if (c > tiles) c = tiles;
-    if (c < 1) c = 1;
+    if (tiles < 1) tiles = 1;                               // n = 0: one empty chunk
+    const int64_t c = tiles < MAX_CHUNKS ? tiles : MAX_CHUNKS;
     p.rows_per_chunk = ((tiles + c - 1) / c) * DW_BR;
     p.chunks = (int)((n + p.rows_per_chunk - 1) / p.rows_per_chunk);
     if (p.chunks < 1) p.chunks = 1;
@@ -266,7 +284,7 @@ extern "C" int nerrf_sage_layer_bwd(const float* h_in, const float* m, const flo
     NERRF_REQUIRE(dy && W && workspace, "null pointer");
     NERRF_REQUIRE(!relu || y, "the ReLU mask needs the layer output y");
     NERRF_REQUIRE(!dW || (h_in && m && db), "dW needs h_in, m and db");
-    NERRF_REQUIRE(!dh || (t_rowptr && t_col && t_w), "dh needs the transposed graph");
+    NERRF_REQUIRE(!dh || t_rowptr, "dh needs the transposed graph");     // t_col / t_w may be null when the graph has no edges
     size_t need = 0;
     nerrf_sage_layer_bwd_workspace_bytes(n_nodes, F, &need);
     if (workspace_bytes < need) {
@@ -289,4 +307,19 @@ extern "C" int nerrf_sage_layer_bwd(const float* h_in, const float* m, const flo
         case 64: return launch_bwd<64>(h_in, m, y, dy, W, t_rowptr, t_rowptr_is64, t_col, t_w, dh, dW, db, workspace, n_nodes, relu, st);
         default: return launch_bwd<128>(h_in, m, y, dy, W, t_rowptr, t_rowptr_is64, t_col, t_w, dh, dW, db, workspace, n_nodes, relu, st);
     }
+}
+
+extern "C" int nerrf_sage_norm_weights(const void* rowptr, int rowptr_is64, const float* ew, float* a, int64_t n_nodes,
+                                       nerrf_stream_t stream) {
+    NERRF_REQUIRE(n_nodes >= 0, "negative node count");
+    NERRF_REQUIRE(rowptr, "null rowptr");                     // ew / a may be null when the graph has no edges
+    if (n_nodes == 0) return NERRF_OK;
+    NERRF_REQUIRE(n_nodes / 8 < (1ll << 31), "too many nodes");
+    const unsigned blocks = (unsigned)((n_nodes + 7) / 8);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (rowptr_is64)
+        sage_norm_weights_kernel<int64_t><<<blocks, 256, 0, st>>>((const int64_t*)rowptr, ew, a, n_nodes);
+    else
+        sage_norm_weights_kernel<int32_t><<<blocks, 256, 0, st>>>((const int32_t*)rowptr, ew, a, n_nodes);
+    return launch_status("sage edge weight normalisation");
 }

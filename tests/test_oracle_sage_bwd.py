@@ -63,3 +63,63 @@ def test_hand_computed_layer_backward():
     # dZ = dy * [2, 4]; dh_u = 2 dy_u + sum over out-edges a_e * 4 dy_dst
     assert np.allclose(dh[:, 0], [2 * 1 + 0.25 * 40, 2 * 10 + 1.0 * 400, 2 * 100 + 0.75 * 40])
     assert np.allclose(dW[:, 0], [1 * 1 + 2 * 10 + 3 * 100, 0 + 2.5 * 10 + 2 * 100]) and np.allclose(db, [111.0])
+
+
+def _pin_graphs():
+    """(name, rowptr, col, ew, x): the small graphs above, a hub-destination graph, and degenerate_graph with and without
+    edges (isolated nodes, self-loops, multi-edges, a row of weights summing below 1e-12, a row of zero weights)."""
+    for (N, E, seed, hub) in [(300, 2500, 3, "src"), (64, 40, 4, "src"), (500, 9000, 5, "src"), (400, 6000, 6, "dst")]:
+        g = synthetic_graph(N=N, E=E, seed=seed, hub=hub)
+        yield f"synthetic-{N}-{hub}", g.rowptr, g.col, g.ew, g.x
+    for (N, E, seed) in [(200, 1500, 7), (50, 0, 8)]:
+        rowptr, col, ew = B.degenerate_graph(N, E, seed)
+        yield f"degenerate-{N}-{E}", rowptr, col, ew, np.random.default_rng(seed).standard_normal((N, 32)).astype(np.float32)
+
+
+def _rel(got, want, what, rtol=1e-12):
+    got, want = np.asarray(got, np.float64), np.asarray(want, np.float64)
+    scale = float(np.abs(want).max()) if want.size else 0.0
+    assert got.shape == want.shape, what
+    assert want.size == 0 or float(np.abs(got - want).max()) <= rtol * max(scale, 1e-300), what
+
+
+def test_degenerate_graph_has_the_rows_it_promises():
+    rowptr, col, ew = B.degenerate_graph(200, 1500, 7)
+    dst = B.edge_dst(rowptr)
+    deg_in, deg_out = np.diff(rowptr), np.bincount(col, minlength=200)
+    iso = np.arange(200) % 7 == 3
+    assert np.all(deg_in[iso] == 0) and np.all(deg_out[iso] == 0)
+    assert np.any(col == dst)                                                     # self-loops
+    pairs = col.astype(np.int64) * 200 + dst
+    assert np.unique(pairs).size < pairs.size                                     # multi-edges
+    assert 0 < ew[dst == 1].sum(dtype=np.float64) < 1e-12 and np.all(ew[dst == 2] == 0) and deg_in[2] > 0
+
+
+def test_sparse_oracle_equals_the_edge_by_edge_oracle():
+    """sparse=True (scipy CSR products) and the np.add.at path compute the same statements: 1e-12 relative."""
+    from edge_head_ref import edge_head_backward, model_backward_with_edges
+    P = S.make_params(32, 128, 2, seed=9)
+    for name, rowptr, col, ew, x in _pin_graphs():
+        N, E = rowptr.size - 1, col.size
+        rng = np.random.default_rng(N + E)
+        h = np.maximum(rng.standard_normal((N, 32)), 0)
+        _rel(B.aggregate(h, rowptr, col, ew, sparse=True), B.aggregate(h, rowptr, col, ew), f"{name} m")
+        dlogit, dedge = rng.standard_normal(N), rng.standard_normal((E, 2))
+        want = B.model_backward(P, x, rowptr, col, ew, dlogit)
+        got = B.model_backward(P, x, rowptr, col, ew, dlogit, sparse=True)
+        for k in ("x", "node_w", "node_b"):
+            _rel(got[k], want[k], f"{name} {k}")
+        for l, ((dW, db), (wW, wb)) in enumerate(zip(got["layers"], want["layers"])):
+            _rel(dW, wW, f"{name} dW[{l}]"); _rel(db, wb, f"{name} db[{l}]")
+        hh = rng.standard_normal((N, 128))
+        for a, b, k in zip(edge_head_backward(hh, P["edge_W"], dedge, rowptr, col, sparse=True),
+                           edge_head_backward(hh, P["edge_W"], dedge, rowptr, col), ("dh", "dWe", "dbe")):
+            _rel(a, b, f"{name} edge head {k}")
+        want = model_backward_with_edges(P, x, rowptr, col, ew, dlogit, dedge)
+        got = model_backward_with_edges(P, x, rowptr, col, ew, dlogit, dedge, sparse=True)
+        for k in ("x", "node_w", "node_b", "edge_W", "edge_b"):
+            _rel(got[k], want[k], f"{name} both heads {k}")
+        for l, ((dW, db), (wW, wb)) in enumerate(zip(got["layers"], want["layers"])):
+            _rel(dW, wW, f"{name} both heads dW[{l}]"); _rel(db, wb, f"{name} both heads db[{l}]")
+        if E == 0:                                   # no edges: the aggregate is zero and dh is the self half of dZ
+            assert np.all(B.aggregate(h, rowptr, col, ew, sparse=True) == 0)
