@@ -78,9 +78,25 @@ def _layers(params, dtype):
     return [[tuple(_arr(w, dtype) for w in d) for d in layer] for layer in params["lstm"]]
 
 
-def logits(params, seq, lengths, dtype=np.float64):
-    """Head logits [B,2] (pre-sigmoid) = [h_fwd_final || h_bwd_final] head_W^T + head_b."""
+def _slices(n, batch):
+    """Consecutive slices of at most `batch` sequences covering [0, n), or None when one pass does (batch None or >= n).
+    Sequences are independent, so logits and dseq of a batch are those of its slices side by side, and the parameter
+    gradients are the sum of the slices' gradients: slicing bounds the float64 tape (~5.7 MB per 100-step sequence of a
+    2-layer H = 256 stack) without changing what is computed."""
+    if batch is None or batch >= n:
+        return None
+    if batch < 1:
+        raise ValueError("batch must be >= 1")
+    return [slice(s, min(s + batch, n)) for s in range(0, n, batch)]
+
+
+def logits(params, seq, lengths, dtype=np.float64, batch=None):
+    """Head logits [B,2] (pre-sigmoid) = [h_fwd_final || h_bwd_final] head_W^T + head_b.  batch: evaluate `batch`
+    sequences at a time (same result; bounds memory)."""
     x = _arr(seq, dtype); lengths = np.asarray(_arr(lengths, np.int64))
+    parts = _slices(x.shape[0], batch)
+    if parts is not None:
+        return np.concatenate([logits(params, x[s], lengths[s], dtype) for s in parts], 0)
     hf = hb = None
     for fw, bw in _layers(params, dtype):
         of, hf, _ = direction_forward(x, lengths, *fw, reverse=False)
@@ -89,12 +105,30 @@ def logits(params, seq, lengths, dtype=np.float64):
     return np.concatenate([hf, hb], 1) @ _arr(params["head_W"], dtype).T + _arr(params["head_b"], dtype)
 
 
-def model_backward(params, seq, lengths, dlogit, dtype=np.float64):
+def model_backward(params, seq, lengths, dlogit, dtype=np.float64, batch=None):
     """Gradients of sum(dlogit * logits(params, seq, lengths)) w.r.t. every parameter and seq.  params as
     oracle/lstm_ref.py (numpy arrays or torch tensors).  -> dict(lstm=[[(dW_ih, dW_hh, db_ih, db_hh) fwd, (...) bwd]
-    per layer], head_W, head_b, seq); db_ih == db_hh (the two biases enter the gates as one sum)."""
-    layers = _layers(params, dtype)
+    per layer], head_W, head_b, seq, logits); db_ih == db_hh (the two biases enter the gates as one sum); logits are
+    those of logits(), from the same forward pass.  batch: differentiate `batch` sequences at a time and sum the parameter
+    gradients over the slices in slice order (bounds memory)."""
     x = _arr(seq, dtype); lengths = np.asarray(_arr(lengths, np.int64))
+    parts = _slices(x.shape[0], batch)
+    if parts is not None:
+        dlogit = _arr(dlogit, dtype)
+        out = None
+        for s in parts:
+            g = model_backward(params, x[s], lengths[s], dlogit[s], dtype)
+            if out is None:
+                out = g
+                out["seq"], out["logits"] = [g["seq"]], [g["logits"]]
+                continue
+            out["head_W"] += g["head_W"]; out["head_b"] += g["head_b"]
+            out["seq"].append(g["seq"]); out["logits"].append(g["logits"])
+            out["lstm"] = [[tuple(a + b for a, b in zip(da, db)) for da, db in zip(la, lb)]
+                           for la, lb in zip(out["lstm"], g["lstm"])]
+        out["seq"], out["logits"] = np.concatenate(out["seq"], 0), np.concatenate(out["logits"], 0)
+        return out
+    layers = _layers(params, dtype)
     B, T, _ = x.shape
     H = layers[0][0][1].shape[1]
     ins, tapes = [], []
@@ -106,7 +140,8 @@ def model_backward(params, seq, lengths, dlogit, dtype=np.float64):
     feat = np.concatenate([hf, hb], 1)
     dlogit = _arr(dlogit, dtype)
     head_W = _arr(params["head_W"], dtype)
-    out = {"head_W": dlogit.T @ feat, "head_b": dlogit.sum(0), "lstm": [None] * len(layers)}
+    out = {"head_W": dlogit.T @ feat, "head_b": dlogit.sum(0), "lstm": [None] * len(layers),
+           "logits": feat @ head_W.T + _arr(params["head_b"], dtype)}
     dfeat = dlogit @ head_W
     dout = np.zeros((B, T, 2 * H), dtype)
     for l in reversed(range(len(layers))):

@@ -93,6 +93,34 @@ def test_oracle_equals_autograd_of_the_forward_oracle(L, D, T):
     assert not np.any(got["seq"][2])
 
 
+@pytest.mark.parametrize("batch", [1, 4, 8])
+def test_sliced_oracle_equals_the_whole_batch(batch):
+    """logits / model_backward with batch= (the form the scale tests use) against one pass over the whole batch: logits
+    and dseq concatenate, parameter gradients sum.  The slice boundaries at 4 and 8 fall between a full-length and a
+    zero-length sequence."""
+    T, D, L = 9, 5, 2
+    P = R.make_params(D, HID, L, seed=17)
+    rng = np.random.default_rng(18)
+    lengths = np.array([3, 1, 6, T, 0, 2, 5, 0, T, 4, 0])
+    seq = rng.standard_normal((lengths.size, T, D))
+    dlogit = rng.standard_normal((lengths.size, 2))
+    whole = B.model_backward(P, seq, lengths, dlogit)
+    part = B.model_backward(P, seq, lengths, dlogit, batch=batch)
+
+    def near(a, b):
+        assert a.shape == b.shape
+        assert np.abs(a - b).max() <= 1e-12 * max(1.0, float(np.abs(b).max()))
+    want_logits = B.logits(P, seq, lengths)
+    near(B.logits(P, seq, lengths, batch=batch), want_logits)
+    near(part["logits"], want_logits); near(whole["logits"], want_logits)
+    near(part["seq"], whole["seq"]); near(part["head_W"], whole["head_W"]); near(part["head_b"], whole["head_b"])
+    for la, lb in zip(part["lstm"], whole["lstm"]):
+        for da, db in zip(la, lb):
+            for a, b in zip(da, db):
+                near(a, b)
+    assert not part["seq"][4].any() and not part["seq"][7].any()
+
+
 def test_hand_computed_h1_t2():
     """H = 1, D_in = 1, T = 2, one layer: the forward direction's gradients written out as scalars, and checked against
     central differences of the scalar forward."""
