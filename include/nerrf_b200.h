@@ -447,6 +447,9 @@ int nerrf_trace_decode_device(const uint8_t* buf, const int64_t* rec_at, const i
  *   retain_out [n_retain] (may be NULL) = in stored order, the events with ts > horizon and, per pid, its latest event
  *     with a path at or before the horizon (a later path-less write still resolves to it).
  * counts (HOST [3]) = n_keep, n_retain, total bytes of the resolved path column; the call synchronises the stream.
+ * The resolved path column repeats a path for every path-less event that resolves to it, so it can be far larger than the
+ * stored one: its size is summed in 64 bits, and 2^31 bytes or more is NERRF_ERR_INVALID (the offsets are scanned in
+ * int32; the outputs are then unspecified and counts is zero).
  * workspace: 256-byte aligned, nerrf_trace_stream_order_workspace_bytes. */
 int nerrf_trace_stream_order_workspace_bytes(int64_t n_events, int64_t* bytes);
 int nerrf_trace_stream_order(int64_t n_events, const int64_t* ts_sec, const int32_t* ts_nanos, const uint32_t* pid,
@@ -463,7 +466,9 @@ int nerrf_trace_stream_columns(int64_t n_events, const int64_t* src, const int64
                                int merge_renames, uint8_t* res_path_data, uint8_t* pf_out, uint8_t* pf_raw_out,
                                uint8_t* slot_out, void* stream);
 /* cols_out row k = cols_in row rows[k] (device int64 [n_rows], distinct rows, so every output data array fits in the
- * input's size); string offsets restart at 0.  Asynchronous; workspace from nerrf_trace_gather_rows_workspace_bytes. */
+ * input's size); string offsets restart at 0.  The string bytes of the gathered rows, all four columns together, must
+ * stay below 2^31 (one int32 scan turns their lengths into offsets; the call is asynchronous and cannot check the sum:
+ * nerrf_b200/stream.py compact() does).  Asynchronous; workspace from nerrf_trace_gather_rows_workspace_bytes. */
 int nerrf_trace_gather_rows_workspace_bytes(int64_t n_rows, int64_t* bytes);
 int nerrf_trace_gather_rows(void* const* cols_in, const int64_t* rows, int64_t n_rows, void* const* cols_out,
                             void* workspace, int64_t workspace_bytes, void* stream);

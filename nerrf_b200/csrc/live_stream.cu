@@ -217,6 +217,7 @@ struct OrderArgs {
     int32_t *A, *G, *C;          // [n] max-scans over the regroup: last named, group start, last named at or before the horizon
     int32_t *F, *R, *L;          // [n] keep flags by time rank, retain flags / resolved path lengths by stored index
     int64_t* src;                // [n] source event of the path (-1: dropped)
+    unsigned long long* res_bytes;   // the sum of L in 64 bits: L is scanned in int32, and the caller checks this first
 };
 
 __device__ __forceinline__ uint64_t orderable(double t) {
@@ -227,6 +228,7 @@ __device__ __forceinline__ uint64_t orderable(double t) {
 
 __global__ void __launch_bounds__(256) order_keys_kernel(OrderArgs a, uint64_t* __restrict__ key, uint32_t* __restrict__ val) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    if (blockIdx.x == 0 && threadIdx.x == 0) *a.res_bytes = 0ull;
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += stride) {
         // seconds + nanos * 1e-9 rounded exactly like numpy (two roundings, no FMA contraction)
         const double t = __dadd_rn((double)a.ts_sec[i], __dmul_rn((double)a.ts_nanos[i], 1e-9));
@@ -270,11 +272,18 @@ __global__ void __launch_bounds__(256) order_resolve_kernel(OrderArgs a) {
 }
 __global__ void __launch_bounds__(256) order_flags_kernel(OrderArgs a) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    unsigned long long bytes = 0ull;
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < a.n; k += stride) {
         a.F[k] = a.src[a.tord[k]] >= 0 ? 1 : 0;
         const int64_t s = a.src[k];
-        a.L[k] = s >= 0 ? (int32_t)(a.path_off[s + 1] - a.path_off[s]) : 0;
+        const int64_t len = s >= 0 ? a.path_off[s + 1] - a.path_off[s] : 0;
+        a.L[k] = (int32_t)len;
+        bytes += (unsigned long long)len;
     }
+    // a path is repeated for every path-less write that resolves to it, so the stored bytes do not bound this sum
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) bytes += __shfl_down_sync(0xffffffffu, bytes, o);
+    if ((threadIdx.x & 31) == 0 && bytes) atomicAdd(a.res_bytes, bytes);
 }
 // exclusive-scanned flags -> compacted lists
 __global__ void __launch_bounds__(256) order_compact_kernel(OrderArgs a, const int32_t* __restrict__ totals, int64_t* __restrict__ order,
@@ -414,6 +423,7 @@ extern "C" int nerrf_trace_stream_order(int64_t n_events, const int64_t* ts_sec,
     a.ts = ts_out; a.tord = (uint32_t*)(ws + L.tord); a.byp = (uint32_t*)(ws + L.byp);
     a.A = (int32_t*)(ws + L.A); a.G = (int32_t*)(ws + L.G); a.C = (int32_t*)(ws + L.C);
     a.F = (int32_t*)(ws + L.F); a.R = (int32_t*)(ws + L.R); a.L = (int32_t*)(ws + L.L); a.src = src_out;
+    a.res_bytes = (unsigned long long*)(ws + L.totals + 16);               // after the three int32 scan totals
     uint64_t *ka = (uint64_t*)(ws + L.ka), *kb = (uint64_t*)(ws + L.kb);
     uint32_t *va = (uint32_t*)(ws + L.va), *vb = (uint32_t*)(ws + L.vb);
     int32_t* sums = (int32_t*)(ws + L.sums);
@@ -435,10 +445,14 @@ extern "C" int nerrf_trace_stream_order(int64_t n_events, const int64_t* ts_sec,
     order_compact_kernel<<<grid, 256, 0, st>>>(a, totals, order_out, ts_sorted_out, retain_out, res_path_off);
     int rc = launch_status("stream order kernels");
     if (rc) return rc;
-    int32_t h[3];
-    NERRF_CHECK_CUDA(cudaMemcpyAsync(h, totals, sizeof(h), cudaMemcpyDeviceToHost, st));
+    struct { int32_t scan[4]; unsigned long long res_bytes; } h;
+    NERRF_CHECK_CUDA(cudaMemcpyAsync(&h, totals, sizeof(h), cudaMemcpyDeviceToHost, st));
     NERRF_CHECK_CUDA(cudaStreamSynchronize(st));
-    counts[0] = h[0]; counts[1] = h[1]; counts[2] = h[2];
+    // the resolved path offsets come from an int32 scan: past 2^31 - 1 bytes they have wrapped and nothing may read them
+    NERRF_REQUIRE(h.res_bytes < (1ull << 31),
+                  "resolved paths of %llu bytes: at most 2^31 - 1 per stream (a path counts once for every path-less event "
+                  "that resolves to it); compact the stream or split it", h.res_bytes);
+    counts[0] = h.scan[0]; counts[1] = h.scan[1]; counts[2] = h.scan[2];
     return NERRF_OK;
 }
 

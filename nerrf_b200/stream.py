@@ -323,6 +323,23 @@ def _decode_into(dc: _DeviceColumns, n: int, used_bytes, raw: np.ndarray, partia
     return m, consumed, used
 
 
+def _rows_string_bytes(dc: _DeviceColumns, rows) -> list:
+    """bytes of each of the four string columns held by `rows` (device int64 indices) of `dc`"""
+    import torch
+    if rows.numel() == 0:
+        return [0, 0, 0, 0]
+    return [int(v) for v in torch.stack([(o[rows + 1] - o[rows]).sum() for o in dc.off]).cpu().numpy()]
+
+
+def _require_gather_fits(nbytes):
+    """nerrf_trace_gather_rows turns the lengths of all four string columns into offsets with ONE int32 scan: the bytes
+    it moves must sum to less than 2^31 (the per-append limit of _decode_into, for the rows a compaction keeps)."""
+    from . import _lib
+    total = sum(int(b) for b in nbytes)
+    if total >= (1 << 31):
+        raise _lib.NerrfError("compaction keeps %d string bytes: at most 2^31 - 1 (advance the horizon, or compact more often)" % total)
+
+
 def decode_event_batch_device(buf, device="cuda") -> ingest.EventColumns:
     """ingest.decode_event_batch with the Event bodies parsed ON THE DEVICE (nerrf_trace_decode_device): the same
     columns, brought back to the host."""
@@ -413,9 +430,14 @@ class DeviceStream:
         self.timings_ms = {}
         m, consumed, used = _decode_into(self._dc, self.n, self._used, raw, partial, self.timings_ms)
         if m:
+            before = self.n, self._used
             self.n += m
             self._used = used
-            self._rebuild()
+            try:
+                self._rebuild()
+            except Exception:                                  # e.g. 2^31 resolved path bytes: the rows stay unused past n
+                self.n, self._used = before
+                raise
         return consumed
 
     def compact(self, horizon: float):
@@ -431,6 +453,10 @@ class DeviceStream:
         self._rebuild()
         if self._n_retain < self.n:
             m = self._n_retain
+            nbytes = self._used                                # distinct rows: at most the stored bytes of each column
+            if sum(nbytes) >= 1 << 31:
+                nbytes = _rows_string_bytes(self._dc, self._retain)
+            _require_gather_fits(nbytes)
             out = _DeviceColumns(self.dev, self._dc.rows, [d.numel() for d in self._dc.data])
             need = C.c_int64()
             _lib.check(_lib.lib().nerrf_trace_gather_rows_workspace_bytes(m, C.byref(need)), "gather_rows_workspace_bytes")
