@@ -507,6 +507,46 @@ int nerrf_trace_intern(int64_t n_events, const int64_t* order, const uint32_t* p
                        int8_t* node_kind, int64_t* node_name_event, int8_t* node_name_which,
                        int64_t node_capacity);
 
+/* ------------------------------------------------------------------ several sources (one tracker per node)
+ * Every event carries a source id s in [0, 2^16) (uint16 column, device or host like the other columns).  A process is
+ * (s, pid) and a file is (s, path merge key): a rename target aliases within its own source, a path-less write resolves
+ * to the latest named event of the same (s, pid), and retention keeps that event per (s, pid).  Name and directory
+ * hashes are qualified by s and equal the unqualified ones at s = 0.  Each _ex entry point with source == NULL is the
+ * entry point without the suffix, bit for bit (those are these calls with source = NULL).
+ *
+ * nerrf_trace_decode_device_ex: every decoded row gets source_col[row] = source (source_col NULL: not written).
+ * nerrf_trace_stream_order_ex: key_bits 32 regroups by pid alone (4 radix passes; right whenever all events share one
+ *   source), 48 by (source << 32) | pid (6 passes; needs the source column).
+ * nerrf_trace_gather_rows_ex: also source_out[k] = source_in[rows[k]] (source_in NULL: 0; source_out NULL: skipped). */
+int nerrf_trace_decode_device_ex(const uint8_t* buf, const int64_t* rec_at, const int64_t* body_off, const int64_t* body_len,
+                                 int64_t n_records, int64_t n_old, void* const* cols, uint16_t* source_col, int source,
+                                 uint64_t* status, void* workspace, int64_t workspace_bytes, void* stream);
+int nerrf_trace_stream_order_ex(int64_t n_events, const int64_t* ts_sec, const int32_t* ts_nanos, const uint32_t* pid,
+                                const uint16_t* source, int key_bits, const int64_t* path_off, double horizon,
+                                double* ts_out, int64_t* order_out, double* ts_sorted_out, int64_t* src_out,
+                                int64_t* res_path_off, int64_t* retain_out, int64_t* counts, void* workspace,
+                                int64_t workspace_bytes, void* stream);
+int nerrf_trace_gather_rows_ex(void* const* cols_in, const uint16_t* source_in, const int64_t* rows, int64_t n_rows,
+                               void* const* cols_out, uint16_t* source_out, void* workspace, int64_t workspace_bytes,
+                               void* stream);
+int nerrf_trace_intern_device_ex(int64_t n_events, int64_t n_stored, const int64_t* order, const uint32_t* pid,
+                                 const uint16_t* source, const int64_t* path_off, const uint8_t* path_data,
+                                 const int64_t* new_path_off, const uint8_t* new_path_data, int merge_renames,
+                                 int32_t* node_p, int32_t* node_f, int32_t* node_g, int64_t* n_nodes, int8_t* node_kind,
+                                 int64_t* node_name_event, int8_t* node_name_which, int64_t node_capacity,
+                                 void* workspace, int64_t workspace_bytes, void* stream);
+int nerrf_trace_name_hash_ex(int64_t n_nodes, const int64_t* node_name_event, const int8_t* node_name_which,
+                             const uint32_t* pid, const uint16_t* source, const int64_t* path_off, const uint8_t* path_data,
+                             const int64_t* new_path_off, const uint8_t* new_path_data, uint64_t* hash_out, void* stream);
+int nerrf_trace_dir_hash_ex(int64_t n_nodes, const int64_t* node_name_event, const int8_t* node_name_which,
+                            const uint32_t* pid, const uint16_t* source, const int64_t* path_off, const uint8_t* path_data,
+                            const int64_t* new_path_off, const uint8_t* new_path_data, uint64_t* hash_out, void* stream);
+int nerrf_trace_intern_ex(int64_t n_events, const int64_t* order, const uint32_t* pid, const uint16_t* source,
+                          const int64_t* path_off, const uint8_t* path_data, const int64_t* new_path_off,
+                          const uint8_t* new_path_data, int merge_renames, int32_t* node_p, int32_t* node_f,
+                          int32_t* node_g, int64_t* n_nodes, int8_t* node_kind, int64_t* node_name_event,
+                          int8_t* node_name_which, int64_t node_capacity);
+
 #ifdef __cplusplus
 }
 #endif

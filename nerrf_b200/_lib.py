@@ -110,6 +110,17 @@ SIGNATURES = {
     "nerrf_trace_dir_hash": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
     "nerrf_trace_intern": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, C.c_int, vp, vp, vp, C.POINTER(C.c_int64),
                                      vp, vp, vp, C.c_int64]),
+    "nerrf_trace_decode_device_ex": (C.c_int, [vp, vp, vp, vp, C.c_int64, C.c_int64, C.POINTER(vp), vp, C.c_int, vp, vp, C.c_int64,
+                                               vp]),
+    "nerrf_trace_stream_order_ex": (C.c_int, [C.c_int64, vp, vp, vp, vp, C.c_int, vp, C.c_double, vp, vp, vp, vp, vp, vp,
+                                              C.POINTER(C.c_int64), vp, C.c_int64, vp]),
+    "nerrf_trace_gather_rows_ex": (C.c_int, [C.POINTER(vp), vp, vp, C.c_int64, C.POINTER(vp), vp, vp, C.c_int64, vp]),
+    "nerrf_trace_intern_device_ex": (C.c_int, [C.c_int64, C.c_int64, vp, vp, vp, vp, vp, vp, vp, C.c_int, vp, vp, vp,
+                                               C.POINTER(C.c_int64), vp, vp, vp, C.c_int64, vp, C.c_int64, vp]),
+    "nerrf_trace_name_hash_ex": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "nerrf_trace_dir_hash_ex": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]),
+    "nerrf_trace_intern_ex": (C.c_int, [C.c_int64, vp, vp, vp, vp, vp, vp, vp, C.c_int, vp, vp, vp, C.POINTER(C.c_int64),
+                                        vp, vp, vp, C.c_int64]),
 }
 
 

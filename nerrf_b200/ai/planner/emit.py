@@ -16,11 +16,25 @@ Reference anchors (prose + the M1 harness; no emitter exists in the reference):
 from __future__ import annotations
 
 import json
+import re
 import shlex
+
+import numpy as np
 
 PLAN_VERSION = 1
 ENCRYPTED_SUFFIX = ".lockbit3"      # benchmarks/m1/scripts/m1_rollback.sh:95 (`for f in *.lockbit3`)
 RESTORED_SUFFIX = ".dat"            # benchmarks/m1/scripts/m1_rollback.sh:98 (`mv "$f" "${base}.dat"`)
+
+
+_HOST_NAME = re.compile(r"[A-Za-z0-9._-]{1,64}")
+
+
+def check_host_name(name) -> str:
+    """A source (host) name becomes a file name (<host>.sh) and a plan field: 1-64 characters of [A-Za-z0-9._-], and
+    not "." or ".." (which name directories).  Anything else raises ValueError."""
+    if not isinstance(name, str) or not _HOST_NAME.fullmatch(name) or name in (".", ".."):
+        raise ValueError("bad host name %r: 1-64 characters of [A-Za-z0-9._-], not '.' or '..'" % (name,))
+    return name
 
 
 def _has_control_chars(path: str) -> bool:
@@ -55,13 +69,16 @@ def restore_dir_step(directory: str, covered_paths) -> dict:
 
 
 def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node_score=None, truncated=False,
-              remaining_candidates=0, restores=None) -> dict:
+              remaining_candidates=0, restores=None, hosts=None) -> dict:
     """names: node id -> path (TemporalGraph.meta['names']); plan_nodes: node ids to revert, in plan order
     (PipelineResult.plan_nodes); scores: Plan.scores (exact reward after each commit, scores[0] = before).
     truncated / remaining_candidates: the planner stopped at its step limit while improving candidates remained --
     such a plan must not be auto-approved as complete.
     restores: PipelineResult.restores -- directory restores, each at its position in the plan ({"position", "dir",
-    "covers": node ids}); the node steps fill the other positions in order."""
+    "covers": node ids}); the node steps fill the other positions in order.
+    hosts: node id -> host name, for a graph of several sources: every step gets the "host" it applies to (a restore:
+    the host of the files it covers; covers on two hosts raise ValueError).  None: no host fields (one source)."""
+    host_of = (lambda n: check_host_name(hosts[int(n)])) if hosts is not None else None
     at = {int(r["position"]): r for r in (restores or [])}
     total = len(plan_nodes) + len(at)
     nodes = iter(plan_nodes)
@@ -70,6 +87,11 @@ def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node
         if k in at:
             r = at[k]
             step = {"order": k, **restore_dir_step(r["dir"], [names[int(c)] for c in r["covers"]])}
+            if host_of is not None and r["covers"]:
+                on = sorted({host_of(c) for c in r["covers"]})
+                if len(on) > 1:
+                    raise ValueError("restore of %r covers files on several hosts: %s" % (r["dir"], ", ".join(on)))
+                step["host"] = on[0]
             if scores is not None and k + 1 < len(scores):
                 step["reward_after"] = float(scores[k + 1])
             steps.append(step)
@@ -77,6 +99,8 @@ def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node
         n = int(next(nodes))
         step = {"order": k, "node": n, **reversion_for(names[n]),
                 "validate": {"check": "md5", "against": "pre_attack_snapshot"}}
+        if host_of is not None:
+            step["host"] = host_of(n)
         if size_mb is not None:
             step["size_mb"] = float(size_mb[n])
         if node_score is not None:
@@ -97,10 +121,20 @@ def to_json(plan: dict) -> str:
     return json.dumps(plan, indent=2, sort_keys=True)
 
 
-def to_shell(plan: dict) -> str:
-    """The same plan as the commands the M1 rollback script runs (m1_rollback.sh:95-99), for dry runs."""
+def plan_hosts(plan: dict) -> list:
+    """the hosts a plan of several sources has steps for, in order of first appearance ([] for a one-source plan)"""
+    return list(dict.fromkeys(check_host_name(s["host"]) for s in plan["steps"] if "host" in s))
+
+
+def to_shell(plan: dict, host=None) -> str:
+    """The same plan as the commands the M1 rollback script runs (m1_rollback.sh:95-99), for dry runs.  host: only that
+    host's steps (a plan of several sources runs one script per host)."""
     lines = ["#!/bin/sh", "set -e"]
+    if host is not None:
+        check_host_name(host)
     for s in plan["steps"]:
+        if host is not None and s.get("host") != host:
+            continue
         if s["op"] == "rename":
             lines.append("mv -- %s %s" % (shlex.quote(s["from"]), shlex.quote(s["to"])))
         elif s["op"] == "restore_snapshot_dir":
@@ -113,10 +147,12 @@ def to_shell(plan: dict) -> str:
     return "\n".join(lines) + "\n"
 
 
-def from_pipeline(g, result, attack_id=None) -> dict:
-    """g: TemporalGraph built from a trace; result: pipeline.PipelineResult."""
+def from_pipeline(g, result, attack_id=None, host_names=None) -> dict:
+    """g: TemporalGraph built from a trace; result: pipeline.PipelineResult.  host_names: source id -> host name for a
+    graph of several sources (g.meta["node_source"]); None: a one-source plan without host fields."""
     score = result.node_score.detach().cpu().numpy() if hasattr(result.node_score, "detach") else result.node_score
+    hosts = None if host_names is None else np.asarray(host_names, object)[np.asarray(g.meta["node_source"], np.int64)]
     return undo_plan(g.meta["names"], result.plan_nodes, scores=result.plan.scores, attack_id=attack_id,
                      size_mb=g.meta.get("size_mb"), node_score=score, truncated=getattr(result.plan, "truncated", False),
                      remaining_candidates=getattr(result.plan, "remaining_candidates", 0),
-                     restores=getattr(result, "restores", None))
+                     restores=getattr(result, "restores", None), hosts=hosts)

@@ -177,15 +177,18 @@ extern "C" int nerrf_trace_path_flags(const int64_t* off, const uint8_t* data, i
 // without its last extension), a non-empty new_path ALIASES its own key to that node (and names it when it ends in
 // .lockbit3) instead of making a node; else every distinct path is a node and a non-empty
 // new_path gets one too (node_g, -1 when absent).
-extern "C" int nerrf_trace_intern(int64_t n_events, const int64_t* order, const uint32_t* pid, const int64_t* path_off,
-                                  const uint8_t* path_data, const int64_t* new_path_off, const uint8_t* new_path_data,
-                                  int merge_renames, int32_t* node_p, int32_t* node_f, int32_t* node_g, int64_t* n_nodes,
-                                  int8_t* node_kind, int64_t* node_name_event, int8_t* node_name_which, int64_t node_capacity) {
+// source (NULL: every event from source 0): a process is (source, pid) and a file (source, merge key), so a rename target
+// aliases within its own source only.
+extern "C" int nerrf_trace_intern_ex(int64_t n_events, const int64_t* order, const uint32_t* pid, const uint16_t* source,
+                                     const int64_t* path_off, const uint8_t* path_data, const int64_t* new_path_off,
+                                     const uint8_t* new_path_data, int merge_renames, int32_t* node_p, int32_t* node_f,
+                                     int32_t* node_g, int64_t* n_nodes, int8_t* node_kind, int64_t* node_name_event,
+                                     int8_t* node_name_which, int64_t node_capacity) {
     NERRF_REQUIRE(n_events >= 0 && pid && path_off && new_path_off && node_p && node_f && node_g && n_nodes && node_kind &&
                       node_name_event && node_name_which,
                   "null pointer");
     NERRF_REQUIRE(n_events < ((int64_t)1 << 30), "too many events for 32-bit node ids");
-    std::unordered_map<uint32_t, int32_t> pids;
+    std::unordered_map<uint64_t, int32_t> pids;
     std::unordered_map<std::string, int32_t> files;
     pids.reserve((size_t)n_events / 8 + 16);
     files.reserve((size_t)n_events / 2 + 16);
@@ -196,19 +199,24 @@ extern "C" int nerrf_trace_intern(int64_t n_events, const int64_t* order, const 
         return (int32_t)nn++;
     };
     std::string key;
+    char sk[2] = {0, 0};                                                 // the source id, appended to every file key
+    auto set_key = [&](const uint8_t* s, uint64_t n) { key.assign((const char*)s, n); key.append(sk, 2); };
     for (int64_t k = 0; k < n_events; ++k) {
         const int64_t i = order ? order[k] : k;
         NERRF_REQUIRE(i >= 0 && i < n_events, "order[%lld]=%lld out of range", (long long)k, (long long)i);
-        auto pit = pids.find(pid[i]);
+        const uint16_t src = source ? source[i] : (uint16_t)0;
+        sk[0] = (char)(src & 0xff); sk[1] = (char)(src >> 8);
+        const uint64_t pkey = ((uint64_t)src << 32) | pid[i];
+        auto pit = pids.find(pkey);
         if (pit == pids.end()) {
             const int32_t id = new_node(1, i, 2);
             NERRF_REQUIRE(id >= 0, "node_capacity=%lld too small", (long long)node_capacity);
-            pit = pids.emplace(pid[i], id).first;
+            pit = pids.emplace(pkey, id).first;
         }
         node_p[i] = pit->second;
         const uint8_t* s = path_data + path_off[i];
         const uint64_t n = (uint64_t)(path_off[i + 1] - path_off[i]);
-        key.assign((const char*)s, merge_renames ? stem_len(s, n) : n);
+        set_key(s, merge_renames ? stem_len(s, n) : n);
         auto fit = files.find(key);
         if (fit == files.end()) {
             const int32_t id = new_node(0, i, 0);
@@ -223,12 +231,12 @@ extern "C" int nerrf_trace_intern(int64_t n_events, const int64_t* order, const 
             // a real rename `a.dat -> a.dat.lockbit3`: the target is the same file identity whatever its stem (merge by
             // inode); later events on the new name land on this node, and an encrypted target names the rollback
             const uint8_t* g = new_path_data + new_path_off[i];
-            key.assign((const char*)g, stem_len(g, gn));
+            set_key(g, stem_len(g, gn));
             files.emplace(key, fit->second);                              // no-op when the key is already known
             if (wire::ends_with(g, gn, ".lockbit3", 9)) { node_name_event[fit->second] = i; node_name_which[fit->second] = 1; }
         }
         if (gn && !merge_renames) {
-            key.assign((const char*)(new_path_data + new_path_off[i]), gn);
+            set_key(new_path_data + new_path_off[i], gn);
             auto git = files.find(key);
             if (git == files.end()) {
                 const int32_t id = new_node(0, i, 1);
@@ -240,4 +248,12 @@ extern "C" int nerrf_trace_intern(int64_t n_events, const int64_t* order, const 
     }
     *n_nodes = nn;
     return NERRF_OK;
+}
+
+extern "C" int nerrf_trace_intern(int64_t n_events, const int64_t* order, const uint32_t* pid, const int64_t* path_off,
+                                  const uint8_t* path_data, const int64_t* new_path_off, const uint8_t* new_path_data,
+                                  int merge_renames, int32_t* node_p, int32_t* node_f, int32_t* node_g, int64_t* n_nodes,
+                                  int8_t* node_kind, int64_t* node_name_event, int8_t* node_name_which, int64_t node_capacity) {
+    return nerrf_trace_intern_ex(n_events, order, pid, nullptr, path_off, path_data, new_path_off, new_path_data, merge_renames,
+                                 node_p, node_f, node_g, n_nodes, node_kind, node_name_event, node_name_which, node_capacity);
 }

@@ -35,6 +35,10 @@ __device__ __forceinline__ uint64_t hash_bytes(const uint8_t* __restrict__ s, in
     for (int64_t i = 0; i < n; ++i) { h ^= s[i]; h *= FNV_PRIME; }
     return mix64(h);
 }
+// source-qualified key and name hashes: the identity at source 0, so a single-source stream hashes as it always did
+__device__ __forceinline__ uint64_t qualify(uint64_t h, uint32_t s) { return s ? mix64(h + (uint64_t)s * 0x9E3779B97F4A7C15ull) : h; }
+__device__ __forceinline__ uint64_t pid_hash(uint32_t pid, uint32_t s) { return mix64((((uint64_t)s << 32) | pid) + 0x9E3779B97F4A7C15ull); }
+__device__ __forceinline__ uint32_t source_at(const uint16_t* __restrict__ source, int64_t i) { return source ? source[i] : 0u; }
 // csrc/ingest.cu stem_len: the path without its last extension (graph.py _stem)
 __device__ __forceinline__ int64_t stem_len_dev(const uint8_t* __restrict__ s, int64_t n) {
     int64_t slash = -1, dot = -1;
@@ -72,6 +76,7 @@ struct InternArgs {
     int64_t n_total;                       // events stored (the columns' length): order[] indexes into [0, n_total)
     const int64_t* order;                  // processing order: rank k handles stored event order[k] (NULL: identity)
     const uint32_t* pid;
+    const uint16_t* source;                // NULL: every event from source 0
     const int64_t *path_off, *gpath_off;
     const uint8_t *path_data, *gpath_data;
     int merge;
@@ -95,15 +100,16 @@ __global__ void __launch_bounds__(256) intern_hash_kernel(InternArgs a) {
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < a.n; k += stride) {
         const int64_t i = stored(a, k);
         if (i < 0 || i >= a.n_total) { *a.err = 4; a.slot_p[k] = a.slot_f[k] = 0; a.slot_g[k] = -1; continue; }
-        const int32_t sp = table_insert(a.pids, mix64((uint64_t)a.pid[i] + 0x9E3779B97F4A7C15ull), (int32_t)k);
+        const uint32_t src = source_at(a.source, i);
+        const int32_t sp = table_insert(a.pids, pid_hash(a.pid[i], src), (int32_t)k);
         const uint8_t* s = a.path_data + a.path_off[i];
         const int64_t n = a.path_off[i + 1] - a.path_off[i];
-        const int32_t sf = table_insert(a.files, hash_bytes(s, a.merge ? stem_len_dev(s, n) : n), (int32_t)(2 * k));
+        const int32_t sf = table_insert(a.files, qualify(hash_bytes(s, a.merge ? stem_len_dev(s, n) : n), src), (int32_t)(2 * k));
         int32_t sg = -1;
         const int64_t gn = a.gpath_off[i + 1] - a.gpath_off[i];
         if (gn > 0) {
             const uint8_t* g = a.gpath_data + a.gpath_off[i];
-            sg = table_insert(a.files, hash_bytes(g, a.merge ? stem_len_dev(g, gn) : gn), (int32_t)(2 * k + 1));
+            sg = table_insert(a.files, qualify(hash_bytes(g, a.merge ? stem_len_dev(g, gn) : gn), src), (int32_t)(2 * k + 1));
             if (sg < 0) *a.err = 1;
         }
         if (sp < 0 || sf < 0) *a.err = 1;
@@ -126,7 +132,7 @@ __device__ __forceinline__ void verify_mention(const InternArgs& a, int32_t slot
     int64_t n0, n1;
     const uint8_t* s0 = mention_key(a, f, &n0);
     const uint8_t* s1 = mention_key(a, m, &n1);
-    bool same = n0 == n1;
+    bool same = n0 == n1 && source_at(a.source, stored(a, f >> 1)) == source_at(a.source, stored(a, m >> 1));
     for (int64_t k = 0; same && k < n0; ++k) same = s0[k] == s1[k];
     if (!same) *a.err = 2;
 }
@@ -135,7 +141,9 @@ __global__ void __launch_bounds__(256) intern_verify_kernel(InternArgs a) {
     if (*a.err) return;
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < a.n; k += stride) {
         const int32_t pf = a.pids.first[a.slot_p[k]];
-        if (pf != (int32_t)k && a.pid[stored(a, pf)] != a.pid[stored(a, k)]) *a.err = 2;
+        if (pf != (int32_t)k && (a.pid[stored(a, pf)] != a.pid[stored(a, k)] ||
+                                 source_at(a.source, stored(a, pf)) != source_at(a.source, stored(a, k))))
+            *a.err = 2;
         verify_mention(a, a.slot_f[k], (int32_t)(2 * k));
         if (a.slot_g[k] >= 0) verify_mention(a, a.slot_g[k], (int32_t)(2 * k + 1));
     }
@@ -213,17 +221,18 @@ __global__ void __launch_bounds__(256) intern_names_kernel(InternArgs a, const i
 // to the host.  Same function as nerrf_b200/ingest.py name_hash.
 __global__ void __launch_bounds__(256) name_hash_kernel(int64_t n_nodes, const int64_t* __restrict__ name_event,
                                                         const int8_t* __restrict__ name_which, const uint32_t* __restrict__ pid,
-                                                        const int64_t* __restrict__ path_off, const uint8_t* __restrict__ path_data,
+                                                        const uint16_t* __restrict__ source, const int64_t* __restrict__ path_off, const uint8_t* __restrict__ path_data,
                                                         const int64_t* __restrict__ gpath_off, const uint8_t* __restrict__ gpath_data,
                                                         unsigned long long* __restrict__ out) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < n_nodes; v += stride) {
         const int64_t e = name_event[v];
         const int w = name_which[v];
+        const uint32_t src = source_at(source, e);
         unsigned long long h;
-        if (w == 2) h = mix64((uint64_t)pid[e] + 0x9E3779B97F4A7C15ull);
-        else if (w == 1) h = hash_bytes(gpath_data + gpath_off[e], gpath_off[e + 1] - gpath_off[e]);
-        else h = hash_bytes(path_data + path_off[e], path_off[e + 1] - path_off[e]);
+        if (w == 2) h = pid_hash(pid[e], src);
+        else if (w == 1) h = qualify(hash_bytes(gpath_data + gpath_off[e], gpath_off[e + 1] - gpath_off[e]), src);
+        else h = qualify(hash_bytes(path_data + path_off[e], path_off[e + 1] - path_off[e]), src);
         out[v] = h;
     }
 }
@@ -238,20 +247,21 @@ __device__ __forceinline__ int64_t dir_len_dev(const uint8_t* __restrict__ s, in
 }
 __global__ void __launch_bounds__(256) dir_hash_kernel(int64_t n_nodes, const int64_t* __restrict__ name_event,
                                                        const int8_t* __restrict__ name_which, const uint32_t* __restrict__ pid,
-                                                       const int64_t* __restrict__ path_off, const uint8_t* __restrict__ path_data,
+                                                       const uint16_t* __restrict__ source, const int64_t* __restrict__ path_off, const uint8_t* __restrict__ path_data,
                                                        const int64_t* __restrict__ gpath_off, const uint8_t* __restrict__ gpath_data,
                                                        unsigned long long* __restrict__ out) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t v = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; v < n_nodes; v += stride) {
         const int64_t e = name_event[v];
         const int w = name_which[v];
+        const uint32_t src = source_at(source, e);
         unsigned long long h;
         if (w == 2) {
-            h = mix64((uint64_t)pid[e] + 0x9E3779B97F4A7C15ull);
+            h = pid_hash(pid[e], src);
         } else {
             const uint8_t* s = w == 1 ? gpath_data + gpath_off[e] : path_data + path_off[e];
             const int64_t n = w == 1 ? gpath_off[e + 1] - gpath_off[e] : path_off[e + 1] - path_off[e];
-            h = hash_bytes(s, dir_len_dev(s, n));
+            h = qualify(hash_bytes(s, dir_len_dev(s, n)), src);
         }
         out[v] = h;
     }
@@ -298,11 +308,12 @@ extern "C" int nerrf_trace_intern_device_workspace_bytes(int64_t n_events, int64
     return NERRF_OK;
 }
 
-extern "C" int nerrf_trace_intern_device(int64_t n_events, int64_t n_stored, const int64_t* order, const uint32_t* pid, const int64_t* path_off, const uint8_t* path_data,
-                                         const int64_t* new_path_off, const uint8_t* new_path_data, int merge_renames,
-                                         int32_t* node_p, int32_t* node_f, int32_t* node_g, int64_t* n_nodes, int8_t* node_kind,
-                                         int64_t* node_name_event, int8_t* node_name_which, int64_t node_capacity,
-                                         void* workspace, int64_t workspace_bytes, void* stream) {
+extern "C" int nerrf_trace_intern_device_ex(int64_t n_events, int64_t n_stored, const int64_t* order, const uint32_t* pid,
+                                            const uint16_t* source, const int64_t* path_off, const uint8_t* path_data,
+                                            const int64_t* new_path_off, const uint8_t* new_path_data, int merge_renames,
+                                            int32_t* node_p, int32_t* node_f, int32_t* node_g, int64_t* n_nodes, int8_t* node_kind,
+                                            int64_t* node_name_event, int8_t* node_name_which, int64_t node_capacity,
+                                            void* workspace, int64_t workspace_bytes, void* stream) {
     NERRF_REQUIRE(n_nodes, "null n_nodes");
     *n_nodes = 0;
     if (n_events == 0) return NERRF_OK;
@@ -318,7 +329,7 @@ extern "C" int nerrf_trace_intern_device(int64_t n_events, int64_t n_stored, con
     cudaStream_t st = (cudaStream_t)stream;
     char* ws = (char*)workspace;
     InternArgs a;
-    a.n = n_events; a.n_total = n_stored; a.order = order; a.pid = pid; a.path_off = path_off; a.gpath_off = new_path_off; a.path_data = path_data; a.gpath_data = new_path_data;
+    a.n = n_events; a.n_total = n_stored; a.order = order; a.pid = pid; a.source = source; a.path_off = path_off; a.gpath_off = new_path_off; a.path_data = path_data; a.gpath_data = new_path_data;
     a.merge = merge_renames ? 1 : 0;
     a.files.key = (unsigned long long*)(ws + L.fkey); a.files.first = (int32_t*)(ws + L.ffirst); a.files.mask = L.fcap - 1;
     a.pids.key = (unsigned long long*)(ws + L.pkey); a.pids.first = (int32_t*)(ws + L.pfirst); a.pids.mask = L.pcap - 1;
@@ -356,26 +367,50 @@ extern "C" int nerrf_trace_intern_device(int64_t n_events, int64_t n_stored, con
     return NERRF_OK;
 }
 
-extern "C" int nerrf_trace_name_hash(int64_t n_nodes, const int64_t* node_name_event, const int8_t* node_name_which,
-                                     const uint32_t* pid, const int64_t* path_off, const uint8_t* path_data,
-                                     const int64_t* new_path_off, const uint8_t* new_path_data, uint64_t* hash_out, void* stream) {
+extern "C" int nerrf_trace_intern_device(int64_t n_events, int64_t n_stored, const int64_t* order, const uint32_t* pid, const int64_t* path_off, const uint8_t* path_data,
+                                         const int64_t* new_path_off, const uint8_t* new_path_data, int merge_renames,
+                                         int32_t* node_p, int32_t* node_f, int32_t* node_g, int64_t* n_nodes, int8_t* node_kind,
+                                         int64_t* node_name_event, int8_t* node_name_which, int64_t node_capacity,
+                                         void* workspace, int64_t workspace_bytes, void* stream) {
+    return nerrf_trace_intern_device_ex(n_events, n_stored, order, pid, nullptr, path_off, path_data, new_path_off, new_path_data,
+                                        merge_renames, node_p, node_f, node_g, n_nodes, node_kind, node_name_event, node_name_which,
+                                        node_capacity, workspace, workspace_bytes, stream);
+}
+
+extern "C" int nerrf_trace_name_hash_ex(int64_t n_nodes, const int64_t* node_name_event, const int8_t* node_name_which,
+                                        const uint32_t* pid, const uint16_t* source, const int64_t* path_off, const uint8_t* path_data,
+                                        const int64_t* new_path_off, const uint8_t* new_path_data, uint64_t* hash_out, void* stream) {
     NERRF_REQUIRE(n_nodes >= 0, "negative node count");
     if (n_nodes == 0) return NERRF_OK;
     NERRF_REQUIRE(node_name_event && node_name_which && pid && path_off && path_data && new_path_off && new_path_data && hash_out,
                   "null pointer");
-    name_hash_kernel<<<sm_count() * 8, 256, 0, (cudaStream_t)stream>>>(n_nodes, node_name_event, node_name_which, pid, path_off, path_data,
-                                                                        new_path_off, new_path_data, (unsigned long long*)hash_out);
+    name_hash_kernel<<<sm_count() * 8, 256, 0, (cudaStream_t)stream>>>(n_nodes, node_name_event, node_name_which, pid, source, path_off,
+                                                                        path_data, new_path_off, new_path_data, (unsigned long long*)hash_out);
     return launch_status("name_hash_kernel");
+}
+
+extern "C" int nerrf_trace_name_hash(int64_t n_nodes, const int64_t* node_name_event, const int8_t* node_name_which,
+                                     const uint32_t* pid, const int64_t* path_off, const uint8_t* path_data,
+                                     const int64_t* new_path_off, const uint8_t* new_path_data, uint64_t* hash_out, void* stream) {
+    return nerrf_trace_name_hash_ex(n_nodes, node_name_event, node_name_which, pid, nullptr, path_off, path_data, new_path_off,
+                                    new_path_data, hash_out, stream);
+}
+
+extern "C" int nerrf_trace_dir_hash_ex(int64_t n_nodes, const int64_t* node_name_event, const int8_t* node_name_which,
+                                       const uint32_t* pid, const uint16_t* source, const int64_t* path_off, const uint8_t* path_data,
+                                       const int64_t* new_path_off, const uint8_t* new_path_data, uint64_t* hash_out, void* stream) {
+    NERRF_REQUIRE(n_nodes >= 0, "negative node count");
+    if (n_nodes == 0) return NERRF_OK;
+    NERRF_REQUIRE(node_name_event && node_name_which && pid && path_off && path_data && new_path_off && new_path_data && hash_out,
+                  "null pointer");
+    dir_hash_kernel<<<sm_count() * 8, 256, 0, (cudaStream_t)stream>>>(n_nodes, node_name_event, node_name_which, pid, source, path_off,
+                                                                       path_data, new_path_off, new_path_data, (unsigned long long*)hash_out);
+    return launch_status("dir_hash_kernel");
 }
 
 extern "C" int nerrf_trace_dir_hash(int64_t n_nodes, const int64_t* node_name_event, const int8_t* node_name_which,
                                     const uint32_t* pid, const int64_t* path_off, const uint8_t* path_data,
                                     const int64_t* new_path_off, const uint8_t* new_path_data, uint64_t* hash_out, void* stream) {
-    NERRF_REQUIRE(n_nodes >= 0, "negative node count");
-    if (n_nodes == 0) return NERRF_OK;
-    NERRF_REQUIRE(node_name_event && node_name_which && pid && path_off && path_data && new_path_off && new_path_data && hash_out,
-                  "null pointer");
-    dir_hash_kernel<<<sm_count() * 8, 256, 0, (cudaStream_t)stream>>>(n_nodes, node_name_event, node_name_which, pid, path_off, path_data,
-                                                                       new_path_off, new_path_data, (unsigned long long*)hash_out);
-    return launch_status("dir_hash_kernel");
+    return nerrf_trace_dir_hash_ex(n_nodes, node_name_event, node_name_which, pid, nullptr, path_off, path_data, new_path_off,
+                                   new_path_data, hash_out, stream);
 }

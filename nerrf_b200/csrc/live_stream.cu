@@ -8,8 +8,9 @@
 //                               offsets; one warp per record copies the bytes and computes path_flags over them.  A
 //                               malformed record does an atomicMin of its byte offset into the status word.
 //   nerrf_trace_stream_order    stable time order (LSD radix sort of the orderable float64 bits, radix_sort.cuh); the
-//                               columnar resolve_columns of nerrf_b200/ingest.py: a stable regroup by pid (radix sort of
-//                               the pid over the time order), then a segmented "last event with a path so far" max-scan
+//                               columnar resolve_columns of nerrf_b200/ingest.py: a stable regroup by (source, pid) (radix
+//                               sort of the pid, or of (source << 32) | pid in 6 digit passes instead of 4 when some
+//                               source is nonzero, over the time order), then a segmented "last event with a path so far" max-scan
 //                               gives the source event of every path-less write, or drops it; the survivors' time order;
 //                               the resolved path offsets; and the rows to keep at a retention horizon.
 //   nerrf_trace_stream_columns  the resolved path column (warp per event) and the per-event flags / slots the window
@@ -95,6 +96,7 @@ struct Cols {
     int64_t* ts_sec; int32_t* ts_nanos; uint32_t* pid; uint32_t* tid; int32_t* flags; int64_t* ret_val; uint64_t* bytes;
     uint8_t* event_slot; uint8_t* path_flags;
     int64_t* off[4]; uint8_t* data[4];
+    uint16_t* source;            // source id per row (not one of the 17; NULL = not stored)
 };
 Cols make_cols(void* const* p) {
     Cols c;
@@ -102,6 +104,7 @@ Cols make_cols(void* const* p) {
     c.flags = (int32_t*)p[4]; c.ret_val = (int64_t*)p[5]; c.bytes = (uint64_t*)p[6]; c.event_slot = (uint8_t*)p[7];
     c.path_flags = (uint8_t*)p[8];
     for (int k = 0; k < 4; ++k) { c.off[k] = (int64_t*)p[9 + 2 * k]; c.data[k] = (uint8_t*)p[10 + 2 * k]; }
+    c.source = nullptr;
     return c;
 }
 bool cols_ok(void* const* p) {
@@ -113,7 +116,7 @@ bool cols_ok(void* const* p) {
 // ---- decode: thread per record
 __global__ void __launch_bounds__(256) decode_records_kernel(const uint8_t* __restrict__ buf, const int64_t* __restrict__ rec_at,
                                                              const int64_t* __restrict__ body_off, const int64_t* __restrict__ body_len,
-                                                             int64_t m, int64_t n_old, Cols c, int64_t* __restrict__ start,
+                                                             int64_t m, int64_t n_old, Cols c, uint16_t source, int64_t* __restrict__ start,
                                                              int32_t* __restrict__ len, unsigned long long* __restrict__ status) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < m; k += stride) {
@@ -127,6 +130,7 @@ __global__ void __launch_bounds__(256) decode_records_kernel(const uint8_t* __re
         const int64_t row = n_old + k;
         c.ts_sec[row] = e.ts_sec; c.ts_nanos[row] = e.ts_nanos; c.pid[row] = e.pid; c.tid[row] = e.tid; c.flags[row] = e.flags;
         c.ret_val[row] = e.ret_val; c.bytes[row] = e.bytes;
+        if (c.source) c.source[row] = source;
         c.event_slot[row] = (uint8_t)wire::event_slot(e.syscall, e.syscall_n);
         const uint8_t* str[4] = {e.comm, e.syscall, e.path, e.new_path};
         const uint64_t sn[4] = {e.comm_n, e.syscall_n, e.path_n, e.new_path_n};
@@ -201,6 +205,7 @@ __global__ void __launch_bounds__(256) gather_scalars_kernel(Cols in, const int6
         out.ts_sec[k] = in.ts_sec[r]; out.ts_nanos[k] = in.ts_nanos[r]; out.pid[k] = in.pid[r]; out.tid[k] = in.tid[r];
         out.flags[k] = in.flags[r]; out.ret_val[k] = in.ret_val[r]; out.bytes[k] = in.bytes[r];
         out.event_slot[k] = in.event_slot[r]; out.path_flags[k] = in.path_flags[r];
+        if (out.source) out.source[k] = in.source ? in.source[r] : (uint16_t)0;
 #pragma unroll
         for (int q = 0; q < 4; ++q) { start[q * m + k] = in.off[q][r]; len[q * m + k] = (int32_t)(in.off[q][r + 1] - in.off[q][r]); }
     }
@@ -210,6 +215,8 @@ __global__ void __launch_bounds__(256) gather_scalars_kernel(Cols in, const int6
 struct OrderArgs {
     int64_t n;
     const int64_t* ts_sec; const int32_t* ts_nanos; const uint32_t* pid; const int64_t* path_off;
+    const uint16_t* source;      // [n] source id per event, read only when key_bits == 48 (NULL: all 0)
+    int key_bits;                // 32: regroup by pid; 48: by (source << 32) | pid
     double horizon;
     double* ts;                  // [n] float64 timestamps by stored index
     uint32_t* tord;              // [n] stored index by time rank
@@ -238,13 +245,13 @@ __global__ void __launch_bounds__(256) order_keys_kernel(OrderArgs a, uint64_t* 
         a.R[i] = t > a.horizon ? 1 : 0;
     }
 }
-// time rank k: remember the time order, key the pid for the stable regroup (in place: same index read and written)
+// time rank k: remember the time order, key the (source, pid) for the stable regroup (in place: same index read and written)
 __global__ void __launch_bounds__(256) order_pid_keys_kernel(OrderArgs a, uint64_t* __restrict__ key, uint32_t* __restrict__ val) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < a.n; k += stride) {
         const uint32_t e = val[k];
         a.tord[k] = e;
-        key[k] = a.pid[e];
+        key[k] = (a.key_bits > 32 && a.source) ? ((uint64_t)a.source[e] << 32) | a.pid[e] : (uint64_t)a.pid[e];
         val[k] = (uint32_t)k;
     }
 }
@@ -267,7 +274,7 @@ __global__ void __launch_bounds__(256) order_resolve_kernel(OrderArgs a) {
         const int32_t g = a.G[j];
         a.src[e] = a.A[j] >= g ? (int64_t)a.byp[a.A[j]] : -1;
         const bool last = j + 1 == a.n || a.G[j + 1] != g;
-        if (last && a.C[j] >= g) a.R[a.byp[a.C[j]]] = 1;                   // the pid's latest named event at the horizon
+        if (last && a.C[j] >= g) a.R[a.byp[a.C[j]]] = 1;                   // the (source, pid)'s latest named event at the horizon
     }
 }
 __global__ void __launch_bounds__(256) order_flags_kernel(OrderArgs a) {
@@ -368,11 +375,12 @@ extern "C" int nerrf_trace_decode_device_workspace_bytes(int64_t n_records, int6
     return NERRF_OK;
 }
 
-extern "C" int nerrf_trace_decode_device(const uint8_t* buf, const int64_t* rec_at, const int64_t* body_off, const int64_t* body_len,
-                                         int64_t n_records, int64_t n_old, void* const* cols, uint64_t* status, void* workspace,
-                                         int64_t workspace_bytes, void* stream) {
+extern "C" int nerrf_trace_decode_device_ex(const uint8_t* buf, const int64_t* rec_at, const int64_t* body_off, const int64_t* body_len,
+                                            int64_t n_records, int64_t n_old, void* const* cols, uint16_t* source_col, int source,
+                                            uint64_t* status, void* workspace, int64_t workspace_bytes, void* stream) {
     NERRF_REQUIRE(status, "null status");
     NERRF_REQUIRE(n_records >= 0 && n_records < ((int64_t)1 << 28) && n_old >= 0, "bad record count");
+    NERRF_REQUIRE(source >= 0 && source < (1 << 16), "source=%d out of range [0, 65536)", source);
     cudaStream_t st = (cudaStream_t)stream;
     NERRF_CHECK_CUDA(cudaMemsetAsync(status, 0xff, 8, st));                  // all ones: no record failed
     if (n_records == 0) return NERRF_OK;
@@ -383,17 +391,25 @@ extern "C" int nerrf_trace_decode_device(const uint8_t* buf, const int64_t* rec_
                   (long long)L.bytes);
     NERRF_REQUIRE(((uintptr_t)workspace & 255) == 0, "workspace must be 256-byte aligned");
     char* ws = (char*)workspace;
-    const Cols c = make_cols(cols);
+    Cols c = make_cols(cols);
+    c.source = source_col;
     int64_t* start = (int64_t*)(ws + L.start);
     int32_t* scan = (int32_t*)(ws + L.scan);
     int32_t* total = (int32_t*)(ws + L.total);
-    decode_records_kernel<<<grid_for(n_records, 256), 256, 0, st>>>(buf, rec_at, body_off, body_len, n_records, n_old, c, start, scan,
-                                                                     (unsigned long long*)status);
+    decode_records_kernel<<<grid_for(n_records, 256), 256, 0, st>>>(buf, rec_at, body_off, body_len, n_records, n_old, c,
+                                                                     (uint16_t)source, start, scan, (unsigned long long*)status);
     exclusive_scan_i32(scan, 4 * n_records, (int32_t*)(ws + L.sums), total, st);
     StrSrc s;
     for (int q = 0; q < 4; ++q) s.base[q] = buf;
     copy_strings_kernel<<<grid_for(n_records, 8), 256, 0, st>>>(s, start, scan, total, n_records, n_old, c, c.path_flags);
     return launch_status("device decoder kernels");
+}
+
+extern "C" int nerrf_trace_decode_device(const uint8_t* buf, const int64_t* rec_at, const int64_t* body_off, const int64_t* body_len,
+                                         int64_t n_records, int64_t n_old, void* const* cols, uint64_t* status, void* workspace,
+                                         int64_t workspace_bytes, void* stream) {
+    return nerrf_trace_decode_device_ex(buf, rec_at, body_off, body_len, n_records, n_old, cols, nullptr, 0, status, workspace,
+                                        workspace_bytes, stream);
 }
 
 extern "C" int nerrf_trace_stream_order_workspace_bytes(int64_t n_events, int64_t* bytes) {
@@ -402,12 +418,14 @@ extern "C" int nerrf_trace_stream_order_workspace_bytes(int64_t n_events, int64_
     return NERRF_OK;
 }
 
-extern "C" int nerrf_trace_stream_order(int64_t n_events, const int64_t* ts_sec, const int32_t* ts_nanos, const uint32_t* pid,
-                                        const int64_t* path_off, double horizon, double* ts_out, int64_t* order_out,
-                                        double* ts_sorted_out, int64_t* src_out, int64_t* res_path_off, int64_t* retain_out,
-                                        int64_t* counts, void* workspace, int64_t workspace_bytes, void* stream) {
+extern "C" int nerrf_trace_stream_order_ex(int64_t n_events, const int64_t* ts_sec, const int32_t* ts_nanos, const uint32_t* pid,
+                                           const uint16_t* source, int key_bits, const int64_t* path_off, double horizon,
+                                           double* ts_out, int64_t* order_out, double* ts_sorted_out, int64_t* src_out,
+                                           int64_t* res_path_off, int64_t* retain_out, int64_t* counts, void* workspace,
+                                           int64_t workspace_bytes, void* stream) {
     NERRF_REQUIRE(counts, "null counts");
     counts[0] = counts[1] = counts[2] = 0;
+    NERRF_REQUIRE(key_bits == 32 || (key_bits == 48 && source), "key_bits=%d: 32, or 48 with a source column", key_bits);
     NERRF_REQUIRE(n_events >= 0 && n_events < ((int64_t)1 << 30), "n_events=%lld out of range", (long long)n_events);
     if (n_events == 0) return NERRF_OK;
     NERRF_REQUIRE(ts_sec && ts_nanos && pid && path_off && ts_out && order_out && ts_sorted_out && src_out && res_path_off && workspace,
@@ -420,6 +438,7 @@ extern "C" int nerrf_trace_stream_order(int64_t n_events, const int64_t* ts_sec,
     char* ws = (char*)workspace;
     OrderArgs a;
     a.n = n_events; a.ts_sec = ts_sec; a.ts_nanos = ts_nanos; a.pid = pid; a.path_off = path_off; a.horizon = horizon;
+    a.source = source; a.key_bits = key_bits;
     a.ts = ts_out; a.tord = (uint32_t*)(ws + L.tord); a.byp = (uint32_t*)(ws + L.byp);
     a.A = (int32_t*)(ws + L.A); a.G = (int32_t*)(ws + L.G); a.C = (int32_t*)(ws + L.C);
     a.F = (int32_t*)(ws + L.F); a.R = (int32_t*)(ws + L.R); a.L = (int32_t*)(ws + L.L); a.src = src_out;
@@ -432,7 +451,7 @@ extern "C" int nerrf_trace_stream_order(int64_t n_events, const int64_t* ts_sec,
     order_keys_kernel<<<grid, 256, 0, st>>>(a, ka, va);
     if (radix_sort_pairs(ka, kb, va, vb, n_events, 0, 64, ws + L.rs, st)) { uint64_t* t = ka; ka = kb; kb = t; uint32_t* u = va; va = vb; vb = u; }
     order_pid_keys_kernel<<<grid, 256, 0, st>>>(a, ka, va);
-    if (radix_sort_pairs(ka, kb, va, vb, n_events, 0, 32, ws + L.rs, st)) { uint64_t* t = ka; ka = kb; kb = t; uint32_t* u = va; va = vb; vb = u; }
+    if (radix_sort_pairs(ka, kb, va, vb, n_events, 0, key_bits, ws + L.rs, st)) { uint64_t* t = ka; ka = kb; kb = t; uint32_t* u = va; va = vb; vb = u; }
     order_segments_kernel<<<grid, 256, 0, st>>>(a, ka, va);
     inclusive_max_scan_i32(a.A, n_events, sums, st);
     inclusive_max_scan_i32(a.G, n_events, sums, st);
@@ -456,6 +475,14 @@ extern "C" int nerrf_trace_stream_order(int64_t n_events, const int64_t* ts_sec,
     return NERRF_OK;
 }
 
+extern "C" int nerrf_trace_stream_order(int64_t n_events, const int64_t* ts_sec, const int32_t* ts_nanos, const uint32_t* pid,
+                                        const int64_t* path_off, double horizon, double* ts_out, int64_t* order_out,
+                                        double* ts_sorted_out, int64_t* src_out, int64_t* res_path_off, int64_t* retain_out,
+                                        int64_t* counts, void* workspace, int64_t workspace_bytes, void* stream) {
+    return nerrf_trace_stream_order_ex(n_events, ts_sec, ts_nanos, pid, nullptr, 32, path_off, horizon, ts_out, order_out,
+                                       ts_sorted_out, src_out, res_path_off, retain_out, counts, workspace, workspace_bytes, stream);
+}
+
 extern "C" int nerrf_trace_stream_columns(int64_t n_events, const int64_t* src, const int64_t* path_off, const uint8_t* path_data,
                                           const uint8_t* path_flags, const int64_t* new_path_off, const uint8_t* new_path_data,
                                           const uint8_t* event_slot, const uint8_t* slot_map, const int64_t* res_path_off,
@@ -476,12 +503,14 @@ extern "C" int nerrf_trace_gather_rows_workspace_bytes(int64_t n_rows, int64_t* 
     return nerrf_trace_decode_device_workspace_bytes(n_rows, bytes);
 }
 
-extern "C" int nerrf_trace_gather_rows(void* const* cols_in, const int64_t* rows, int64_t n_rows, void* const* cols_out,
-                                       void* workspace, int64_t workspace_bytes, void* stream) {
+extern "C" int nerrf_trace_gather_rows_ex(void* const* cols_in, const uint16_t* source_in, const int64_t* rows, int64_t n_rows,
+                                          void* const* cols_out, uint16_t* source_out, void* workspace, int64_t workspace_bytes,
+                                          void* stream) {
     NERRF_REQUIRE(n_rows >= 0 && n_rows < ((int64_t)1 << 28), "bad row count");
     NERRF_REQUIRE(cols_ok(cols_in) && cols_ok(cols_out), "null column pointer");
     cudaStream_t st = (cudaStream_t)stream;
-    const Cols in = make_cols(cols_in), out = make_cols(cols_out);
+    Cols in = make_cols(cols_in), out = make_cols(cols_out);
+    in.source = (uint16_t*)source_in; out.source = source_out;
     for (int q = 0; q < 4; ++q) NERRF_CHECK_CUDA(cudaMemsetAsync(out.off[q], 0, 8, st));
     if (n_rows == 0) return NERRF_OK;
     NERRF_REQUIRE(rows && workspace, "null pointer");
@@ -499,4 +528,9 @@ extern "C" int nerrf_trace_gather_rows(void* const* cols_in, const int64_t* rows
     for (int q = 0; q < 4; ++q) s.base[q] = in.data[q];
     copy_strings_kernel<<<grid_for(n_rows, 8), 256, 0, st>>>(s, start, scan, total, n_rows, 0, out, nullptr);
     return launch_status("gather kernels");
+}
+
+extern "C" int nerrf_trace_gather_rows(void* const* cols_in, const int64_t* rows, int64_t n_rows, void* const* cols_out,
+                                       void* workspace, int64_t workspace_bytes, void* stream) {
+    return nerrf_trace_gather_rows_ex(cols_in, nullptr, rows, n_rows, cols_out, nullptr, workspace, workspace_bytes, stream);
 }

@@ -35,6 +35,7 @@ class EventColumns:
     event_slot: np.ndarray    # uint8  [n]   feature slot of the syscall / event name (graph._EVENT_SLOT, 7 = other)
     path_flags: np.ndarray    # uint8  [n]   NERRF_PATH_* bits
     strings: dict             # name -> (offsets int64 [n+1], data uint8 [bytes])
+    source: np.ndarray = None  # uint16 [n] source id of each event (the host whose tracker sent it); None = all source 0
 
     def text(self, column: str, i: int) -> str:
         off, data = self.strings[column]
@@ -124,17 +125,26 @@ def _gather_strings(off, data, idx):
     return new_off, data[pos]
 
 
+def process_keys(cols: EventColumns) -> np.ndarray:
+    """uint64 [n] process identity of every event: (source << 32) | pid (the pid alone without a source column)"""
+    key = cols.pid.astype(np.uint64)
+    if cols.source is not None:
+        key |= cols.source.astype(np.uint64) << np.uint64(32)
+    return key
+
+
 def resolve_columns(cols: EventColumns) -> EventColumns:
     """Columnar form of graph.resolve_event_paths: every event must name a file.  The tracker zeroes `path` on write
-    events (tracker/bpf/tracepoints.c:62-64); such an event takes the most recent non-empty path of the same pid
-    (in time order), or is dropped when there is none.  Returns `cols` itself when no path is empty."""
+    events (tracker/bpf/tracepoints.c:62-64); such an event takes the most recent non-empty path of the same process
+    -- (source, pid) -- in time order, or is dropped when there is none.  Returns `cols` itself when no path is empty."""
     poff, pdata = cols.strings["path"]
     empty = (poff[1:] - poff[:-1]) == 0
     if cols.n == 0 or not empty.any():
         return cols
     order = np.argsort(cols.timestamp, kind="stable")
-    by_pid = order[np.argsort(cols.pid[order], kind="stable")]          # grouped by pid, time order inside a group
-    pid_g = cols.pid[by_pid]
+    key = process_keys(cols)
+    by_pid = order[np.argsort(key[order], kind="stable")]               # grouped by process, time order inside a group
+    pid_g = key[by_pid]
     start = np.r_[True, pid_g[1:] != pid_g[:-1]]
     grp_first = np.maximum.accumulate(np.where(start, np.arange(cols.n), 0))
     have = np.where(~empty[by_pid], np.arange(cols.n), -1)
@@ -146,7 +156,8 @@ def resolve_columns(cols: EventColumns) -> EventColumns:
     strings = {name: _gather_strings(*cols.strings[name], keep) for name in STRING_COLUMNS if name != "path"}
     strings["path"] = _gather_strings(poff, pdata, src[keep])
     sc = {k: getattr(cols, k)[keep] for k in ("ts_sec", "ts_nanos", "pid", "tid", "flags", "ret_val", "bytes", "event_slot")}
-    return EventColumns(n=int(keep.shape[0]), path_flags=cols.path_flags[src[keep]], strings=strings, **sc)
+    return EventColumns(n=int(keep.shape[0]), path_flags=cols.path_flags[src[keep]], strings=strings,
+                        source=None if cols.source is None else cols.source[keep], **sc)
 
 
 def path_flags_of(off, data) -> np.ndarray:
@@ -173,9 +184,10 @@ def intern_nodes(cols: EventColumns, order=None, merge_renames=True):
     (poff, pdata), (goff, gdata) = cols.strings["path"], cols.strings["new_path"]
     pdata = pdata if pdata.size else np.zeros(1, np.uint8)
     gdata = gdata if gdata.size else np.zeros(1, np.uint8)
-    _lib.check(_lib.lib().nerrf_trace_intern(n, order_p, _p(cols.pid), _p(poff), _p(pdata), _p(goff), _p(gdata),
-                                             int(bool(merge_renames)), _p(node_p), _p(node_f), _p(node_g), C.byref(nn),
-                                             _p(kind), _p(name_event), _p(name_which), cap), "nerrf_trace_intern")
+    src = None if cols.source is None else np.ascontiguousarray(cols.source, np.uint16)
+    _lib.check(_lib.lib().nerrf_trace_intern_ex(n, order_p, _p(cols.pid), None if src is None else _p(src), _p(poff), _p(pdata),
+                                                _p(goff), _p(gdata), int(bool(merge_renames)), _p(node_p), _p(node_f), _p(node_g),
+                                                C.byref(nn), _p(kind), _p(name_event), _p(name_which), cap), "nerrf_trace_intern_ex")
     N = nn.value
     return node_p, node_f, node_g, kind[:N].copy(), name_event[:N].copy(), name_which[:N].copy()
 
@@ -196,6 +208,7 @@ def intern_nodes_device(cols: EventColumns, order=None, merge_renames=True, devi
     d_pdata = up(pdata if pdata.size else np.zeros(1, np.uint8), np.uint8)
     d_gdata = up(gdata if gdata.size else np.zeros(1, np.uint8), np.uint8)
     d_order = None if order is None else up(order, np.int64)
+    d_src = None if cols.source is None else up(cols.source.astype(np.uint16).view(np.int16), np.int16)
     node_p = torch.empty(max(n, 1), dtype=torch.int32, device=dev); node_f = torch.empty_like(node_p); node_g = torch.empty_like(node_p)
     kind = torch.zeros(cap, dtype=torch.int8, device=dev); name_event = torch.zeros(cap, dtype=torch.int64, device=dev)
     name_which = torch.zeros(cap, dtype=torch.int8, device=dev)
@@ -205,12 +218,12 @@ def intern_nodes_device(cols: EventColumns, order=None, merge_renames=True, devi
     ws_ptr = (ws.data_ptr() + 255) & ~255
     nn = C.c_int64()
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().nerrf_trace_intern_device(n, n, _lib.ptr(d_order), _lib.ptr(d_pid), _lib.ptr(d_poff), _lib.ptr(d_pdata),
-                                                        _lib.ptr(d_goff), _lib.ptr(d_gdata), int(bool(merge_renames)),
-                                                        _lib.ptr(node_p), _lib.ptr(node_f), _lib.ptr(node_g), C.byref(nn),
-                                                        _lib.ptr(kind), _lib.ptr(name_event), _lib.ptr(name_which), cap,
-                                                        C.c_void_p(ws_ptr), need.value, _lib.current_stream_ptr()),
-                   "nerrf_trace_intern_device")
+        _lib.check(_lib.lib().nerrf_trace_intern_device_ex(n, n, _lib.ptr(d_order), _lib.ptr(d_pid), _lib.ptr(d_src), _lib.ptr(d_poff),
+                                                           _lib.ptr(d_pdata), _lib.ptr(d_goff), _lib.ptr(d_gdata), int(bool(merge_renames)),
+                                                           _lib.ptr(node_p), _lib.ptr(node_f), _lib.ptr(node_g), C.byref(nn),
+                                                           _lib.ptr(kind), _lib.ptr(name_event), _lib.ptr(name_which), cap,
+                                                           C.c_void_p(ws_ptr), need.value, _lib.current_stream_ptr()),
+                   "nerrf_trace_intern_device_ex")
     N = nn.value
     host = lambda t_: t_.cpu().numpy()
     if return_device:
@@ -265,7 +278,8 @@ def graph_from_columns(cols: EventColumns, merge_renames=True, window=None, devi
 
     names = _node_names(cols, name_event, name_which)
     meta = {"kind": "trace", "names": names, "node_kind": kind.astype(np.int64), "t0": t0, "span": span,
-            "merge_renames": bool(merge_renames)}
+            "merge_renames": bool(merge_renames),
+            "node_source": np.zeros(N, np.int64) if cols.source is None else cols.source[name_event].astype(np.int64)}
     if device is not None:
         # device path: features by integer atomics + one node pass, edges sorted into CSR by the radix-sort stage
         import torch

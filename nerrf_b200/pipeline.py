@@ -205,15 +205,17 @@ def edge_kill_confidence(g: G.TemporalGraph, candidates: np.ndarray, pids: np.nd
 
 def node_dir_hashes(g: G.TemporalGraph, nodes=None):
     """int64 parent-directory hash (stream.dir_hash) of the given nodes (all when None): on the device for graphs of a
-    device-resident stream (nerrf_trace_dir_hash), from the name strings for host graphs."""
+    device-resident stream (nerrf_trace_dir_hash_ex), from the name strings and meta["node_source"] for host graphs --
+    qualified by each node's source either way, so a directory group never spans two hosts."""
     from .stream import dir_hash
     fn = g.meta.get("dir_hash")
     if callable(fn):
         dh = fn()
         return dh if nodes is None else dh[torch.as_tensor(np.asarray(nodes, np.int64)).to(dh.device)]
     names = g.meta["names"]
+    src = g.meta.get("node_source")
     idx = range(len(names)) if nodes is None else np.asarray(nodes, np.int64).tolist()
-    return torch.tensor([dir_hash(names[int(i)]) for i in idx], dtype=torch.int64)
+    return torch.tensor([dir_hash(names[int(i)], 0 if src is None else int(src[int(i)])) for i in idx], dtype=torch.int64)
 
 
 def propose_restores(cand_dir, file_dir, file_size, file_is_cand, max_restores: int = 4, min_files: int = 8):

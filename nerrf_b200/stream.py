@@ -83,7 +83,10 @@ def concat_columns(parts) -> ingest.EventColumns:
             offs.append(off[:-1] + base); datas.append(data); base += int(off[-1])
         strings[name] = (np.concatenate(offs + [np.asarray([base], np.int64)]), np.concatenate(datas) if datas else np.zeros(0, np.uint8))
     cat = lambda k: np.concatenate([getattr(c, k) for c in parts])
-    return ingest.EventColumns(n=sum(c.n for c in parts), strings=strings,
+    source = None
+    if any(c.source is not None for c in parts):
+        source = np.concatenate([c.source if c.source is not None else np.zeros(c.n, np.uint16) for c in parts]).astype(np.uint16)
+    return ingest.EventColumns(n=sum(c.n for c in parts), strings=strings, source=source,
                                **{k: cat(k) for k in ("ts_sec", "ts_nanos", "pid", "tid", "flags", "ret_val", "bytes", "event_slot", "path_flags")})
 
 
@@ -124,7 +127,54 @@ def window(cols: ingest.EventColumns, t_lo: float, t_hi: float) -> ingest.EventC
     keep = np.nonzero((ts > t_lo) & (ts <= t_hi))[0]
     strings = {name: ingest._gather_strings(*cols.strings[name], keep) for name in ingest.STRING_COLUMNS}
     sc = {k: getattr(cols, k)[keep] for k in ("ts_sec", "ts_nanos", "pid", "tid", "flags", "ret_val", "bytes", "event_slot", "path_flags")}
-    return ingest.EventColumns(n=int(keep.shape[0]), strings=strings, **sc)
+    return ingest.EventColumns(n=int(keep.shape[0]), strings=strings, source=None if cols.source is None else cols.source[keep], **sc)
+
+
+def with_source(cols: ingest.EventColumns, source: int) -> ingest.EventColumns:
+    """`cols` with every event from source id `source`"""
+    check_source_id(source)
+    return ingest.EventColumns(**{**cols.__dict__, "source": np.full(cols.n, source, np.uint16)})
+
+
+def host_streams(k_hosts: int, n_procs: int, n_attacked: int, attacked_hosts=None, seed: int = 0, bystanders: int = 0):
+    """K hosts' traces whose processes and files collide on purpose: every host runs fleet_columns(n_procs, ...) with the
+    same seed, so all hosts reuse the same pids and /app/uploads file names and the same clock; the hosts in
+    `attacked_hosts` (default: every other host, starting with host 0) run `n_attacked` LockBit processes, the others only
+    benign ones -- whose pids equal the attackers' pids on the attacked hosts.
+    -> list of (EventColumns of source h, encrypted paths, attacker node names "pid:<n>"), one per host h."""
+    attacked = set(range(0, k_hosts, 2)) if attacked_hosts is None else set(attacked_hosts)
+    out = []
+    for h in range(k_hosts):
+        cols, enc, pids = fleet_columns(n_procs, n_attacked if h in attacked else 0, seed=seed, return_pids=True,
+                                        bystanders=bystanders if h in attacked else 0)
+        out.append((with_source(cols, h), enc, pids))
+    return out
+
+
+def relabel_single_source(cols: ingest.EventColumns) -> ingest.EventColumns:
+    """The multi-source stream `cols` as ONE source, the identity the source column stands for: every (source, pid)
+    becomes a pid of its own (numbered in (source, pid) order), every non-empty path / new_path gets the prefix
+    "@<source>/", empty paths stay empty (so path-less writes resolve as before).  path_flags are kept as they were (the
+    prefix would hide the /tmp rule).  Feeding the result to the single-source path gives the multi-source graph."""
+    if cols.source is None:
+        return cols
+    uniq, inv = np.unique(ingest.process_keys(cols), return_inverse=True)
+    if uniq.size >= (1 << 32):
+        raise ValueError("more than 2^32 processes")
+    strings = dict(cols.strings)
+    for name in ("path", "new_path"):
+        off, data = cols.strings[name]
+        ln = off[1:] - off[:-1]
+        pre = [("@%d/" % s).encode() for s in range(int(cols.source.max()) + 1)]
+        plen = np.asarray([len(p) for p in pre], np.int64)[cols.source.astype(np.int64)] * (ln > 0)
+        new_off = np.zeros(cols.n + 1, np.int64); np.cumsum(ln + plen, out=new_off[1:])
+        raw, parts = data.tobytes(), []
+        src = cols.source.tolist()
+        for i, (a, b) in enumerate(zip(off[:-1].tolist(), off[1:].tolist())):
+            if b > a:
+                parts.append(pre[src[i]]); parts.append(raw[a:b])
+        strings[name] = (new_off, np.frombuffer(b"".join(parts), np.uint8).copy())
+    return ingest.EventColumns(**{**cols.__dict__, "pid": inv.astype(np.uint32).reshape(-1), "strings": strings, "source": None})
 
 
 # ---------------------------------------------------------------------------------------------- device-resident stream
@@ -136,29 +186,40 @@ def _mix64(h: int) -> int:
     return h or 1
 
 
-def name_hash(name) -> int:
-    """The 64-bit name hash of csrc/intern_device.cu (nerrf_trace_name_hash) on the host, as a SIGNED int64: FNV-1a over
-    the bytes seeded with the length, murmur3 finaliser; "pid:<n>" names hash their pid."""
+def check_source_id(source: int) -> int:
+    from . import _lib
+    if not isinstance(source, (int, np.integer)) or not 0 <= int(source) < (1 << 16):
+        raise _lib.NerrfError("source id %r out of range [0, 65536)" % (source,))
+    return int(source)
+
+
+def name_hash(name, source: int = 0) -> int:
+    """The 64-bit name hash of csrc/intern_device.cu (nerrf_trace_name_hash_ex) on the host, as a SIGNED int64: FNV-1a
+    over the bytes seeded with the length, murmur3 finaliser; "pid:<n>" names hash (source << 32) | pid; a file name of
+    a nonzero source is qualified by it (source 0: the unqualified hash)."""
+    source = check_source_id(source)
     if isinstance(name, str) and name.startswith("pid:") and name[4:].isdigit():
-        h = _mix64((int(name[4:]) + 0x9E3779B97F4A7C15) & _M64)
+        h = _mix64((((source << 32) | int(name[4:])) + 0x9E3779B97F4A7C15) & _M64)
     else:
         b = name.encode("utf-8") if isinstance(name, str) else bytes(name)
         h = (0xcbf29ce484222325 ^ len(b)) & _M64
         for c in b:
             h = ((h ^ c) * 0x100000001b3) & _M64
         h = _mix64(h)
+        if source:
+            h = _mix64((h + source * 0x9E3779B97F4A7C15) & _M64)
     return h - (1 << 64) if h >= (1 << 63) else h
 
 
-def dir_hash(name) -> int:
-    """The 64-bit hash of a node's parent directory (csrc/intern_device.cu nerrf_trace_dir_hash) on the host, as a SIGNED
-    int64: name_hash of the bytes up to (not including) the last '/' -- the empty string when there is none; "pid:<n>"
-    names hash as in name_hash."""
+def dir_hash(name, source: int = 0) -> int:
+    """The 64-bit hash of a node's parent directory (csrc/intern_device.cu nerrf_trace_dir_hash_ex) on the host, as a
+    SIGNED int64: name_hash of the bytes up to (not including) the last '/' -- the empty string when there is none;
+    "pid:<n>" names hash as in name_hash.  Qualified by `source` like name_hash."""
     if isinstance(name, str) and name.startswith("pid:") and name[4:].isdigit():
-        return name_hash(name)
+        return name_hash(name, source)
     b = name.encode("utf-8") if isinstance(name, str) else bytes(name)
     k = b.rfind(b"/")
-    return name_hash(b[:k] if k >= 0 else b"")
+    return name_hash(b[:k] if k >= 0 else b"", source)
 
 
 def parent_dir(name) -> str:
@@ -235,6 +296,7 @@ class _DeviceColumns:
         self.s = {k: torch.zeros(max(rows, 1), dtype=getattr(torch, dt), device=dev) for k, dt in _SCALARS}
         self.off = [torch.zeros(max(rows, 1) + 1, dtype=torch.int64, device=dev) for _ in range(4)]
         self.data = [torch.zeros(max(int(b), 1), dtype=torch.uint8, device=dev) for b in nbytes]
+        self.source = torch.zeros(max(rows, 1), dtype=torch.int16, device=dev)   # uint16 source ids, stored as int16
 
     @property
     def rows(self):
@@ -255,6 +317,7 @@ class _DeviceColumns:
                 t = torch.zeros(new, dtype=self.s[k].dtype, device=self.dev); t[:n_used] = self.s[k][:n_used]; self.s[k] = t
             for q in range(4):
                 t = torch.zeros(new + 1, dtype=torch.int64, device=self.dev); t[:n_used + 1] = self.off[q][:n_used + 1]; self.off[q] = t
+            t = torch.zeros(new, dtype=torch.int16, device=self.dev); t[:n_used] = self.source[:n_used]; self.source = t
         for q in range(4):
             if nbytes[q] > self.data[q].numel():
                 t = torch.zeros(max(int(nbytes[q]), 2 * self.data[q].numel()), dtype=torch.uint8, device=self.dev)
@@ -269,7 +332,8 @@ class _DeviceColumns:
         for q, name in enumerate(ingest.STRING_COLUMNS):
             off = self.off[q][:n + 1].cpu().numpy()
             strings[name] = (off, self.data[q][:int(off[-1])].cpu().numpy())
-        return ingest.EventColumns(n=n, strings=strings, **sc)
+        source = self.source[:n].cpu().numpy().view(np.uint16)
+        return ingest.EventColumns(n=n, strings=strings, source=source if source.any() else None, **sc)
 
 
 def _lib_ptr_array(tensors):
@@ -277,9 +341,9 @@ def _lib_ptr_array(tensors):
     return _lib.ptr_array(tensors)
 
 
-def _decode_into(dc: _DeviceColumns, n: int, used_bytes, raw: np.ndarray, partial: bool, timings=None):
-    """Frame `raw` on the host, decode its Event records on the device into rows n.. of `dc`.  -> (rows added, bytes
-    consumed, new used_bytes).  Raises (and adds nothing) when a record is malformed: same message and byte offset as
+def _decode_into(dc: _DeviceColumns, n: int, used_bytes, raw: np.ndarray, partial: bool, timings=None, source: int = 0):
+    """Frame `raw` on the host, decode its Event records on the device into rows n.. of `dc`, all from source id `source`.
+    -> (rows added, bytes consumed, new used_bytes).  Raises (and adds nothing) when a record is malformed: same message and byte offset as
     ingest.decode_event_batch."""
     import ctypes as C
     import time
@@ -307,9 +371,10 @@ def _decode_into(dc: _DeviceColumns, n: int, used_bytes, raw: np.ndarray, partia
         ev0 = torch.cuda.Event(enable_timing=True); ev1 = torch.cuda.Event(enable_timing=True)
         with torch.cuda.device(dc.dev):
             ev0.record()
-            _lib.check(_lib.lib().nerrf_trace_decode_device(
-                _lib.ptr(wire_d), _lib.ptr(rec_d[0]), _lib.ptr(rec_d[1]), _lib.ptr(rec_d[2]), m, n, dc.ptrs(), _lib.ptr(status),
-                C.c_void_p((ws.data_ptr() + 255) & ~255), need.value, _lib.current_stream_ptr()), "nerrf_trace_decode_device")
+            _lib.check(_lib.lib().nerrf_trace_decode_device_ex(
+                _lib.ptr(wire_d), _lib.ptr(rec_d[0]), _lib.ptr(rec_d[1]), _lib.ptr(rec_d[2]), m, n, dc.ptrs(), _lib.ptr(dc.source),
+                int(source), _lib.ptr(status), C.c_void_p((ws.data_ptr() + 255) & ~255), need.value, _lib.current_stream_ptr()),
+                "nerrf_trace_decode_device_ex")
             ev1.record()
         back = torch.cat([status] + [o[n + m:n + m + 1] for o in dc.off]).cpu().numpy()
         if timings is not None:
@@ -372,6 +437,7 @@ class DeviceStream:
         self.d_order = up(self.order, np.int64)
         self.d_ts = up(ts, np.float64)
         self.d_pid = up(cols.pid.astype(np.uint32).view(np.int32), np.int32)
+        self.d_source = None if cols.source is None else up(cols.source.astype(np.uint16).view(np.int16), np.int16)
         self.d_poff, self.d_goff = up(poff, np.int64), up(goff, np.int64)
         self.d_pdata = up(pdata if pdata.size else np.zeros(1, np.uint8), np.uint8)
         self.d_gdata = up(gdata if gdata.size else np.zeros(1, np.uint8), np.uint8)
@@ -409,6 +475,7 @@ class DeviceStream:
         self.cols = None
         self._dc = _DeviceColumns(self.dev, 1024, [1 << 16] * 4)
         self._used = [0, 0, 0, 0]
+        self._key_bits = 32                                    # 48 once a nonzero source has appended: (source, pid) regroup
         self._horizon = -np.inf
         self._slot_map = torch.tensor(G.OBSERVABLE_SLOT, dtype=torch.uint8, device=self.dev) if observable else None
         self.n = 0
@@ -418,31 +485,44 @@ class DeviceStream:
         return self
 
     @property
+    def multi_source(self) -> bool:
+        """some event comes from a nonzero source (the live stream: since the first such append)"""
+        if self.cols is None:
+            return self._key_bits == 48
+        return self.cols.source is not None and bool(self.cols.source.any())
+
+    @property
     def resident_events(self) -> int:
         """events held in HBM (live stream)"""
         return self.n
 
-    def append(self, wire_bytes, partial=False) -> int:
-        """Decode whole EventBatch records on the device and append them.  partial=True: a cut-off trailing record is
-        left for the caller to resend with the rest of its bytes.  -> bytes consumed.  A malformed record raises and
-        leaves the stream as it was."""
+    def append(self, wire_bytes, partial=False, source: int = 0) -> int:
+        """Decode whole EventBatch records on the device and append them, every one from source id `source` (the host
+        whose tracker sent them; processes and files of different sources never merge).  partial=True: a cut-off trailing
+        record is left for the caller to resend with the rest of its bytes.  -> bytes consumed.  A malformed record
+        raises and leaves the stream as it was."""
+        source = check_source_id(source)
         raw = np.frombuffer(wire_bytes, dtype=np.uint8) if not isinstance(wire_bytes, np.ndarray) else np.ascontiguousarray(wire_bytes, np.uint8)
         self.timings_ms = {}
-        m, consumed, used = _decode_into(self._dc, self.n, self._used, raw, partial, self.timings_ms)
+        m, consumed, used = _decode_into(self._dc, self.n, self._used, raw, partial, self.timings_ms, source)
+        self.appended = (self.n, self.n + m)
         if m:
-            before = self.n, self._used
+            before = self.n, self._used, self._key_bits
             self.n += m
             self._used = used
+            if source:
+                self._key_bits = 48
             try:
                 self._rebuild()
             except Exception:                                  # e.g. 2^31 resolved path bytes: the rows stay unused past n
-                self.n, self._used = before
+                self.n, self._used, self._key_bits = before
+                self.appended = (self.n, self.n)
                 raise
         return consumed
 
     def compact(self, horizon: float):
-        """Drop the events no window ending after `horizon + window` can hold (ts <= horizon), except each pid's latest
-        event with a path, which a later path-less write of that pid still resolves to.  Stored order is kept."""
+        """Drop the events no window ending after `horizon + window` can hold (ts <= horizon), except each (source, pid)'s
+        latest event with a path, which a later path-less write of that process still resolves to.  Stored order is kept."""
         import ctypes as C
         from . import _lib
         torch = self.torch
@@ -462,9 +542,9 @@ class DeviceStream:
             _lib.check(_lib.lib().nerrf_trace_gather_rows_workspace_bytes(m, C.byref(need)), "gather_rows_workspace_bytes")
             ws = torch.empty(need.value + 256, dtype=torch.uint8, device=self.dev)
             with torch.cuda.device(self.dev):
-                _lib.check(_lib.lib().nerrf_trace_gather_rows(self._dc.ptrs(), _lib.ptr(self._retain), m, out.ptrs(),
-                                                              C.c_void_p((ws.data_ptr() + 255) & ~255), need.value,
-                                                              _lib.current_stream_ptr()), "nerrf_trace_gather_rows")
+                _lib.check(_lib.lib().nerrf_trace_gather_rows_ex(self._dc.ptrs(), _lib.ptr(self._dc.source), _lib.ptr(self._retain), m,
+                                                                 out.ptrs(), _lib.ptr(out.source), C.c_void_p((ws.data_ptr() + 255) & ~255),
+                                                                 need.value, _lib.current_stream_ptr()), "nerrf_trace_gather_rows_ex")
             self._dc, self.n = out, m
             self._used = [int(v) for v in torch.cat([o[m:m + 1] for o in out.off]).cpu().numpy()]
             self._rebuild()
@@ -491,10 +571,11 @@ class DeviceStream:
         counts = (C.c_int64 * 3)()
         poff, pdata, goff, gdata = dc.off[2], dc.data[2], dc.off[3], dc.data[3]
         with torch.cuda.device(dev):
-            _lib.check(_lib.lib().nerrf_trace_stream_order(
-                n, _lib.ptr(dc.s["ts_sec"]), _lib.ptr(dc.s["ts_nanos"]), _lib.ptr(dc.s["pid"]), _lib.ptr(poff), float(self._horizon),
-                _lib.ptr(ts), _lib.ptr(order), _lib.ptr(ts_sorted), _lib.ptr(src), _lib.ptr(res_off), _lib.ptr(retain), counts,
-                C.c_void_p((ws.data_ptr() + 255) & ~255), need.value, _lib.current_stream_ptr()), "nerrf_trace_stream_order")
+            _lib.check(_lib.lib().nerrf_trace_stream_order_ex(
+                n, _lib.ptr(dc.s["ts_sec"]), _lib.ptr(dc.s["ts_nanos"]), _lib.ptr(dc.s["pid"]), _lib.ptr(dc.source), self._key_bits,
+                _lib.ptr(poff), float(self._horizon), _lib.ptr(ts), _lib.ptr(order), _lib.ptr(ts_sorted), _lib.ptr(src),
+                _lib.ptr(res_off), _lib.ptr(retain), counts, C.c_void_p((ws.data_ptr() + 255) & ~255), need.value,
+                _lib.current_stream_ptr()), "nerrf_trace_stream_order_ex")
         n_keep, n_retain, pbytes = int(counts[0]), int(counts[1]), int(counts[2])
         res_data = torch.zeros(max(pbytes, 1), dtype=torch.uint8, device=dev)
         pf, pf_raw, slot = e(torch.uint8), e(torch.uint8), e(torch.uint8)
@@ -507,6 +588,7 @@ class DeviceStream:
         self.n_keep, self._n_retain, self._retain = n_keep, n_retain, retain[:n_retain]
         self.d_order, self.d_ts_sorted, self.d_ts = order[:n_keep], ts_sorted[:n_keep], ts
         self.d_pid, self.d_poff, self.d_pdata, self.d_goff, self.d_gdata = dc.s["pid"], res_off, res_data, goff, gdata
+        self.d_source = dc.source
         self.d_raw_slot, self.d_slot, self.d_bytes, self.d_pf, self.d_pf_raw = dc.s["event_slot"], slot, dc.s["bytes"], pf, pf_raw
         if n_keep:
             lohi = torch.stack([ts_sorted[0], ts_sorted[n_keep - 1]]).cpu().numpy()
@@ -576,11 +658,11 @@ class DeviceStream:
         nn = C.c_int64()
         ws_ptr = (self._ws.data_ptr() + 255) & ~255
         with torch.cuda.device(self.dev):
-            _lib.check(_lib.lib().nerrf_trace_intern_device(
-                nw, self.n, _lib.ptr(sel), _lib.ptr(self.d_pid), _lib.ptr(self.d_poff), _lib.ptr(self.d_pdata), _lib.ptr(self.d_goff),
-                _lib.ptr(self.d_gdata), int(self.merge), _lib.ptr(self.node_p), _lib.ptr(self.node_f), _lib.ptr(self.node_g),
-                C.byref(nn), _lib.ptr(self.kind), _lib.ptr(self.name_event), _lib.ptr(self.name_which), self.cap,
-                C.c_void_p(ws_ptr), self._ws_bytes, _lib.current_stream_ptr()), "nerrf_trace_intern_device")
+            _lib.check(_lib.lib().nerrf_trace_intern_device_ex(
+                nw, self.n, _lib.ptr(sel), _lib.ptr(self.d_pid), _lib.ptr(self.d_source), _lib.ptr(self.d_poff), _lib.ptr(self.d_pdata),
+                _lib.ptr(self.d_goff), _lib.ptr(self.d_gdata), int(self.merge), _lib.ptr(self.node_p), _lib.ptr(self.node_f),
+                _lib.ptr(self.node_g), C.byref(nn), _lib.ptr(self.kind), _lib.ptr(self.name_event), _lib.ptr(self.name_which),
+                self.cap, C.c_void_p(ws_ptr), self._ws_bytes, _lib.current_stream_ptr()), "nerrf_trace_intern_device_ex")
         N = int(nn.value)
         t0 = t_first; span = max(t_last - t0, 1e-6)
         window = window_s or max(span, G.WINDOW)
@@ -609,26 +691,28 @@ class DeviceStream:
             lab = (torch.bincount(F[(raw == 1) | (raw == 2)].long(), minlength=N) > 0)
         nh = torch.empty(N, dtype=torch.int64, device=self.dev)
         with torch.cuda.device(self.dev):
-            _lib.check(_lib.lib().nerrf_trace_name_hash(N, _lib.ptr(self.name_event), _lib.ptr(self.name_which), _lib.ptr(self.d_pid),
-                                                        _lib.ptr(self.d_poff), _lib.ptr(self.d_pdata), _lib.ptr(self.d_goff),
-                                                        _lib.ptr(self.d_gdata), _lib.ptr(nh), _lib.current_stream_ptr()),
-                       "nerrf_trace_name_hash")
-        bufs = (self.name_event, self.name_which, self.d_pid, self.d_poff, self.d_pdata, self.d_goff, self.d_gdata)
+            _lib.check(_lib.lib().nerrf_trace_name_hash_ex(N, _lib.ptr(self.name_event), _lib.ptr(self.name_which), _lib.ptr(self.d_pid),
+                                                           _lib.ptr(self.d_source), _lib.ptr(self.d_poff), _lib.ptr(self.d_pdata),
+                                                           _lib.ptr(self.d_goff), _lib.ptr(self.d_gdata), _lib.ptr(nh),
+                                                           _lib.current_stream_ptr()), "nerrf_trace_name_hash_ex")
+        bufs = (self.name_event, self.name_which, self.d_pid, self.d_source, self.d_poff, self.d_pdata, self.d_goff, self.d_gdata)
 
         def dir_hash_device(bufs=bufs):
             """int64 [N] parent-directory hash of every node (nerrf_trace_dir_hash); valid until the stream changes."""
             dh = torch.empty(N, dtype=torch.int64, device=self.dev)
             with torch.cuda.device(self.dev):
-                _lib.check(_lib.lib().nerrf_trace_dir_hash(N, *(_lib.ptr(b) for b in bufs), _lib.ptr(dh), _lib.current_stream_ptr()),
-                           "nerrf_trace_dir_hash")
+                _lib.check(_lib.lib().nerrf_trace_dir_hash_ex(N, *(_lib.ptr(b) for b in bufs), _lib.ptr(dh), _lib.current_stream_ptr()),
+                           "nerrf_trace_dir_hash_ex")
             return dh
         ne, nwh = self.name_event[:N].cpu().numpy(), self.name_which[:N].cpu().numpy()
+        node_source = np.zeros(N, np.int64) if self.d_source is None else \
+            (self.d_source[self.name_event[:N]].to(torch.int64) & 0xffff).cpu().numpy()
         names = LazyNames(self.cols, ne, nwh) if self.cols is not None else \
             DeviceNames(self.d_pid, self.d_poff, self.d_pdata, self.d_goff, self.d_gdata, ne, nwh)
         meta = {"kind": "trace", "names": names,
                 "node_kind": kind_d.cpu().numpy().astype(np.int64), "t0": t0, "span": span, "merge_renames": self.merge,
                 "label": lab.cpu().numpy().astype(np.int64), "size_mb": size_mb.cpu().numpy(), "device": str(self.dev),
-                "name_hash": nh, "dir_hash": dir_hash_device, "events": nw, "window_ranks": (lo, hi), "perm": perm if Gn is None else None}
+                "name_hash": nh, "dir_hash": dir_hash_device, "events": nw, "node_source": node_source, "window_ranks": (lo, hi), "perm": perm if Gn is None else None}
         if edge_labels:
             meta["edge_label"] = G.edge_labels_device(P, F, self.d_raw_slot[sel], rowptr, col, N)
         return G.TemporalGraph(rowptr, col, ew, x, meta)
@@ -676,7 +760,7 @@ class TickResult:
     events: int
     nodes: int
     edges: int
-    planned: list                  # paths this tick's plan reverts (new ones only)
+    planned: list                  # paths this tick's plan reverts (new ones only); (host, path) with several sources
     timings_ms: dict
     truncated: bool = False
     restored: list = field(default_factory=list)   # directories this tick's plan restores from the snapshot
@@ -708,33 +792,87 @@ class StreamingPlanner:
     killed: set = field(default_factory=set)
     restored_dirs: list = field(default_factory=list)
     ticks: list = field(default_factory=list)
-    lateness_s: float = 0.0        # live feed: a tick at t_hi fires once an event with ts > t_hi + lateness_s has arrived
+    lateness_s: float = 0.0        # live feed: a tick at t_hi fires once every open source has delivered an event with ts > t_hi + lateness_s
     live: object = None            # live feed: the DeviceStream the bytes go to
-    _carry: bytes = b""
+    sources: dict = field(default_factory=dict)    # source name -> source id (add_source); ids number the hosts from 0
+    _open: set = field(default_factory=set)        # ids of the sources the watermark waits for
+    _latest: dict = field(default_factory=dict)    # source id -> latest event time it delivered
+    _carry: dict = field(default_factory=dict)     # source id -> cut-off record bytes carried to its next chunk
+    _names: list = field(default_factory=list)     # source id -> name
+    _host_keys: bool = None        # plan names are (host, name) pairs: fixed by the first tick, for the planner's lifetime
     _t0: float = None
     _t_hi: float = None
 
-    def feed(self, chunk) -> list:
-        """Live form of run(): `chunk` = the next bytes of the tracker's EventBatch stream, cut anywhere (a partial record
-        is carried over to the next call).  The bytes are decoded and appended on the device; every tick that can no
-        longer change fires.  -> the TickResults fired by this call.  Ticks, windows and plans are those run() computes
-        over the whole stream when no event arrives more than lateness_s late."""
+    def add_source(self, name: str) -> int:
+        """Register a source (a host's tracker stream) -> its id (the next free one; an existing name keeps its id).
+        Names are 1-64 characters of [A-Za-z0-9._-], not "." or "..": they name per-host plan files.
+        Register every host before feeding: the watermark only waits for registered sources.  A host registered after
+        ticks have fired joins the watermark from then on, and its events at or before the last tick are late data (later
+        windows hold them, fired ticks do not).  A second source cannot join once ticks have fired with one, whose plans
+        name files without a host: that raises ValueError."""
+        from .ai.planner import emit
+        emit.check_host_name(name)
+        if name not in self.sources:
+            if len(self.sources) >= (1 << 16):
+                raise ValueError("at most 65536 sources")
+            if self._host_keys is False:
+                raise ValueError("source %r registered after ticks fired with one source: register every source before "
+                                 "the first tick" % name)
+            self.sources[name] = len(self._names)
+            self._names.append(name)
+            self._open.add(self.sources[name])
+        return self.sources[name]
+
+    def host_name(self, source: int) -> str:
+        """the registered name of source id `source` (its decimal id when it has none)"""
+        return self._names[source] if 0 <= source < len(self._names) else str(int(source))
+
+    def feed(self, chunk, source: str = "default") -> list:
+        """Live form of run(): `chunk` = the next bytes of source `source`'s EventBatch stream (registered on first use;
+        with several hosts, register them all with add_source before the first chunk), cut anywhere: a partial record is carried over to that source's next call, never glued to another source's bytes.
+        The bytes are decoded and appended on the device; every tick that can no longer change fires: with several
+        sources, once every open source has delivered an event past it (the low watermark).  -> the TickResults fired by
+        this call.  Ticks, windows and plans are those run() computes over the whole stream when no event arrives more
+        than lateness_s late."""
         if self.dist_ctx is not None and self.dist_ctx.world > 1:
             raise NotImplementedError("live feeding runs on one GPU")
+        sid = self.add_source(source)
+        if sid not in self._open:
+            raise ValueError("source %r was closed" % source)
         if self.live is None:
             self.live = DeviceStream.live(self.device, observable=True)
-        buf = self._carry + bytes(chunk)
-        used = self.live.append(buf, partial=True)
-        self._carry = buf[used:]
+        buf = self._carry.get(sid, b"") + bytes(chunk)
+        used = self.live.append(buf, partial=True, source=sid)
+        self._carry[sid] = buf[used:]
+        self._note_latest(sid)
+        return self._fire(final=False)
+
+    def _note_latest(self, sid: int):
+        a, b = self.live.appended
+        if b > a:
+            t = float(self.live.d_ts[a:b].max())
+            self._latest[sid] = max(self._latest.get(sid, -np.inf), t)
+
+    def close_source(self, name: str) -> list:
+        """Source `name` has ended: the watermark stops waiting for it.  A carried-over partial record of it is malformed
+        input.  -> the TickResults this releases."""
+        sid = self.sources[name]
+        if self._carry.get(sid):
+            self.live.append(self._carry[sid], source=sid)    # raises: the source ended inside a record
+        self._carry[sid] = b""
+        self._open.discard(sid)
+        if self.live is None:
+            return []
         return self._fire(final=False)
 
     def flush(self) -> list:
-        """End of the stream: fire the remaining ticks, the last one at the last event (like run()).  A carried-over
-        partial record is malformed input."""
+        """End of the stream (of every source): fire the remaining ticks, the last one at the last event (like run()).
+        A carried-over partial record is malformed input."""
         if self.live is None:
             return []
-        if self._carry:
-            self.live.append(self._carry)                      # raises: the stream ended inside a record
+        for sid, rest in self._carry.items():
+            if rest:
+                self.live.append(rest, source=sid)             # raises: the stream ended inside a record
         return self._fire(final=True)
 
     def _fire(self, final: bool) -> list:
@@ -751,7 +889,10 @@ class StreamingPlanner:
                 nxt = min(t_hi + self.tick_s, last)
             else:
                 nxt = t_hi + self.tick_s
-                if not last > nxt + self.lateness_s:
+                mark = last                                      # one source: the latest surviving event
+                if len(self.sources) > 1 and self._open:         # several: the low watermark over the open sources
+                    mark = min(self._latest.get(sid, -np.inf) for sid in self._open)
+                if not mark > nxt + self.lateness_s:
                     break
             self._t0, self._t_hi = t0, nxt
             k = len(self.ticks)
@@ -873,18 +1014,31 @@ class StreamingPlanner:
                 tm[k] = tm.get(k, 0.0) + float(v)
             got = []
             if lead:
+                node_src = g.meta.get("node_source")
+                if self._host_keys is None:              # decided once per planner, so reverted / killed hold one form
+                    self._host_keys = len(self.sources) > 1 or ds.multi_source
+                multi_src = self._host_keys
+                # several sources: a file or process is named (host, name), and its hash is qualified by its source
+                key = (lambda n, nm: (self.host_name(int(node_src[n])), nm)) if multi_src else (lambda n, nm: nm)
+                src_of = (lambda n: int(node_src[n])) if multi_src else (lambda n: 0)
+
+                def revert(nodes, node_names):
+                    """mark the files not reverted yet as reverted -> their keys, in plan order"""
+                    fresh = {}
+                    for n, nm in zip(nodes, node_names):
+                        if kind[n] == 0 and key(n, nm) not in self.reverted:
+                            fresh.setdefault(key(n, nm), name_hash(nm, src_of(n)))
+                    self.reverted.update(fresh)
+                    self._reverted_hash.update(fresh.values())
+                    return list(fresh)
                 plan_names = names.take(res.plan_nodes)           # one bulk fetch (device names of a live stream)
-                self.killed.update(nm for n, nm in zip(res.plan_nodes, plan_names) if kind[n] == 1)
-                got = [nm for n, nm in zip(res.plan_nodes, plan_names) if kind[n] == 0]
-                got = [nm for nm in dict.fromkeys(got) if nm not in self.reverted]
-                self.reverted.update(got)
-                self._reverted_hash.update(name_hash(nm) for nm in got)
+                self.killed.update(key(n, nm) for n, nm in zip(res.plan_nodes, plan_names) if kind[n] == 1)
+                got = revert(res.plan_nodes, plan_names)
                 new += got
                 for r in res.restores:                         # a restored directory brings back every file it covers
-                    cov = [nm for nm in dict.fromkeys(names.take(r["covers"])) if nm not in self.reverted]
-                    self.reverted.update(cov)
-                    self._reverted_hash.update(name_hash(nm) for nm in cov)
-                    restored.append(r["dir"]); self.restored_dirs.append(r["dir"])
+                    cov = revert(r["covers"], names.take(r["covers"]))
+                    d = key(r["covers"][0], r["dir"]) if r["covers"] else r["dir"]
+                    restored.append(d); self.restored_dirs.append(d)
                     got = got + cov
             # a pass proposes at most 32 - (restores) kills (word 0 holds both): plan again while the budget was used up
             more = bool(self.kill_candidates and res.n_kill >= 32 - res.n_restore and got)

@@ -3,15 +3,23 @@ ROADMAP.md:28,86 -- scheduled, never written).
 
     python -m nerrf_b200.undo --trace events.pb   --weights weights.pt --out plan.json --shell plan.sh
     python -m nerrf_b200.undo --trace trace.jsonl --train-epochs 25    --out plan.json
+    python -m nerrf_b200.undo --trace nodeA=a.pb --trace nodeB=b.pb --weights weights.pt --out plan.json --shell-dir DIR
 
 trace: serialized nerrf.trace.EventBatch bytes (*.pb; proto/trace.proto:47-49, e.g. a buffered StreamEvents stream) or
 the simulator's TRACE json lines (*.jsonl; benchmarks/m1/scripts/sim_lockbit_m1.py:24-36).  Stages: ingest -> temporal
 graph (features + CSR on the GPU for *.pb) -> GraphSAGE_T.forward -> top-A candidates -> lstm.forward -> mcts plan ->
 emit.  Everything between the graph and the plan runs in the CUDA kernels; there is no CPU fallback.
+
+Several `--trace HOST=PATH` arguments (*.pb, one per node's tracker) are planned as one graph whose processes and files
+are per host (source ids in argument order); every step of the plan names its "host", and --shell-dir writes one
+DIR/<host>.sh per host (--shell is refused: one script would hold every host's commands, and the hosts share file
+names).  A bare `--trace PATH`, or a single `--trace HOST=PATH`, is one source, as before: no host fields, and
+--shell-dir needs the HOST name.
 """
 from __future__ import annotations
 
 import argparse
+import os
 import sys
 import time
 
@@ -22,6 +30,42 @@ from .ai import train as T
 from .ai.models import GraphSAGE_T
 from .ai.models.lstm import LSTMScorer
 from .ai.planner import emit
+from .stream import concat_columns, with_source
+
+
+def parse_traces(specs) -> list:
+    """--trace values -> [(host or None, path)]: one bare PATH, or HOST=PATH for every source"""
+    out = []
+    for sp in specs:
+        host, eq, path = sp.partition("=")
+        out.append((emit.check_host_name(host), path) if eq and not os.path.exists(sp) else (None, sp))
+    if len(out) > 1 and any(h is None for h, _ in out):
+        raise SystemExit("several --trace arguments: give every one as HOST=PATH")
+    if len({h for h, _ in out}) < len(out):
+        raise SystemExit("--trace: a host name appears twice")
+    return out
+
+
+def check_outputs(traces, shell, shell_dir):
+    """refuse script outputs that do not fit the traces: --shell with several hosts, --shell-dir without host names"""
+    if shell and len(traces) > 1:
+        raise SystemExit("--shell with several --trace HOST=PATH: use --shell-dir (one script per host)")
+    if shell_dir and traces[0][0] is None:
+        raise SystemExit("--shell-dir names its scripts by host: give the trace as --trace HOST=PATH")
+
+
+def load_hosts(paths, device="cuda"):
+    """several hosts' EventBatch files as one stream, source id k = the k-th file -> (graph, seq, lengths, seq_nodes, n)"""
+    parts = []
+    for k, path in enumerate(paths):
+        if not path.endswith(".pb"):
+            raise SystemExit("several --trace arguments take EventBatch files (*.pb): %s" % path)
+        with open(path, "rb") as f:
+            parts.append(with_source(ingest.decode_event_batch(f.read()), k))
+    cols = concat_columns(parts)
+    g = ingest.graph_from_columns(cols, device=device, observable=True)
+    seq, lengths, nodes = ingest.sequences_from_columns(cols, observable=True)
+    return g, seq, lengths, nodes, cols.n
 
 
 def load_trace(path: str, device="cuda"):
@@ -59,7 +103,9 @@ def load_models(weights: str | None, train_epochs: int, layers: int = 2, log=pri
 
 def main(argv=None) -> dict:
     ap = argparse.ArgumentParser(prog="python -m nerrf_b200.undo", description=__doc__.split("\n")[0])
-    ap.add_argument("--trace", required=True); ap.add_argument("--id", default=None, help="attack id carried into the plan")
+    ap.add_argument("--trace", required=True, action="append",
+                    help="trace file, or HOST=FILE once per host (*.pb) for a plan over several hosts")
+    ap.add_argument("--id", default=None, help="attack id carried into the plan")
     ap.add_argument("--weights", default=None); ap.add_argument("--train-epochs", type=int, default=0)
     ap.add_argument("--out", default=None, help="plan JSON (default: stdout)"); ap.add_argument("--shell", default=None)
     ap.add_argument("--top-a", type=int, default=1024); ap.add_argument("--rollouts", type=int, default=1024)
@@ -67,19 +113,26 @@ def main(argv=None) -> dict:
     ap.add_argument("--max-steps", type=int, default=None,
                     help="cap on the number of reversions (default: every candidate may be reverted); a capped plan that "
                          "leaves improving candidates is marked truncated and is not auto-approvable")
+    ap.add_argument("--shell-dir", default=None, help="write DIR/<host>.sh per --trace HOST=PATH")
     ap.add_argument("--device", default="cuda")
     a = ap.parse_args(argv)
+    traces = parse_traces(a.trace)
+    check_outputs(traces, a.shell, a.shell_dir)
+    hosts = [h for h, _ in traces] if len(traces) > 1 else None     # host fields only with several sources
     if not torch.cuda.is_available():
         raise SystemExit("nerrf_b200.undo needs a CUDA device (no CPU fallback for the hot path)")
     log = lambda *m: print(*m, file=sys.stderr)
     t0 = time.perf_counter()
-    g, seq, lengths, nodes, n_events = load_trace(a.trace, a.device)
+    if hosts is None:
+        g, seq, lengths, nodes, n_events = load_trace(traces[0][1], a.device)
+    else:
+        g, seq, lengths, nodes, n_events = load_hosts([p for _, p in traces], a.device)
     t_ingest = (time.perf_counter() - t0) * 1e3
     model, scorer = load_models(a.weights, a.train_epochs, log=log)
     model.to(a.device); scorer.to(a.device)
     res = pipeline.run(g, seq, lengths, nodes, model, scorer, top_a=min(a.top_a, 4096), n_rollouts=a.rollouts, depth=a.depth,
                        iterations=a.iterations, plan_steps=a.max_steps, device=a.device)
-    plan = emit.from_pipeline(g, res, attack_id=a.id)
+    plan = emit.from_pipeline(g, res, attack_id=a.id, host_names=hosts)
     plan["stats"] = {"events": int(n_events), "nodes": int(g.num_nodes), "edges": int(g.num_edges),
                      "candidates": int(len(res.candidates)), "ingest_ms": t_ingest,
                      "timings_ms": {k: float(v) for k, v in res.timings_ms.items()}}
@@ -92,6 +145,11 @@ def main(argv=None) -> dict:
     if a.shell:
         with open(a.shell, "w") as f:
             f.write(emit.to_shell(plan))
+    if a.shell_dir:
+        os.makedirs(a.shell_dir, exist_ok=True)
+        for h, _ in traces:
+            with open(os.path.join(a.shell_dir, emit.check_host_name(h) + ".sh"), "w") as f:
+                f.write(emit.to_shell(plan, host=h if hosts else None))
     log(f"{n_events} events -> {g.num_nodes} nodes / {g.num_edges} edges -> {len(plan['steps'])} reversions "
         f"(ingest {t_ingest:.1f} ms, hot path {res.timings_ms['total']:.1f} ms)")
     return plan
