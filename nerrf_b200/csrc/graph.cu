@@ -96,6 +96,13 @@ __global__ void csr_empty_kernel(RP* rowptr, int64_t N) {
 // graph.py graph_from_events (node schema: docs/content/docs/architecture.mdx:144-160, threat-model.mdx:154-184).
 // Pass 1 over events: integer atomics only (event-kind counts, byte sums, first/last touch time as ordered int64,
 // path flag bits, degree) -> deterministic.  Pass 2 over nodes: the 20 used feature columns in double, rounded once.
+//
+// An event's byte count is the count argument of write(2) as traced at syscall entry: the traced process picks it, up to
+// 2^64 - 1.  Every feature reads it as uint64 clamped to Linux's per-call transfer cap MAX_RW_COUNT (graph.py
+// MAX_RW_COUNT), so a node's sum of fewer than 2^29 events stays below 2^60: exact in uint64, converted to double once.
+constexpr unsigned long long kMaxRwCount = 0x7ffff000ull;
+
+__device__ __forceinline__ unsigned long long clamp_rw(uint64_t b) { return b < kMaxRwCount ? b : kMaxRwCount; }
 struct NodeAcc {            // 64 bytes per node
     int32_t cnt[8];
     unsigned long long bytes;
@@ -139,7 +146,7 @@ __global__ void __launch_bounds__(256) node_acc_events_kernel(const int32_t* __r
         }
         const long long tb = __double_as_longlong(ti + 0.0);
         const int s = slot[i];
-        const unsigned long long sz = bytes[i];
+        const unsigned long long sz = clamp_rw(bytes[i]);
         touch(acc, p, s, sz, tb, 1);
         touch(acc, f, s, sz, tb, g >= 0 ? 2 : 1);
         if (g >= 0) touch(acc, g, s, sz, tb, 1);
@@ -219,7 +226,7 @@ __global__ void __launch_bounds__(256) trace_sequences_kernel(const int64_t* __r
         const int sl = slot[si];
 #pragma unroll
         for (int j = 0; j < 8; ++j) row[j] = (j == sl) ? 1.f : 0.f;
-        row[8] = (float)(log1p((double)bytes[si]) / 20.0);
+        row[8] = (float)(log1p((double)clamp_rw((uint64_t)bytes[si])) / 20.0);   // the wire's uint64, stored as int64
         row[9] = (float)dt;
         row[10] = (float)((t - t0) / span);
         const int pf = pflags[si];

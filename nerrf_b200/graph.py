@@ -25,6 +25,14 @@ import numpy as np
 F_IN = 32          # padded node feature width (SURVEY.md 8a a1)
 TAU = 30.0         # seconds
 WINDOW = 60.0      # seconds
+# Linux's cap on what one read / write can transfer.  An event's byte count is the count ARGUMENT of write(2), traced
+# before the call fails, so the traced process can put any uint64 there; every feature clamps it to this first.
+MAX_RW_COUNT = 0x7ffff000
+
+
+def clamp_bytes(size) -> int:
+    """An event's byte count as the features see it: the wire's uint64 clamped to MAX_RW_COUNT (a Python int)."""
+    return min(int(size or 0), MAX_RW_COUNT)
 
 
 @dataclass
@@ -281,11 +289,11 @@ def graph_from_events(events, merge_renames=True, window=None, observable=False)
             src += [f, g]; dst += [g, f]; tt += [t, t]
             touched.append(g)
         for n in touched:
-            fv = feats.setdefault(n, {"cnt": np.zeros(_N_EVENT_SLOTS), "bytes": 0.0, "first": t, "last": t,
+            fv = feats.setdefault(n, {"cnt": np.zeros(_N_EVENT_SLOTS), "bytes": 0, "first": t, "last": t,
                                        "lockbit": 0.0, "note": 0.0, "tmp": 0.0})
             slot = _EVENT_SLOT.get(e["event"], _N_EVENT_SLOTS - 1)
             fv["cnt"][OBSERVABLE_SLOT[slot] if observable else slot] += 1
-            fv["bytes"] += float(e.get("size", 0) or 0)
+            fv["bytes"] += clamp_bytes(e.get("size", 0))      # an exact integer sum, converted to float once below
             fv["last"] = t
         fv = feats[f]
         fv["lockbit"] = max(fv["lockbit"], 1.0 if ".lockbit" in path or (merge_renames and ".lockbit" in new_path) else 0.0)
@@ -315,7 +323,7 @@ def graph_from_events(events, merge_renames=True, window=None, observable=False)
         x[n, 1] = 1.0 if kinds[n] == 1 else 0.0         # process   (x[:,2] = socket, unused here)
         x[n, 3] = math.log1p(indeg[n]); x[n, 4] = math.log1p(outdeg[n])
         x[n, 5:5 + _N_EVENT_SLOTS] = np.log1p(fv["cnt"])
-        x[n, 13] = math.log1p(fv["bytes"]) / 20.0
+        x[n, 13] = math.log1p(float(fv["bytes"])) / 20.0
         x[n, 14] = (fv["last"] - fv["first"]) / window   # temporal delta
         x[n, 15] = fv["first"] / window
         x[n, 16] = fv["lockbit"]; x[n, 17] = fv["note"]; x[n, 18] = fv["tmp"]
@@ -328,7 +336,7 @@ def graph_from_events(events, merge_renames=True, window=None, observable=False)
     for n in range(N):
         c = feats[n]["cnt"]
         k = max(c[0] + c[1] + c[2], 1.0)
-        size_mb[n] = feats[n]["bytes"] / k / 1e6 if kinds[n] == 0 else 0.0
+        size_mb[n] = float(feats[n]["bytes"]) / k / 1e6 if kinds[n] == 0 else 0.0
     file_keys = {k[1]: v for k, v in node_id.items() if k[0] == "f"}      # merge key (or path) -> node, incl. rename aliases
     return TemporalGraph(rowptr, col, ew, x, {"kind": "trace", "names": names, "node_kind": np.asarray(kinds),
                                               "label": y, "size_mb": size_mb, "t0": t0, "span": span,

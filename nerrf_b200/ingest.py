@@ -263,7 +263,7 @@ def graph_from_columns(cols: EventColumns, merge_renames=True, window=None, devi
     t = ts[order] - t0
     raw_slot = cols.event_slot[order].astype(np.int64)
     slot = np.asarray(G.OBSERVABLE_SLOT, np.int64)[raw_slot] if observable else raw_slot
-    size = cols.bytes[order].astype(np.float64)
+    size = np.minimum(cols.bytes[order], np.uint64(G.MAX_RW_COUNT)).astype(np.int64)
     pf = cols.path_flags[order]
     if merge_renames:                                         # the renamed twin is this node: its .lockbit bit counts
         pf = pf | (path_flags_of(*cols.strings["new_path"])[order] & np.uint8(1))
@@ -300,7 +300,9 @@ def graph_from_columns(cols: EventColumns, merge_renames=True, window=None, devi
     tn = np.concatenate([P, F, Gn[has_g]]); tslot = np.concatenate([slot, slot, slot[has_g]])
     tsize = np.concatenate([size, size, size[has_g]]); ttime = np.concatenate([t, t, t[has_g]])
     cnt = np.bincount(tn * G._N_EVENT_SLOTS + tslot, minlength=N * G._N_EVENT_SLOTS).reshape(N, G._N_EVENT_SLOTS).astype(np.float64)
-    nbytes = np.bincount(tn, weights=tsize, minlength=N)
+    nbytes = np.zeros(N, np.int64)
+    np.add.at(nbytes, tn, tsize)                              # exact: < 2^29 events of < 2^31 bytes each
+    nbytes = nbytes.astype(np.float64)
     first = np.full(N, np.inf); last = np.full(N, -np.inf)
     np.minimum.at(first, tn, ttime); np.maximum.at(last, tn, ttime)
     flag = lambda bit: (np.bincount(F[(pf & bit) != 0], minlength=N) > 0).astype(np.float64)
@@ -373,7 +375,7 @@ def sequences_core(cols: EventColumns, order, F, tt, t0, span, n_nodes, t_max=No
     if observable:
         slot = np.asarray(G.OBSERVABLE_SLOT, np.int64)[slot]
     seq[row, k, slot] = 1.0
-    seq[row, k, 8] = np.log1p(cols.bytes[order][ev].astype(np.float64)) / 20.0
+    seq[row, k, 8] = np.log1p(np.minimum(cols.bytes[order][ev], np.uint64(G.MAX_RW_COUNT)).astype(np.float64)) / 20.0
     prev_t = np.empty(n); prev_t[1:] = tt[by_file][:-1]; prev_t[0] = 0.0
     dt = np.minimum(tt[by_file] - prev_t, 10.0)
     dt[(pos == keep_from)] = 0.0                          # first kept event of a file has no predecessor in the window

@@ -54,7 +54,7 @@ def file_sequences(events, g: G.TemporalGraph, t_max=lstm.T_MAX, observable=Fals
             t = G._parse_ts(e["timestamp"])
             slot = _SEQ_EVENT_SLOT.get(e["event"], 7)
             seq[i, k, G.OBSERVABLE_SLOT[slot] if observable else slot] = 1.0
-            seq[i, k, 8] = np.log1p(float(e.get("size", 0) or 0)) / 20.0
+            seq[i, k, 8] = np.log1p(float(G.clamp_bytes(e.get("size", 0)))) / 20.0
             seq[i, k, 9] = min(t - prev, 10.0) if prev is not None else 0.0
             seq[i, k, 10] = (t - t0) / span
             seq[i, k, 11] = 1.0 if ".lockbit" in e["path"] else 0.0

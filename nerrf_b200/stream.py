@@ -729,7 +729,10 @@ class DeviceStream:
         if perm is None:
             raise _lib.NerrfError("sequences_device needs a merge-mode window graph (two edges per event)")
         lo, hi = g.meta["window_ranks"]
-        cand = torch.as_tensor(np.asarray(only_nodes, np.int64)).to(self.dev)
+        only_nodes = np.asarray(only_nodes, np.int64).reshape(-1)
+        if only_nodes.size and (only_nodes.min() < 0 or only_nodes.max() >= g.num_nodes):   # the kernel reads rowptr[f], rowptr[f + 1]
+            raise _lib.NerrfError("sequences_device: candidate node ids must lie in [0, %d)" % g.num_nodes)
+        cand = torch.as_tensor(only_nodes).to(self.dev)
         A = int(cand.shape[0])
         seq = torch.empty(A, lstm.T_MAX, lstm.D_IN, dtype=torch.float32, device=self.dev)
         ln = torch.empty(A, dtype=torch.int32, device=self.dev)
