@@ -142,6 +142,50 @@ int nerrf_sage_layer_bwd(const float* h_in, const float* m, const float* y, cons
                          float* dh, float* dW, float* db, float* workspace, size_t workspace_bytes,
                          int64_t n_nodes, int F, int H, int relu, nerrf_stream_t stream);
 
+/* nerrf_sage_layer_bwd with the edge-weight gradient (node explanations, nerrf_b200.explain; DESIGN.md 1.1.1).  d_ew
+ * [E] != NULL ACCUMULATES this layer's term of d(out)/d(ew) in CSR-by-destination order (rowptr [n+1], int32 or int64
+ * when rowptr_is64; col, ew [E]: the graph the forward read):
+ *     d_ew[e] += dZ[dst(e), F:] . (h_in[src(e)] - [S >= 1e-12] m[dst(e)]) / max(S, 1e-12),   S = sum of dst(e)'s weights
+ * with S summed as nerrf_sage_aggregate sums it ([S >= 1e-12] is the gradient of torch's clamp_min) and h - m taken as
+ * (h - r) - (m - r) against r = h_in of the row's first source (exactly 0 when a row's sources are one node).  One warp
+ * per destination row, no atomics: bit-reproducible.  d_ew needs h_in and rowptr (col / ew / d_ew may be NULL when the
+ * graph has no edges).  nerrf_sage_layer_bwd is this call with d_ew = NULL. */
+int nerrf_sage_layer_bwd_ex(const float* h_in, const float* m, const float* y, const float* dy, const float* W,
+                            const void* t_rowptr, int t_rowptr_is64, const int32_t* t_col, const float* t_w,
+                            float* dh, float* dW, float* db, float* workspace, size_t workspace_bytes,
+                            int64_t n_nodes, int F, int H, int relu, const void* rowptr, int rowptr_is64,
+                            const int32_t* col, const float* ew, float* d_ew, nerrf_stream_t stream);
+
+/* ------------------------------------------------------------------ node explanations (DESIGN.md 1.1.1)
+ * Receptive-field extraction: for each of n_targets target nodes (int32 ids into a CSR-by-destination graph of n_nodes
+ * nodes), its `hops`-hop in-neighbourhood: every node within distance <= hops - 1 keeps ALL its in-edges (in their
+ * original order), nodes at distance hops keep none (their features only).  The result is one block-diagonal batched
+ * CSR, the targets' blocks in target order, each block's nodes in ascending global id.
+ *   _count: counts [2 * n_targets] = (nodes, edges) per target; (-1, -1) when its kept edges exceed max_edges.
+ *   _fill:  for targets that fit (pass only those), with node_off / edge_off [n_targets] their blocks' first node / edge:
+ *           out_rowptr [total nodes + 1] (int64), out_col [total edges] (int32, batched node ids), out_ew, out_epos (int64:
+ *           the edge's CSR position in the input graph), out_node [total nodes] (global id of each batched node), out_x
+ *           [total nodes, F_in] (the node features), out_target [n_targets] (each target's batched node id).
+ * Deterministic (the output is a function of the graph and the targets).  workspace: nerrf_explain_subgraph_workspace_bytes,
+ * max_edges in [0, 2^28); hops in 1..16.  All pointers device. */
+int nerrf_explain_subgraph_workspace_bytes(int64_t n_targets, int64_t max_edges, size_t* bytes);
+int nerrf_explain_subgraph_count(const void* rowptr, int rowptr_is64, const int32_t* col, int64_t n_nodes,
+                                 const int32_t* targets, int64_t n_targets, int hops, int64_t max_edges,
+                                 int64_t* counts, void* workspace, size_t workspace_bytes, nerrf_stream_t stream);
+int nerrf_explain_subgraph_fill(const void* rowptr, int rowptr_is64, const int32_t* col, const float* ew,
+                                const float* x, int F_in, int64_t n_nodes, const int32_t* targets, int64_t n_targets,
+                                int hops, int64_t max_edges, const int64_t* node_off, const int64_t* edge_off,
+                                int64_t* out_rowptr, int32_t* out_col, float* out_ew, int64_t* out_epos,
+                                int32_t* out_node, float* out_x, int32_t* out_target, void* workspace,
+                                size_t workspace_bytes, nerrf_stream_t stream);
+/* Segmented top-k: per segment t (edges [seg[t], seg[t+1]) of a batched graph), the k edges of largest
+ * |a_e| = |ew[e] * d_ew[e]|, ties to the lower index, in that order: out_edge [n_seg, k] (batched edge index, -1 past the
+ * segment's end), out_attr (a_e), out_pos (epos[e], or e when epos is NULL) and, when out_event != NULL, out_event =
+ * edge_event[out_pos] (-1 when edge_event is NULL or the pick is empty).  One CTA per segment, k in 1..1024. */
+int nerrf_explain_topk(const int64_t* seg, int64_t n_seg, const float* ew, const float* d_ew, const int64_t* epos,
+                       const int64_t* edge_event, int k, int64_t* out_edge, float* out_attr, int64_t* out_pos,
+                       int64_t* out_event, nerrf_stream_t stream);
+
 /* The normalised edge weights of the graph, for t_w above: a[e] = ew[e] * (1 / max(weight sum of e's destination row,
  * 1e-12)), edges in CSR-by-destination order (rowptr [n+1], int32 or int64 when rowptr_is64; ew, a [E]).  The weight sum
  * is taken in the order nerrf_sage_aggregate takes it, so the entries are the forward's to the bit.  No atomics:

@@ -32,6 +32,14 @@ SIGNATURES = {
     "nerrf_sage_layer_bwd": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, C.c_size_t, C.c_int64, C.c_int,
                                        C.c_int, C.c_int, vp]),
     "nerrf_sage_norm_weights": (C.c_int, [vp, C.c_int, vp, vp, C.c_int64, vp]),
+    "nerrf_sage_layer_bwd_ex": (C.c_int, [vp, vp, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, C.c_size_t, C.c_int64,
+                                          C.c_int, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp]),
+    "nerrf_explain_subgraph_workspace_bytes": (C.c_int, [C.c_int64, C.c_int64, C.POINTER(C.c_size_t)]),
+    "nerrf_explain_subgraph_count": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, C.c_int64, C.c_int, C.c_int64, vp, vp,
+                                               C.c_size_t, vp]),
+    "nerrf_explain_subgraph_fill": (C.c_int, [vp, C.c_int, vp, vp, vp, C.c_int, C.c_int64, vp, C.c_int64, C.c_int, C.c_int64,
+                                              vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]),
+    "nerrf_explain_topk": (C.c_int, [vp, C.c_int64, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]),
     "nerrf_sage_edge_head_bwd_workspace_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "nerrf_sage_edge_head_bwd": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, C.c_size_t,
                                            C.c_int64, C.c_int, vp]),

@@ -68,8 +68,34 @@ def restore_dir_step(directory: str, covered_paths) -> dict:
     return r
 
 
+def evidence_fields(ex, host_names=None) -> dict:
+    """The plan fields of one node's explanation (pipeline.PipelineResult.evidence[node]): "evidence" = one entry per
+    attributed edge, strongest first -- {"event": {"time", "pid", "syscall", "path"[, "host"]}, "src", "dst" (the edge's
+    two node names), "attribution"} -- and "evidence_logit"; or "evidence": None with "evidence_reason" when the node
+    was not explained.  host_names: source id -> host name (several sources).  Names and paths come from the trace:
+    a control character in any of them flags the step "hostile_name", as for the step's own path."""
+    if ex.get("scope") is None:
+        return {"evidence": None, "evidence_reason": str(ex.get("reason", ""))}
+    out, hostile = [], False
+    for e in ex["edges"]:
+        ev = e.get("event")
+        rec = None
+        if ev is not None:
+            rec = {"time": float(ev["time"]), "pid": int(ev["pid"]), "syscall": str(ev["syscall"]), "path": str(ev["path"])}
+            if host_names is not None and "source" in ev:
+                rec["host"] = check_host_name(host_names[int(ev["source"])])
+            hostile = hostile or _has_control_chars(rec["path"]) or _has_control_chars(rec["syscall"])
+        src, dst = str(e.get("src_name", e["src"])), str(e.get("dst_name", e["dst"]))
+        hostile = hostile or _has_control_chars(src) or _has_control_chars(dst)
+        out.append({"event": rec, "src": src, "dst": dst, "attribution": float(e["attr"])})
+    r = {"evidence": out, "evidence_logit": float(ex["logit"])}
+    if hostile:
+        r["hostile_name"] = True
+    return r
+
+
 def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node_score=None, truncated=False,
-              remaining_candidates=0, restores=None, hosts=None) -> dict:
+              remaining_candidates=0, restores=None, hosts=None, evidence=None, host_names=None) -> dict:
     """names: node id -> path (TemporalGraph.meta['names']); plan_nodes: node ids to revert, in plan order
     (PipelineResult.plan_nodes); scores: Plan.scores (exact reward after each commit, scores[0] = before).
     truncated / remaining_candidates: the planner stopped at its step limit while improving candidates remained --
@@ -77,7 +103,9 @@ def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node
     restores: PipelineResult.restores -- directory restores, each at its position in the plan ({"position", "dir",
     "covers": node ids}); the node steps fill the other positions in order.
     hosts: node id -> host name, for a graph of several sources: every step gets the "host" it applies to (a restore:
-    the host of the files it covers; covers on two hosts raise ValueError).  None: no host fields (one source)."""
+    the host of the files it covers; covers on two hosts raise ValueError).  None: no host fields (one source).
+    evidence: node id -> explanation (pipeline.PipelineResult.evidence): each node step found there gets the fields of
+    evidence_fields (host_names: source id -> host name for its events).  None: no evidence fields."""
     host_of = (lambda n: check_host_name(hosts[int(n)])) if hosts is not None else None
     at = {int(r["position"]): r for r in (restores or [])}
     total = len(plan_nodes) + len(at)
@@ -107,6 +135,8 @@ def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node
             step["anomaly_score"] = float(node_score[n])
         if scores is not None and k + 1 < len(scores):
             step["reward_after"] = float(scores[k + 1])
+        if evidence is not None and evidence.get(n) is not None:
+            step.update(evidence_fields(evidence[n], host_names))
         steps.append(step)
     out = {"version": PLAN_VERSION, "kind": "nerrf.undo_plan", "attack_id": attack_id, "steps": steps,
            "approve_if": "all_checks_pass" if not truncated else "all_checks_pass_and_operator_confirms_partial_plan",
@@ -155,4 +185,5 @@ def from_pipeline(g, result, attack_id=None, host_names=None) -> dict:
     return undo_plan(g.meta["names"], result.plan_nodes, scores=result.plan.scores, attack_id=attack_id,
                      size_mb=g.meta.get("size_mb"), node_score=score, truncated=getattr(result.plan, "truncated", False),
                      remaining_candidates=getattr(result.plan, "remaining_candidates", 0),
-                     restores=getattr(result, "restores", None), hosts=hosts)
+                     restores=getattr(result, "restores", None), hosts=hosts,
+                     evidence=getattr(result, "evidence", None), host_names=host_names)

@@ -18,6 +18,8 @@
 //                        (4 x 8 per thread) and writes a partial; slab 0 also accumulates db
 //   sage_bwd_reduce_kernel  partials -> dW / db, chunk order fixed
 //   sage_bwd_dh_kernel   one warp per source row: dZ[u, :F] + gather of dZ[dst, F:] over the transposed row
+//   sage_bwd_dew_kernel  one warp per destination row: the edge-weight gradient d_ew (nerrf_sage_layer_bwd_ex; node
+//                        explanations, nerrf_b200.explain)
 //   sage_norm_weights_kernel  one warp per destination row: a_e = w_e / max(row weight sum, 1e-12), the weight sum taken in
 //                        gather_row's lane order and warp_sum, so A^T holds the forward aggregate's A entries to the bit
 #include "common.cuh"
@@ -202,6 +204,63 @@ __global__ void __launch_bounds__(256) sage_bwd_dh_kernel(const float* __restric
     }
 }
 
+// d_ew[e] += dZ[u, F:] . (h[src(e)] - [S_u >= 1e-12] m_u) / max(S_u, 1e-12) for every edge e of destination row u: the
+// derivative of this layer's output w.r.t. the edge weight (the derivative of m_u = sum_e w_e h_src / max(S_u, 1e-12)).
+// One warp per row, no atomics (each edge belongs to one row).  S_u is summed in gather_row's lane order and warp_sum, so
+// it is the forward's S_u to the bit.  The differences are taken against r = h[src(first edge)]:
+//     h_src - m = (h_src - r) - (m - r),   m - r = sum_e w_e (h_src(e) - r) / max(S, 1e-12)
+// so a row whose sources are one node (a file written by one process, event after event) gets exactly 0 instead of the
+// fp32 rounding of h - m / S amplified by 1 / S.  dZ[u, F:] is read once; G = 32 / LPR edges per step get one LPR-lane
+// dot product each.
+template <int F, typename RP>
+__global__ void __launch_bounds__(256) sage_bwd_dew_kernel(const float* __restrict__ dz, const float* __restrict__ h,
+                                                           const RP* __restrict__ rowptr, const int32_t* __restrict__ col,
+                                                           const float* __restrict__ ew, float* __restrict__ d_ew, int64_t n) {
+    constexpr int LPR = F / 4;
+    constexpr int G = 32 / LPR;
+    const int lane = threadIdx.x & 31;
+    const int64_t row = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (row >= n) return;
+    const int64_t e0 = rowptr[row], e1 = rowptr[row + 1];
+    if (e1 <= e0) return;
+    float wpart = 0.f;
+    for (int64_t e = e0 + lane; e < e1; e += 32) wpart += __ldg(ew + e);
+    const float wsum = warp_sum(wpart);
+    const float inv = 1.0f / fmaxf(wsum, 1e-12f);
+    const int g = lane / LPR, sub = lane % LPR;
+    const float4 r = ldg4(h + (int64_t)__ldg(col + e0) * F + 4 * sub);
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);                       // sum_e w_e (h_src(e) - r), this lane's group's edges
+    for (int64_t e = e0 + g; e < e1; e += G) {
+        const float w = __ldg(ew + e);
+        const float4 v = ldg4(h + (int64_t)__ldg(col + e) * F + 4 * sub);
+        acc.x = fmaf(w, v.x - r.x, acc.x); acc.y = fmaf(w, v.y - r.y, acc.y);
+        acc.z = fmaf(w, v.z - r.z, acc.z); acc.w = fmaf(w, v.w - r.w, acc.w);
+    }
+#pragma unroll
+    for (int o = LPR; o < 32; o <<= 1) {
+        acc.x += __shfl_xor_sync(0xffffffffu, acc.x, o); acc.y += __shfl_xor_sync(0xffffffffu, acc.y, o);
+        acc.z += __shfl_xor_sync(0xffffffffu, acc.z, o); acc.w += __shfl_xor_sync(0xffffffffu, acc.w, o);
+    }
+    const float4 d = ldg4(dz + row * (2 * F) + F + 4 * sub);
+    // c = dZ . (m - r) when the gradient of max(S, 1e-12) passes ([S >= 1e-12], torch clamp_min); else -dZ . r, so that
+    // p - c below is dZ . h_src either way
+    float c = (wsum >= 1e-12f) ? (d.x * (acc.x * inv) + d.y * (acc.y * inv) + d.z * (acc.z * inv) + d.w * (acc.w * inv))
+                               : -(d.x * r.x + d.y * r.y + d.z * r.z + d.w * r.w);
+#pragma unroll
+    for (int o = 1; o < LPR; o <<= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+    for (int64_t base = e0; base < e1; base += G) {
+        const int64_t e = base + g;
+        float p = 0.f;
+        if (e < e1) {
+            const float4 v = ldg4(h + (int64_t)__ldg(col + e) * F + 4 * sub);
+            p = d.x * (v.x - r.x) + d.y * (v.y - r.y) + d.z * (v.z - r.z) + d.w * (v.w - r.w);
+        }
+#pragma unroll
+        for (int o = 1; o < LPR; o <<= 1) p += __shfl_xor_sync(0xffffffffu, p, o);
+        if (sub == 0 && e < e1) d_ew[e] += (p - c) * inv;
+    }
+}
+
 // a[e] = ew[e] * (1 / max(sum of the row's weights, 1e-12)) over the CSR-by-destination rows: lane l sums edges e0 + l,
 // e0 + l + 32, ... then warp_sum, exactly as gather_row sums the weights it normalises by
 template <typename RP>
@@ -239,7 +298,7 @@ BwdPlan bwd_plan(int64_t n, int F) {
 template <int F>
 int launch_bwd(const float* h, const float* m, const float* y, const float* dy, const float* W, const void* t_rowptr, int is64,
                const int32_t* t_col, const float* t_w, float* dh, float* dW, float* db, float* ws, int64_t n, int relu,
-               cudaStream_t st) {
+               const void* rowptr, int rp64, const int32_t* col, const float* ew, float* d_ew, cudaStream_t st) {
     const BwdPlan p = bwd_plan(n, F);
     float* dz = ws;
     float* part = reinterpret_cast<float*>(reinterpret_cast<unsigned char*>(ws) + p.dz_bytes);
@@ -251,12 +310,18 @@ int launch_bwd(const float* h, const float* m, const float* y, const float* dy, 
         sage_bwd_reduce_kernel<<<(2 * F * HB + 255) / 256, 256, 0, st>>>(part, dW, 2 * F * HB, p.chunks);
         sage_bwd_reduce_kernel<<<1, 256, 0, st>>>(dbpart, db, HB, p.chunks);
     }
+    if (dh || d_ew) sage_bwd_dz_kernel<F><<<(unsigned)((n + DZ_BM - 1) / DZ_BM), 256, DZ_SMEM, st>>>(dy, y, W, dz, n, relu);
     if (dh) {
-        sage_bwd_dz_kernel<F><<<(unsigned)((n + DZ_BM - 1) / DZ_BM), 256, DZ_SMEM, st>>>(dy, y, W, dz, n, relu);
         if (is64)
             sage_bwd_dh_kernel<F, int64_t><<<(unsigned)((n + 7) / 8), 256, 0, st>>>(dz, (const int64_t*)t_rowptr, t_col, t_w, dh, n);
         else
             sage_bwd_dh_kernel<F, int32_t><<<(unsigned)((n + 7) / 8), 256, 0, st>>>(dz, (const int32_t*)t_rowptr, t_col, t_w, dh, n);
+    }
+    if (d_ew) {
+        if (rp64)
+            sage_bwd_dew_kernel<F, int64_t><<<(unsigned)((n + 7) / 8), 256, 0, st>>>(dz, h, (const int64_t*)rowptr, col, ew, d_ew, n);
+        else
+            sage_bwd_dew_kernel<F, int32_t><<<(unsigned)((n + 7) / 8), 256, 0, st>>>(dz, h, (const int32_t*)rowptr, col, ew, d_ew, n);
     }
     return launch_status("sage layer backward");
 }
@@ -274,10 +339,11 @@ extern "C" int nerrf_sage_layer_bwd_workspace_bytes(int64_t n_nodes, int F, size
     return NERRF_OK;
 }
 
-extern "C" int nerrf_sage_layer_bwd(const float* h_in, const float* m, const float* y, const float* dy, const float* W,
-                                    const void* t_rowptr, int t_rowptr_is64, const int32_t* t_col, const float* t_w,
-                                    float* dh, float* dW, float* db, float* workspace, size_t workspace_bytes,
-                                    int64_t n_nodes, int F, int H, int relu, nerrf_stream_t stream) {
+extern "C" int nerrf_sage_layer_bwd_ex(const float* h_in, const float* m, const float* y, const float* dy, const float* W,
+                                       const void* t_rowptr, int t_rowptr_is64, const int32_t* t_col, const float* t_w,
+                                       float* dh, float* dW, float* db, float* workspace, size_t workspace_bytes,
+                                       int64_t n_nodes, int F, int H, int relu, const void* rowptr, int rowptr_is64,
+                                       const int32_t* col, const float* ew, float* d_ew, nerrf_stream_t stream) {
     NERRF_REQUIRE(H == HB, "hidden width must be 128 (got %d)", H);
     NERRF_REQUIRE(F == 32 || F == 64 || F == 128, "F must be 32, 64 or 128 (got %d)", F);
     NERRF_REQUIRE(n_nodes >= 0, "negative node count");
@@ -285,6 +351,8 @@ extern "C" int nerrf_sage_layer_bwd(const float* h_in, const float* m, const flo
     NERRF_REQUIRE(!relu || y, "the ReLU mask needs the layer output y");
     NERRF_REQUIRE(!dW || (h_in && m && db), "dW needs h_in, m and db");
     NERRF_REQUIRE(!dh || t_rowptr, "dh needs the transposed graph");     // t_col / t_w may be null when the graph has no edges
+    NERRF_REQUIRE(!d_ew || (h_in && rowptr), "d_ew needs h_in and the graph");   // col / ew / d_ew null: no edges
+    NERRF_REQUIRE(n_nodes / 8 < (1ll << 31), "too many nodes");
     size_t need = 0;
     nerrf_sage_layer_bwd_workspace_bytes(n_nodes, F, &need);
     if (workspace_bytes < need) {
@@ -303,10 +371,21 @@ extern "C" int nerrf_sage_layer_bwd(const float* h_in, const float* m, const flo
     }
     cudaStream_t st = (cudaStream_t)stream;
     switch (F) {
-        case 32: return launch_bwd<32>(h_in, m, y, dy, W, t_rowptr, t_rowptr_is64, t_col, t_w, dh, dW, db, workspace, n_nodes, relu, st);
-        case 64: return launch_bwd<64>(h_in, m, y, dy, W, t_rowptr, t_rowptr_is64, t_col, t_w, dh, dW, db, workspace, n_nodes, relu, st);
-        default: return launch_bwd<128>(h_in, m, y, dy, W, t_rowptr, t_rowptr_is64, t_col, t_w, dh, dW, db, workspace, n_nodes, relu, st);
+        case 32: return launch_bwd<32>(h_in, m, y, dy, W, t_rowptr, t_rowptr_is64, t_col, t_w, dh, dW, db, workspace, n_nodes, relu,
+                                       rowptr, rowptr_is64, col, ew, d_ew, st);
+        case 64: return launch_bwd<64>(h_in, m, y, dy, W, t_rowptr, t_rowptr_is64, t_col, t_w, dh, dW, db, workspace, n_nodes, relu,
+                                       rowptr, rowptr_is64, col, ew, d_ew, st);
+        default: return launch_bwd<128>(h_in, m, y, dy, W, t_rowptr, t_rowptr_is64, t_col, t_w, dh, dW, db, workspace, n_nodes, relu,
+                                        rowptr, rowptr_is64, col, ew, d_ew, st);
     }
+}
+
+extern "C" int nerrf_sage_layer_bwd(const float* h_in, const float* m, const float* y, const float* dy, const float* W,
+                                    const void* t_rowptr, int t_rowptr_is64, const int32_t* t_col, const float* t_w,
+                                    float* dh, float* dW, float* db, float* workspace, size_t workspace_bytes,
+                                    int64_t n_nodes, int F, int H, int relu, nerrf_stream_t stream) {
+    return nerrf_sage_layer_bwd_ex(h_in, m, y, dy, W, t_rowptr, t_rowptr_is64, t_col, t_w, dh, dW, db, workspace, workspace_bytes,
+                                   n_nodes, F, H, relu, nullptr, 0, nullptr, nullptr, nullptr, stream);
 }
 
 extern "C" int nerrf_sage_norm_weights(const void* rowptr, int rowptr_is64, const float* ew, float* a, int64_t n_nodes,

@@ -263,11 +263,11 @@ def graph_from_events(events, merge_renames=True, window=None, observable=False)
             node_id[key] = len(names); names.append(name); kinds.append(kind)
         return node_id[key]
 
-    src, dst, tt = [], [], []
+    src, dst, tt, eid = [], [], [], []
     feats: dict = {}
     labels: dict = {}
     attack_pairs: set = set()          # (process, file) pairs with an ATTACK_EVENTS event of that process on that file
-    for e in evs:
+    for i_ev, e in enumerate(evs):
         t = _parse_ts(e["timestamp"]) - t0
         p = nid(("p", e["pid"]), 1, f"pid:{e['pid']}")
         path = e["path"]
@@ -275,7 +275,7 @@ def graph_from_events(events, merge_renames=True, window=None, observable=False)
         f = nid(key, 0, path)
         if path.endswith(".lockbit3"):
             names[f] = path                       # keep the encrypted name: the rollback target
-        src += [p, f]; dst += [f, p]; tt += [t, t]
+        src += [p, f]; dst += [f, p]; tt += [t, t]; eid += [i_ev, i_ev]
         touched = [p, f]
         new_path = e.get("new_path") or ""
         if new_path and merge_renames:
@@ -286,7 +286,7 @@ def graph_from_events(events, merge_renames=True, window=None, observable=False)
                 names[f] = new_path
         if new_path and not merge_renames:
             g = nid(("f", new_path), 0, new_path)
-            src += [f, g]; dst += [g, f]; tt += [t, t]
+            src += [f, g]; dst += [g, f]; tt += [t, t]; eid += [i_ev, i_ev]
             touched.append(g)
         for n in touched:
             fv = feats.setdefault(n, {"cnt": np.zeros(_N_EVENT_SLOTS), "bytes": 0, "first": t, "last": t,
@@ -338,10 +338,18 @@ def graph_from_events(events, merge_renames=True, window=None, observable=False)
         k = max(c[0] + c[1] + c[2], 1.0)
         size_mb[n] = float(feats[n]["bytes"]) / k / 1e6 if kinds[n] == 0 else 0.0
     file_keys = {k[1]: v for k, v in node_id.items() if k[0] == "f"}      # merge key (or path) -> node, incl. rename aliases
+    # edge_event: the event (index into the time-sorted, path-resolved events) that made each CSR edge
+    edge_event = np.asarray(eid, np.int64)[np.lexsort((tt, dst))]
     return TemporalGraph(rowptr, col, ew, x, {"kind": "trace", "names": names, "node_kind": np.asarray(kinds),
                                               "label": y, "size_mb": size_mb, "t0": t0, "span": span,
                                               "file_keys": file_keys, "merge_renames": bool(merge_renames),
-                                              "edge_label": edge_label})
+                                              "edge_label": edge_label, "edge_event": edge_event,
+                                              "event_info": lambda ids: [event_record(evs[int(i)]) for i in ids]})
+
+
+def event_record(e) -> dict:
+    """The fields of one event an explanation shows: time (seconds), pid, syscall, path (resolved)"""
+    return {"time": _parse_ts(e["timestamp"]), "pid": int(e["pid"]), "syscall": str(e["event"]), "path": str(e["path"])}
 
 
 def graph_from_jsonl(path, **kw) -> TemporalGraph:

@@ -113,6 +113,22 @@ def events_from_columns(cols: EventColumns) -> list:
              "pid": int(cols.pid[i]), "new_path": new_path[i]} for i in range(cols.n)]
 
 
+def column_event_records(cols: EventColumns, ids) -> list:
+    """graph.event_record of rows `ids` of `cols`, plus "source" when the columns carry one"""
+    ts = cols.timestamp
+    out = []
+    for i in np.asarray(ids, np.int64).tolist():
+        txt = {}
+        for name in ("syscall", "path"):
+            off, data = cols.strings[name]
+            txt[name] = bytes(data[off[i]:off[i + 1]]).decode("utf-8", "replace")
+        r = {"time": float(ts[i]), "pid": int(cols.pid[i]), "syscall": txt["syscall"], "path": txt["path"]}
+        if cols.source is not None:
+            r["source"] = int(cols.source[i])
+        out.append(r)
+    return out
+
+
 def _gather_strings(off, data, idx):
     """Packed string column restricted / re-ordered to rows `idx` (vectorised variable-length gather)."""
     ln = (off[idx + 1] - off[idx]).astype(np.int64)
@@ -288,8 +304,16 @@ def graph_from_columns(cols: EventColumns, merge_renames=True, window=None, devi
         x, label, size_mb = G.node_features_device(up(P, np.int32), up(F, np.int32), up(Gn, np.int32) if has_g.any() else None,
                                                    up(t, np.float64), up(slot, np.uint8), up(cols.bytes[order], np.int64),
                                                    up(pf, np.uint8), up(kind, np.int8), window)
-        rowptr, col, ew = G.build_csr_device(up(src, np.int32), up(dst, np.int32), up(tt, np.float32), up(conf, np.float32), N,
-                                             t_ref=float(span), tau=G.TAU)
+        rowptr, col, ew, perm = G.build_csr_device(up(src, np.int32), up(dst, np.int32), up(tt, np.float32), up(conf, np.float32),
+                                                   N, t_ref=float(span), tau=G.TAU, return_perm=True)
+
+        def edge_event(perm=perm, keep=keep, order=order, E=int(src.shape[0])):
+            """the event (row of the path-resolved columns) that made each CSR edge"""
+            if E == 0:                                                        # perm holds one spare entry
+                return torch.zeros(0, dtype=torch.int64, device=perm.device)
+            ev = up(np.repeat(order, 4)[keep], np.int64)                      # edge in constructor order -> event row
+            return ev[perm.long() & 0xffffffff]
+        meta.update(edge_event=edge_event, event_info=lambda ids, cols=cols: column_event_records(cols, ids))
         lab = label.cpu().numpy().astype(np.int64)
         if observable:                                        # the kernel saw the folded slots: labels come from the annotations
             lab = (np.bincount(F[(raw_slot == 1) | (raw_slot == 2)], minlength=N) > 0).astype(np.int64)

@@ -78,6 +78,8 @@ class PipelineResult:
     restores: list = field(default_factory=list)   # per APPLIED restore, in plan order: {"position": index in plan.actions,
                                                    # "dir": directory, "dir_hash": int, "covers": covered node ids}
     actions: Actions | None = None    # the action set the plan was made over (cand[i] is the node of action i)
+    evidence: dict | None = None      # run(explain=k): node id of each planned node step -> its explanation
+                                      # (explain.explain_nodes + explain.attach_events); None when not asked for
 
 
 @dataclass
@@ -251,7 +253,8 @@ def propose_restores(cand_dir, file_dir, file_size, file_is_cand, max_restores: 
 def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_model, top_a=1024, confidence=None,
         plan_steps=None, n_rollouts=4096, depth=50, iterations=16, device="cuda", exclude=None, commit_per_search=1,
         dist_ctx: DistContext | None = None, kill_candidates: bool = False, restore_candidates: bool = False,
-        max_restores: int = 4, min_restore_files: int = 8) -> PipelineResult:
+        max_restores: int = 4, min_restore_files: int = 8, explain: int = 0,
+        explain_max_edges: int | None = None, explain_max_full_graph: int | None = None) -> PipelineResult:
     """seq/lengths/seq_nodes: LSTM inputs for (a superset of) the candidate file nodes (file_sequences()).
     seq may instead be a CALLABLE nodes -> (seq, lengths, nodes_with_sequences): the sequences are then built only for
     the top-A candidates (large windows: a million file nodes, a few thousand candidates); seq_nodes = the file nodes.
@@ -265,9 +268,14 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
     directories holding the most candidate files (at least `min_restore_files`); a restore covers every candidate file of
     its directory and costs the directory's other files as collateral (planner spec v2, DESIGN.md 1.3).  Restores take
     the state-word-0 slots after the kills (kill budget 32 - restores).  res.plan_nodes lists node actions only;
-    res.restores lists the applied restores."""
+    res.restores lists the applied restores.
+    explain = k > 0: after planning, res.evidence holds each planned node's k strongest GraphSAGE-T edge attributions with
+    their events (nerrf_b200.explain; a kill step explains its process node, restores carry none).  The plan is the
+    plan of explain=0.  One GPU only."""
     if restore_candidates and dist_ctx is not None and dist_ctx.world > 1:
         raise NotImplementedError("restore candidates are planned on one GPU (dist_ctx.world > 1 is not supported)")
+    if explain and dist_ctx is not None and dist_ctx.world > 1:
+        raise NotImplementedError("explanations are computed on one GPU (dist_ctx.world > 1 is not supported)")
     dev = torch.device(device)
     tm = {}
     sync = torch.cuda.synchronize
@@ -394,4 +402,16 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
                 res.restores.append({"position": k, "dir": d, "dir_hash": int(r_dirs[i - n_kill]), "covers": [int(c) for c in covers]})
     if confidence is None and kill_candidates:
         res.kill_attribution = "writer" if edge_attack is None else "edges"
+    if explain:
+        from . import explain as X
+        t0 = time.perf_counter()
+        todo = list(dict.fromkeys(res.plan_nodes))
+        kw = {}
+        if explain_max_edges is not None:
+            kw["max_edges_per_target"] = explain_max_edges
+        if explain_max_full_graph is not None:
+            kw["max_full_graph_targets"] = explain_max_full_graph
+        ex = X.explain_nodes(G.TemporalGraph(rp, col, ew, x, g.meta), model, todo, k=int(explain), **kw)
+        res.evidence = dict(zip(todo, X.attach_events(g, ex)))
+        sync(); tm["explain"] = (time.perf_counter() - t0) * 1e3
     return res

@@ -713,9 +713,45 @@ class DeviceStream:
                 "node_kind": kind_d.cpu().numpy().astype(np.int64), "t0": t0, "span": span, "merge_renames": self.merge,
                 "label": lab.cpu().numpy().astype(np.int64), "size_mb": size_mb.cpu().numpy(), "device": str(self.dev),
                 "name_hash": nh, "dir_hash": dir_hash_device, "events": nw, "node_source": node_source, "window_ranks": (lo, hi), "perm": perm if Gn is None else None}
+        per_event = 2 if Gn is None else 4
+
+        def edge_event(perm=perm, sel=sel, keep=None if Gn is None else keep):
+            """the event (stream row) that made each CSR edge"""
+            if perm.numel() != col.numel():                                 # E = 0: perm holds one spare entry
+                return torch.zeros(0, dtype=torch.int64, device=self.dev)
+            rank = torch.arange(nw, device=self.dev).repeat_interleave(per_event)
+            return sel[(rank if keep is None else rank[keep])[perm.long() & 0xffffffff]]
+        meta.update(edge_event=edge_event, event_info=self.event_records)
         if edge_labels:
             meta["edge_label"] = G.edge_labels_device(P, F, self.d_raw_slot[sel], rowptr, col, N)
         return G.TemporalGraph(rowptr, col, ew, x, meta)
+
+    def event_records(self, rows) -> list:
+        """graph.event_record of stream rows `rows` (valid until the stream is compacted), plus "source" for a stream of
+        several sources.  A live stream holds no syscall strings: its records name the event kind of the row's slot."""
+        rows = np.asarray(rows, np.int64)
+        if self.cols is not None:
+            recs = ingest.column_event_records(self.cols, rows)
+            if not self.multi_source:
+                for r in recs:
+                    r.pop("source", None)
+            return recs
+        torch = self.torch
+        r = torch.from_numpy(rows).to(self.dev)
+        ts, pid = self.d_ts[r].cpu().numpy(), self.d_pid[r].cpu().numpy().view(np.uint32)
+        slot = self.d_raw_slot[r].cpu().numpy()
+        po = self.d_poff[torch.stack([r, r + 1], 1)].cpu().numpy() if rows.size else np.zeros((0, 2), np.int64)
+        src = None if self.d_source is None or not self.multi_source else (self.d_source[r].to(torch.int64) & 0xffff).cpu().numpy()
+        kinds = {v: k for k, v in G._EVENT_SLOT.items()}
+        out = []
+        for k in range(rows.size):
+            a, b = int(po[k, 0]), int(po[k, 1])
+            path = bytes(self.d_pdata[a:b].cpu().numpy()).decode("utf-8", "replace") if b > a else ""
+            rec = {"time": float(ts[k]), "pid": int(pid[k]), "syscall": kinds.get(int(slot[k]), "other"), "path": path}
+            if src is not None:
+                rec["source"] = int(src[k])
+            out.append(rec)
+        return out
 
     def sequences_device(self, g: G.TemporalGraph, only_nodes):
         """LSTM sequences of the given file nodes of window graph `g`, built ON THE DEVICE (nerrf_trace_sequences) from the
@@ -767,6 +803,8 @@ class TickResult:
     timings_ms: dict
     truncated: bool = False
     restored: list = field(default_factory=list)   # directories this tick's plan restores from the snapshot
+    evidence: dict = field(default_factory=dict)   # StreamingPlanner(explain=k): plan key of each node step this tick
+                                                   # planned (as in `planned`, kills included) -> its explanation
 
 
 @dataclass
@@ -787,6 +825,7 @@ class StreamingPlanner:
     restore_candidates: bool = False   # also propose directory restores (planner spec v2, one GPU); covered files count as reverted
     max_restores: int = 4
     min_restore_files: int = 8
+    explain: int = 0               # k > 0: each tick's TickResult.evidence explains its new steps (pipeline.run(explain=k))
     device: str = "cuda"
     dist_ctx: object = None        # pipeline.DistContext for the multi-GPU form
     reverted: set = field(default_factory=set)
@@ -913,6 +952,8 @@ class StreamingPlanner:
         multi = ctx is not None and ctx.world > 1
         if multi and self.restore_candidates:
             raise NotImplementedError("restore candidates are planned on one GPU (dist_ctx.world > 1 is not supported)")
+        if multi and self.explain:
+            raise NotImplementedError("explanations are computed on one GPU (dist_ctx.world > 1 is not supported)")
         lead = not multi or ctx.rank == 0
         dev = torch.device(self.device)
         if multi:
@@ -996,7 +1037,7 @@ class StreamingPlanner:
                 return sq_t.cpu().numpy(), ln_t.cpu().numpy(), hv_t.cpu().numpy()
             return sq, ln, have
 
-        new, truncated, restored = [], False, []
+        new, truncated, restored, evidence = [], False, [], {}
         for rnd in range(4):
             # a planning pass proposes at most 32 process kills (planner spec v1: guards live in state word 0); a tick
             # with more suspicious processes than that plans again over what is still unreverted
@@ -1012,7 +1053,7 @@ class StreamingPlanner:
                                depth=self.depth, iterations=self.iterations, device=self.device, exclude=skip,
                                commit_per_search=self.commit_per_search, dist_ctx=self.dist_ctx,
                                kill_candidates=self.kill_candidates, restore_candidates=self.restore_candidates,
-                               max_restores=self.max_restores, min_restore_files=self.min_restore_files)
+                               max_restores=self.max_restores, min_restore_files=self.min_restore_files, explain=self.explain)
             for k, v in res.timings_ms.items():
                 tm[k] = tm.get(k, 0.0) + float(v)
             got = []
@@ -1035,8 +1076,14 @@ class StreamingPlanner:
                     self._reverted_hash.update(fresh.values())
                     return list(fresh)
                 plan_names = names.take(res.plan_nodes)           # one bulk fetch (device names of a live stream)
+                fresh_kills = [key(n, nm) for n, nm in zip(res.plan_nodes, plan_names) if kind[n] == 1 and key(n, nm) not in self.killed]
                 self.killed.update(key(n, nm) for n, nm in zip(res.plan_nodes, plan_names) if kind[n] == 1)
                 got = revert(res.plan_nodes, plan_names)
+                if res.evidence is not None:
+                    fresh = set(got) | set(fresh_kills)
+                    for n, nm in zip(res.plan_nodes, plan_names):
+                        if key(n, nm) in fresh and key(n, nm) not in evidence:
+                            evidence[key(n, nm)] = res.evidence.get(n)
                 new += got
                 for r in res.restores:                         # a restored directory brings back every file it covers
                     cov = revert(r["covers"], names.take(r["covers"]))
@@ -1050,4 +1097,4 @@ class StreamingPlanner:
             truncated = truncated or bool(res.plan.truncated)
             if not more:
                 break
-        self.ticks.append(TickResult(t_hi - t0, n_events, g.num_nodes, g.num_edges, new, tm, truncated, restored))
+        self.ticks.append(TickResult(t_hi - t0, n_events, g.num_nodes, g.num_edges, new, tm, truncated, restored, evidence))

@@ -3,6 +3,7 @@ ROADMAP.md:28,86 -- scheduled, never written).
 
     python -m nerrf_b200.undo --trace events.pb   --weights weights.pt --out plan.json --shell plan.sh
     python -m nerrf_b200.undo --trace trace.jsonl --train-epochs 25    --out plan.json
+    python -m nerrf_b200.undo --trace trace.jsonl --train-epochs 25    --out plan.json --explain 8
     python -m nerrf_b200.undo --trace nodeA=a.pb --trace nodeB=b.pb --weights weights.pt --out plan.json --shell-dir DIR
 
 trace: serialized nerrf.trace.EventBatch bytes (*.pb; proto/trace.proto:47-49, e.g. a buffered StreamEvents stream) or
@@ -114,6 +115,8 @@ def main(argv=None) -> dict:
                     help="cap on the number of reversions (default: every candidate may be reverted); a capped plan that "
                          "leaves improving candidates is marked truncated and is not auto-approvable")
     ap.add_argument("--shell-dir", default=None, help="write DIR/<host>.sh per --trace HOST=PATH")
+    ap.add_argument("--explain", type=int, default=0, metavar="K",
+                    help="attach to every node step the K trace events whose edges drove its GraphSAGE-T score most")
     ap.add_argument("--device", default="cuda")
     a = ap.parse_args(argv)
     traces = parse_traces(a.trace)
@@ -131,7 +134,7 @@ def main(argv=None) -> dict:
     model, scorer = load_models(a.weights, a.train_epochs, log=log)
     model.to(a.device); scorer.to(a.device)
     res = pipeline.run(g, seq, lengths, nodes, model, scorer, top_a=min(a.top_a, 4096), n_rollouts=a.rollouts, depth=a.depth,
-                       iterations=a.iterations, plan_steps=a.max_steps, device=a.device)
+                       iterations=a.iterations, plan_steps=a.max_steps, device=a.device, explain=a.explain)
     plan = emit.from_pipeline(g, res, attack_id=a.id, host_names=hosts)
     plan["stats"] = {"events": int(n_events), "nodes": int(g.num_nodes), "edges": int(g.num_edges),
                      "candidates": int(len(res.candidates)), "ingest_ms": t_ingest,
