@@ -185,6 +185,16 @@ int nerrf_explain_subgraph_fill(const void* rowptr, int rowptr_is64, const int32
 int nerrf_explain_topk(const int64_t* seg, int64_t n_seg, const float* ew, const float* d_ew, const int64_t* epos,
                        const int64_t* edge_event, int k, int64_t* out_edge, float* out_attr, int64_t* out_pos,
                        int64_t* out_event, nerrf_stream_t stream);
+/* Sequence-step evidence of the BiLSTM (DESIGN.md 1.2.1): per sequence b (seq, dseq fp32 [B, T, D_in]; dseq = the
+ * gradient of its encrypt logit, nerrf_lstm_input_grad), over the valid steps t < len[b] (len clamped to [0, T]):
+ *     a_t = sum_d seq[b,t,d] * dseq[b,t,d]   (each product rounded, summed left to right, d ascending)
+ * and the k steps of largest |a_t|, ties to the lower t, NaN below every number: out_step int32 [B, k] (t, -1 past the
+ * valid steps), out_attr fp32 (a_t, 0 there), out_feature int32 (argmax_d |seq * dseq|, ties to the lower d, -1 when every
+ * term is 0), out_event int64 (step_event[b, t] of int64 [B, T], -1 when step_event is NULL or the pick is empty).
+ * One warp per sequence; k in 1..1024, D_in in 1..1024.  Deterministic.  All pointers device. */
+int nerrf_lstm_explain_steps(const float* seq, const float* dseq, const int32_t* len, int64_t B, int T, int D_in,
+                             const int64_t* step_event, int k, int32_t* out_step, float* out_attr, int32_t* out_feature,
+                             int64_t* out_event, nerrf_stream_t stream);
 
 /* The normalised edge weights of the graph, for t_w above: a[e] = ew[e] * (1 / max(weight sum of e's destination row,
  * 1e-12)), edges in CSR-by-destination order (rowptr [n+1], int32 or int64 when rowptr_is64; ew, a [E]).  The weight sum
@@ -356,6 +366,14 @@ int nerrf_lstm_backward(const float* seq, const int32_t* len, int64_t B, int T, 
                         const float* const* W_ih, const float* const* W_hh, void* tape, size_t tape_bytes,
                         const float* dhfin, float* dseq, float* const* dW_ih, float* const* dW_hh, float* const* db,
                         void* workspace, size_t workspace_bytes, nerrf_stream_t stream);
+/* Input gradient only (explanations, DESIGN.md 1.2.1): nerrf_lstm_backward without dW_ih, dW_hh and db.  It runs the same
+ * recurrence and input-gradient launches and skips the weight gradients, so dseq (required here) equals
+ * nerrf_lstm_backward's on the same tape bit for bit.  The workspace is the layer-output gradient buffer alone
+ * (B*T*2H floats, rounded up to 256 bytes); tape_bytes as for nerrf_lstm_backward.  Consumes the tape the same way. */
+int nerrf_lstm_input_grad_workspace_bytes(int64_t B, int T, int D_in, int H, int num_layers, size_t* bytes);
+int nerrf_lstm_input_grad(const float* seq, const int32_t* len, int64_t B, int T, int D_in, int H, int num_layers,
+                          const float* const* W_ih, const float* const* W_hh, void* tape, size_t tape_bytes,
+                          const float* dhfin, float* dseq, void* workspace, size_t workspace_bytes, nerrf_stream_t stream);
 
 /* ------------------------------------------------------------------ temporal-graph constructor, device half
  * (SURVEY.md 8f rank 1 -- the step immediately before GraphSAGE_T.forward)
@@ -391,6 +409,13 @@ int nerrf_trace_sequences(const int64_t* cand_nodes, int n_cand, const void* row
                           const int64_t* order, const double* ts, const uint8_t* event_slot, const int64_t* bytes,
                           const uint8_t* path_flags, double t0, double span, int t_max, float* seq_out,
                           int32_t* len_out, void* stream);
+/* The same, and also event_out (int64 [n_cand, t_max], may be NULL): event_out[c, k] = order[perm[e] >> 1], the stored
+ * row of the event that made step k of candidate c (the id space of the stream's event records), -1 at padded steps.
+ * The plain symbol is this call with event_out = NULL; seq_out and len_out are the same bits either way. */
+int nerrf_trace_sequences_ex(const int64_t* cand_nodes, int n_cand, const void* rowptr, int rowptr_is64,
+                             const uint32_t* perm, const int64_t* order, const double* ts, const uint8_t* event_slot,
+                             const int64_t* bytes, const uint8_t* path_flags, double t0, double span, int t_max,
+                             float* seq_out, int32_t* len_out, int64_t* event_out, void* stream);
 
 /* Per-pair edge labels of a trace graph on the device (the training target of the edge head; spec = nerrf_b200/graph.py
  * graph_from_events meta['edge_label']).  node_p / node_f [n_events] = the graph's events mapped to node ids (as handed

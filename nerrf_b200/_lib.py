@@ -40,6 +40,7 @@ SIGNATURES = {
     "nerrf_explain_subgraph_fill": (C.c_int, [vp, C.c_int, vp, vp, vp, C.c_int, C.c_int64, vp, C.c_int64, C.c_int, C.c_int64,
                                               vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]),
     "nerrf_explain_topk": (C.c_int, [vp, C.c_int64, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]),
+    "nerrf_lstm_explain_steps": (C.c_int, [vp, vp, vp, C.c_int64, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp]),
     "nerrf_sage_edge_head_bwd_workspace_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "nerrf_sage_edge_head_bwd": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, C.c_size_t,
                                            C.c_int64, C.c_int, vp]),
@@ -88,10 +89,15 @@ SIGNATURES = {
     "nerrf_lstm_backward": (C.c_int, [vp, vp, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp), C.POINTER(vp),
                                       vp, C.c_size_t, vp, vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp), vp, C.c_size_t,
                                       vp]),
+    "nerrf_lstm_input_grad_workspace_bytes": (C.c_int, [C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]),
+    "nerrf_lstm_input_grad": (C.c_int, [vp, vp, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(vp), C.POINTER(vp),
+                                        vp, C.c_size_t, vp, vp, vp, C.c_size_t, vp]),
     "nerrf_graph_csr_workspace_bytes": (C.c_int, [C.c_int64, C.c_int64, C.POINTER(C.c_int64)]),
     "nerrf_graph_build_csr_ex": (C.c_int, [vp, vp, vp, vp, C.c_int64, C.c_int64, C.c_float, C.c_float, vp, C.c_int,
                                            vp, vp, vp, vp, C.c_int64, vp]),
     "nerrf_trace_sequences": (C.c_int, [vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, C.c_double, C.c_double, C.c_int, vp, vp, vp]),
+    "nerrf_trace_sequences_ex": (C.c_int, [vp, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp, vp, C.c_double, C.c_double, C.c_int, vp, vp,
+                                           vp, vp]),
     "nerrf_graph_build_csr": (C.c_int, [vp, vp, vp, vp, C.c_int64, C.c_int64, C.c_float, C.c_float, vp, C.c_int,
                                         vp, vp, vp, C.c_int64, vp]),
     "nerrf_trace_edge_labels_workspace_bytes": (C.c_int, [C.c_int64, C.POINTER(C.c_int64)]),

@@ -19,6 +19,11 @@ from ... import _lib as L
 
 D_IN = 16      # event feature width (SURVEY.md 8a a4: syscall one-hot, log1p(bytes), dt, flags, ext pattern ...)
 T_MAX = 100
+# name of each of the D_IN event features, in the layout of pipeline.file_sequences (event kind one-hot x 8, size, dt,
+# time, .lockbit name, /tmp|/proc path, 3 spare); sequence explanations name a step's dominant feature by it
+FEATURE_NAMES = ("kind:file_created", "kind:file_encrypt_start", "kind:file_encrypt_complete", "kind:ransom_note_created",
+                 "kind:openat", "kind:write", "kind:rename", "kind:other", "size", "dt", "time", "lockbit_name",
+                 "tmp_or_proc_path", "spare_13", "spare_14", "spare_15")
 
 
 class LSTMScorer(nn.Module):

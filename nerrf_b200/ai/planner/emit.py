@@ -68,6 +68,37 @@ def restore_dir_step(directory: str, covered_paths) -> dict:
     return r
 
 
+def event_fields(ev, host_names=None):
+    """The plan record of one evidence event (an event_info record, or None) -> (record or None, hostile): record =
+    {"time", "pid", "syscall", "path"[, "host"]}; hostile = a control character in its path or syscall."""
+    if ev is None:
+        return None, False
+    rec = {"time": float(ev["time"]), "pid": int(ev["pid"]), "syscall": str(ev["syscall"]), "path": str(ev["path"])}
+    if host_names is not None and "source" in ev:
+        rec["host"] = check_host_name(host_names[int(ev["source"])])
+    return rec, _has_control_chars(rec["path"]) or _has_control_chars(rec["syscall"])
+
+
+def sequence_evidence_fields(sx, host_names=None) -> dict:
+    """The plan fields of one file's sequence explanation (pipeline.PipelineResult.sequence_evidence[node]):
+    "sequence_evidence" = one entry per attributed step, strongest first -- {"event": {"time", "pid", "syscall",
+    "path"[, "host"]}, "step" (position in the file's sequence, oldest first), "feature" (name of the step's dominant
+    feature, lstm.FEATURE_NAMES; None when every term is 0), "attribution"} -- and "sequence_evidence_logit" (the
+    BiLSTM's encrypt logit).  A control character in an event's path flags the step "hostile_name"."""
+    from ..models.lstm import FEATURE_NAMES
+    out, hostile = [], False
+    for s in sx["steps"]:
+        rec, bad = event_fields(s.get("event"), host_names)
+        hostile = hostile or bad
+        f = int(s["feature"])
+        out.append({"event": rec, "step": int(s["t"]), "feature": FEATURE_NAMES[f] if 0 <= f < len(FEATURE_NAMES) else None,
+                    "attribution": float(s["attr"])})
+    r = {"sequence_evidence": out, "sequence_evidence_logit": float(sx["logit"])}
+    if hostile:
+        r["hostile_name"] = True
+    return r
+
+
 def evidence_fields(ex, host_names=None) -> dict:
     """The plan fields of one node's explanation (pipeline.PipelineResult.evidence[node]): "evidence" = one entry per
     attributed edge, strongest first -- {"event": {"time", "pid", "syscall", "path"[, "host"]}, "src", "dst" (the edge's
@@ -78,13 +109,8 @@ def evidence_fields(ex, host_names=None) -> dict:
         return {"evidence": None, "evidence_reason": str(ex.get("reason", ""))}
     out, hostile = [], False
     for e in ex["edges"]:
-        ev = e.get("event")
-        rec = None
-        if ev is not None:
-            rec = {"time": float(ev["time"]), "pid": int(ev["pid"]), "syscall": str(ev["syscall"]), "path": str(ev["path"])}
-            if host_names is not None and "source" in ev:
-                rec["host"] = check_host_name(host_names[int(ev["source"])])
-            hostile = hostile or _has_control_chars(rec["path"]) or _has_control_chars(rec["syscall"])
+        rec, bad = event_fields(e.get("event"), host_names)
+        hostile = hostile or bad
         src, dst = str(e.get("src_name", e["src"])), str(e.get("dst_name", e["dst"]))
         hostile = hostile or _has_control_chars(src) or _has_control_chars(dst)
         out.append({"event": rec, "src": src, "dst": dst, "attribution": float(e["attr"])})
@@ -95,7 +121,8 @@ def evidence_fields(ex, host_names=None) -> dict:
 
 
 def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node_score=None, truncated=False,
-              remaining_candidates=0, restores=None, hosts=None, evidence=None, host_names=None) -> dict:
+              remaining_candidates=0, restores=None, hosts=None, evidence=None, host_names=None,
+              sequence_evidence=None) -> dict:
     """names: node id -> path (TemporalGraph.meta['names']); plan_nodes: node ids to revert, in plan order
     (PipelineResult.plan_nodes); scores: Plan.scores (exact reward after each commit, scores[0] = before).
     truncated / remaining_candidates: the planner stopped at its step limit while improving candidates remained --
@@ -105,7 +132,9 @@ def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node
     hosts: node id -> host name, for a graph of several sources: every step gets the "host" it applies to (a restore:
     the host of the files it covers; covers on two hosts raise ValueError).  None: no host fields (one source).
     evidence: node id -> explanation (pipeline.PipelineResult.evidence): each node step found there gets the fields of
-    evidence_fields (host_names: source id -> host name for its events).  None: no evidence fields."""
+    evidence_fields (host_names: source id -> host name for its events).  None: no evidence fields.
+    sequence_evidence: node id -> sequence explanation (pipeline.PipelineResult.sequence_evidence): each file step found
+    there gets the fields of sequence_evidence_fields.  None: no sequence evidence fields.  to_shell reads neither."""
     host_of = (lambda n: check_host_name(hosts[int(n)])) if hosts is not None else None
     at = {int(r["position"]): r for r in (restores or [])}
     total = len(plan_nodes) + len(at)
@@ -137,6 +166,11 @@ def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node
             step["reward_after"] = float(scores[k + 1])
         if evidence is not None and evidence.get(n) is not None:
             step.update(evidence_fields(evidence[n], host_names))
+        if sequence_evidence is not None and sequence_evidence.get(n) is not None:
+            sf = sequence_evidence_fields(sequence_evidence[n], host_names)
+            if sf.pop("hostile_name", False):
+                step["hostile_name"] = True
+            step.update(sf)
         steps.append(step)
     out = {"version": PLAN_VERSION, "kind": "nerrf.undo_plan", "attack_id": attack_id, "steps": steps,
            "approve_if": "all_checks_pass" if not truncated else "all_checks_pass_and_operator_confirms_partial_plan",
@@ -186,4 +220,5 @@ def from_pipeline(g, result, attack_id=None, host_names=None) -> dict:
                      size_mb=g.meta.get("size_mb"), node_score=score, truncated=getattr(result.plan, "truncated", False),
                      remaining_candidates=getattr(result.plan, "remaining_candidates", 0),
                      restores=getattr(result, "restores", None), hosts=hosts,
-                     evidence=getattr(result, "evidence", None), host_names=host_names)
+                     evidence=getattr(result, "evidence", None), host_names=host_names,
+                     sequence_evidence=getattr(result, "sequence_evidence", None))

@@ -17,7 +17,13 @@
 //
 // Top-k, one CTA per target segment: k rounds of a block arg-max of (|a|, -position) below the previous pick, so ties go
 // to the lower CSR position and the result has no order that depends on scheduling.
+//
+// Sequence steps (DESIGN.md 1.2.1), nerrf_lstm_explain_steps, one warp per sequence: a_t = sum_d x[t,d] * dseq[t,d] over
+// the valid steps, as __fmul_rn products summed left to right with __fadd_rn (so a float32 restatement over the same
+// dseq reproduces it bit for bit), then k rounds of a warp arg-max of (|a_t|, -t) below the previous pick -- the same
+// rule (explain_rank.cuh) as the edge top-k.
 #include "common.cuh"
+#include "explain_rank.cuh"
 
 namespace nerrf {
 namespace {
@@ -249,11 +255,6 @@ __global__ void __launch_bounds__(XT) subgraph_fill_kernel(const RP* __restrict_
     }
 }
 
-// (|a|, local index) ordering: larger |a| first, then the lower index; NaN ranks below every number
-__device__ inline bool better(float a, int64_t i, float b, int64_t j) {
-    return a > b || (a == b && i < j);
-}
-
 __global__ void __launch_bounds__(XT) topk_kernel(const int64_t* __restrict__ seg, const float* __restrict__ ew,
                                                   const float* __restrict__ d_ew, const int64_t* __restrict__ epos,
                                                   const int64_t* __restrict__ edge_event, int k, int64_t* __restrict__ out_edge,
@@ -272,8 +273,7 @@ __global__ void __launch_bounds__(XT) topk_kernel(const int64_t* __restrict__ se
         float bv = -1.f;
         int64_t bi = -1;
         for (int64_t e = e0 + threadIdx.x; e < e1; e += XT) {
-            float v = fabsf(ew[e] * d_ew[e]);
-            if (v != v) v = -0.5f;                                    // NaN: below every number, above "none"
+            const float v = rank_key(ew[e] * d_ew[e]);               // NaN: below every number, above "none"
             const int64_t i = e - e0;
             if (better(pv, pi, v, i) && (bi < 0 || better(v, i, bv, bi))) { bv = v; bi = i; }
         }
@@ -309,6 +309,73 @@ __global__ void __launch_bounds__(XT) topk_kernel(const int64_t* __restrict__ se
             }
             return;
         }
+    }
+}
+
+constexpr int SW = 8;                 // sequences (one warp each) per CTA of the step kernel
+
+// a_t of one step: the D products x[d] * g[d], each rounded, summed left to right (fixed order, no contraction)
+__device__ __forceinline__ float step_attr(const float* __restrict__ x, const float* __restrict__ g, int D) {
+    float s = __fmul_rn(__ldg(x), __ldg(g));
+    for (int d = 1; d < D; ++d) s = __fadd_rn(s, __fmul_rn(__ldg(x + d), __ldg(g + d)));
+    return s;
+}
+
+// argmax_d |x[d] * g[d]|, ties to the lower d; -1 when every term is 0 (a NaN term is never dominant)
+__device__ __forceinline__ int dominant_feature(const float* __restrict__ x, const float* __restrict__ g, int D) {
+    int best = -1;
+    float bm = 0.f;
+    for (int d = 0; d < D; ++d) {
+        const float m = fabsf(__fmul_rn(__ldg(x + d), __ldg(g + d)));
+        if (m > bm) { bm = m; best = d; }
+    }
+    return best;
+}
+
+__global__ void __launch_bounds__(32 * SW) explain_steps_kernel(const float* __restrict__ seq, const float* __restrict__ dseq,
+                                                                const int32_t* __restrict__ len, int64_t B, int T, int D,
+                                                                const int64_t* __restrict__ step_event, int k,
+                                                                int32_t* __restrict__ out_step, float* __restrict__ out_attr,
+                                                                int32_t* __restrict__ out_feature, int64_t* __restrict__ out_event) {
+    const int lane = threadIdx.x & 31;
+    const int64_t b = (int64_t)blockIdx.x * SW + (threadIdx.x >> 5);
+    if (b >= B) return;                                               // warp-uniform
+    const int lb = len[b];
+    const int L = lb < 0 ? 0 : (lb > T ? T : lb);
+    const float* X = seq + b * T * D;
+    const float* G = dseq + b * T * D;
+    float pv = __int_as_float(0x7f800000);                            // +inf: every key is below the "previous pick" of round 0
+    int pi = -1;
+    for (int r = 0; r < k; ++r) {
+        float bv = -1.f;
+        int bi = -1;
+        for (int t = lane; t < L; t += 32) {
+            const float v = rank_key(step_attr(X + (int64_t)t * D, G + (int64_t)t * D, D));
+            if (better(pv, pi, v, t) && (bi < 0 || better(v, t, bv, bi))) { bv = v; bi = t; }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {                            // a total order: every lane ends on the same pick
+            const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+            if (oi >= 0 && (bi < 0 || better(ov, oi, bv, bi))) { bv = ov; bi = oi; }
+        }
+        if (bi < 0) {                                                 // valid steps exhausted: the remaining picks are empty
+            for (int q = r + lane; q < k; q += 32) {
+                const int64_t o = b * k + q;
+                out_step[o] = -1; out_attr[o] = 0.f; out_feature[o] = -1; out_event[o] = -1;
+            }
+            return;
+        }
+        if (lane == 0) {
+            const int64_t o = b * k + r;
+            const float* x = X + (int64_t)bi * D;
+            const float* g = G + (int64_t)bi * D;
+            out_step[o] = bi;
+            out_attr[o] = step_attr(x, g, D);
+            out_feature[o] = dominant_feature(x, g, D);
+            out_event[o] = step_event ? step_event[b * T + bi] : -1;
+        }
+        pv = bv; pi = bi;
     }
 }
 
@@ -398,4 +465,19 @@ extern "C" int nerrf_explain_topk(const int64_t* seg, int64_t n_seg, const float
     topk_kernel<<<(unsigned)n_seg, XT, 0, (cudaStream_t)stream>>>(seg, ew, d_ew, epos, edge_event, k, out_edge, out_attr, out_pos,
                                                                    out_event);
     return launch_status("explain top-k");
+}
+
+extern "C" int nerrf_lstm_explain_steps(const float* seq, const float* dseq, const int32_t* len, int64_t B, int T, int D_in,
+                                        const int64_t* step_event, int k, int32_t* out_step, float* out_attr,
+                                        int32_t* out_feature, int64_t* out_event, nerrf_stream_t stream) {
+    NERRF_REQUIRE(B >= 0, "negative sequence count");
+    NERRF_REQUIRE(T >= 1 && D_in >= 1 && D_in <= 1024, "need T >= 1 and D_in in 1..1024 (got T = %d, D_in = %d)", T, D_in);
+    NERRF_REQUIRE(k >= 1 && k <= 1024, "k must lie in 1..1024 (got %d)", k);
+    if (B == 0) return NERRF_OK;
+    NERRF_REQUIRE(seq && dseq && len && out_step && out_attr && out_feature && out_event, "null pointer");
+    const int64_t grid = (B + SW - 1) / SW;
+    NERRF_REQUIRE(grid < (1ll << 31), "too many sequences for one launch");
+    explain_steps_kernel<<<(unsigned)grid, 32 * SW, 0, (cudaStream_t)stream>>>(seq, dseq, len, B, T, D_in, step_event, k, out_step,
+                                                                               out_attr, out_feature, out_event);
+    return launch_status("explain sequence steps");
 }

@@ -203,7 +203,7 @@ __global__ void __launch_bounds__(256) trace_sequences_kernel(const int64_t* __r
                                                                const double* __restrict__ ts, const uint8_t* __restrict__ slot,
                                                                const int64_t* __restrict__ bytes, const uint8_t* __restrict__ pflags,
                                                                double t0, double span, int t_max, float* __restrict__ seq,
-                                                               int32_t* __restrict__ len_out) {
+                                                               int32_t* __restrict__ len_out, int64_t* __restrict__ event_out) {
     const int lane = threadIdx.x & 31;
     const int c = blockIdx.x * 8 + (threadIdx.x >> 5);
     if (c >= n_cand) return;
@@ -214,9 +214,12 @@ __global__ void __launch_bounds__(256) trace_sequences_kernel(const int64_t* __r
     const int len = (int)(deg - start);
     if (lane == 0) len_out[c] = len;
     float* out = seq + (size_t)c * t_max * 16;
+    if (event_out)                                                   // the stored row of each step, -1 at padded steps
+        for (int k = len + lane; k < t_max; k += 32) event_out[(size_t)c * t_max + k] = -1;
     for (int k = lane; k < len; k += 32) {
         const int64_t e = e0 + start + k;
         const int64_t si = order[perm[e] >> 1];
+        if (event_out) event_out[(size_t)c * t_max + k] = si;
         const double t = ts[si];
         double dt = 0.0;
         if (k > 0) { const double tp = ts[order[perm[e - 1] >> 1]]; dt = fmin(t - tp, 10.0); }
@@ -520,6 +523,14 @@ extern "C" int nerrf_trace_sequences(const int64_t* cand_nodes, int n_cand, cons
                                      const int64_t* order, const double* ts, const uint8_t* event_slot, const int64_t* bytes,
                                      const uint8_t* path_flags, double t0, double span, int t_max, float* seq_out,
                                      int32_t* len_out, void* stream) {
+    return nerrf_trace_sequences_ex(cand_nodes, n_cand, rowptr, rowptr_is64, perm, order, ts, event_slot, bytes, path_flags, t0, span,
+                                    t_max, seq_out, len_out, nullptr, stream);
+}
+
+extern "C" int nerrf_trace_sequences_ex(const int64_t* cand_nodes, int n_cand, const void* rowptr, int rowptr_is64,
+                                        const uint32_t* perm, const int64_t* order, const double* ts, const uint8_t* event_slot,
+                                        const int64_t* bytes, const uint8_t* path_flags, double t0, double span, int t_max,
+                                        float* seq_out, int32_t* len_out, int64_t* event_out, void* stream) {
     NERRF_REQUIRE(n_cand >= 0 && t_max >= 1, "bad sizes");
     if (n_cand == 0) return NERRF_OK;
     NERRF_REQUIRE(cand_nodes && rowptr && perm && order && ts && event_slot && bytes && path_flags && seq_out && len_out, "null pointer");
@@ -529,9 +540,9 @@ extern "C" int nerrf_trace_sequences(const int64_t* cand_nodes, int n_cand, cons
     const unsigned grid = (unsigned)((n_cand + 7) / 8);
     if (rowptr_is64)
         trace_sequences_kernel<int64_t><<<grid, 256, 0, st>>>(cand_nodes, n_cand, (const int64_t*)rowptr, perm, order, ts, event_slot, bytes,
-                                                              path_flags, t0, span, t_max, seq_out, len_out);
+                                                              path_flags, t0, span, t_max, seq_out, len_out, event_out);
     else
         trace_sequences_kernel<int32_t><<<grid, 256, 0, st>>>(cand_nodes, n_cand, (const int32_t*)rowptr, perm, order, ts, event_slot, bytes,
-                                                              path_flags, t0, span, t_max, seq_out, len_out);
+                                                              path_flags, t0, span, t_max, seq_out, len_out, event_out);
     return launch_status("trace_sequences_kernel");
 }

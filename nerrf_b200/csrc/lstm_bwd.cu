@@ -15,6 +15,8 @@
 //   lstm_bwd_reduce_kernel partials -> gradients, chunk order fixed
 //   lstm_bwd_din_kernel    d in_l = [dg_fwd || dg_bwd] [W_ih_fwd ; W_ih_bwd], K = 8H (the directions add in a fixed order);
 //                          the injected gradient of layer l-1's output, or dseq at l = 0
+// nerrf_lstm_input_grad is the same backward without the weight gradients (explanations, DESIGN.md 1.2.1): the recurrence
+// and din launches only, so its dseq equals nerrf_lstm_backward's bit for bit, and its workspace is the dout buffer.
 #include "common.cuh"
 #include "lstm_tape.cuh"
 
@@ -279,6 +281,51 @@ int weight_grad(const float* gates, const float* x, int ldx, int xoff_b, int N, 
     return launch_status("lstm weight gradient");
 }
 
+// The backward proper, layer by layer, top layer first.  weights = false is the input-gradient mode (explanations): the
+// same recurrence and din launches in the same order, without the weight-gradient calls, so dseq is the same bits; the
+// workspace is then the dout buffer alone.  Arguments are checked by the callers.
+int backward(const float* seq, const int32_t* len, int64_t B, int T, int D_in, int num_layers, const float* const* W_ih,
+             const float* const* W_hh, void* tape, const float* dhfin, float* dseq, float* const* dW_ih, float* const* dW_hh,
+             float* const* db, void* workspace, bool weights, cudaStream_t st) {
+    const LstmTape tp(B, T);
+    const BwdPlan p = bwd_plan(B, T, D_in, num_layers);
+    float* dout = (float*)workspace;
+    float* part = weights ? (float*)((char*)workspace + p.dout_bytes) : nullptr;
+    float* dbpart = weights ? (float*)((char*)part + p.part_bytes) : nullptr;
+    float* tf = (float*)tape;
+    const int64_t BT = B * (int64_t)T;
+    int rc = set_max_dynamic_smem((const void*)lstm_bwd_rec_kernel, REC_SMEM);
+    if (rc) return rc;
+    for (int l = num_layers - 1; l >= 0; --l) {
+        float* gates = tp.gates(tf, l);
+        const float* out_l = tp.out(tf, l);
+        const float* in_l = l ? tp.out(tf, l - 1) : seq;
+        const int D = l ? 2 * H : D_in;
+        const bool top = l == num_layers - 1;
+        lstm_bwd_rec_kernel<<<dim3((unsigned)((B + BS - 1) / BS), 2), H, REC_SMEM, st>>>(
+            len, B, T, W_hh[2 * l], W_hh[2 * l + 1], gates, tp.cell(tf, l), top ? nullptr : dout, top ? dhfin : nullptr);
+        rc = launch_status("lstm_bwd_rec_kernel");
+        if (rc) return rc;
+        if (weights) {
+            rc = weight_grad(gates, in_l, D, 0, D, 0, len, B, T, p, part, dbpart, dW_ih[2 * l], dW_ih[2 * l + 1], db[2 * l],
+                             db[2 * l + 1], st);
+            if (rc) return rc;
+            // h_prev: out_l one step earlier in each direction's order (forward half t-1, backward half t+1), zero at the start
+            rc = weight_grad(gates, out_l, 2 * H, H, H, 1, len, B, T, p, part, dbpart, dW_hh[2 * l], dW_hh[2 * l + 1], nullptr,
+                             nullptr, st);
+            if (rc) return rc;
+        }
+        if (l > 0 || dseq) {
+            float* din = l ? dout : dseq;          // the recurrence of layer l has consumed dout: overwrite it
+            lstm_bwd_din_kernel<<<dim3((unsigned)((BT + GT - 1) / GT), (D + GT - 1) / GT), 256, 0, st>>>(
+                gates, W_ih[2 * l], W_ih[2 * l + 1], din, D, D, BT);
+            rc = launch_status("lstm_bwd_din_kernel");
+            if (rc) return rc;
+        }
+    }
+    return NERRF_OK;
+}
+
 }  // namespace
 }  // namespace nerrf
 
@@ -327,39 +374,39 @@ extern "C" int nerrf_lstm_backward(const float* seq, const int32_t* len, int64_t
         }
         return NERRF_OK;
     }
-    const LstmTape tp(B, T);
-    const BwdPlan p = bwd_plan(B, T, D_in, num_layers);
-    float* dout = (float*)workspace;
-    float* part = (float*)((char*)workspace + p.dout_bytes);
-    float* dbpart = (float*)((char*)part + p.part_bytes);
-    float* tf = (float*)tape;
-    const int64_t BT = B * (int64_t)T;
-    rc = set_max_dynamic_smem((const void*)lstm_bwd_rec_kernel, REC_SMEM);
+    return backward(seq, len, B, T, D_in, num_layers, W_ih, W_hh, tape, dhfin, dseq, dW_ih, dW_hh, db, workspace, true, st);
+}
+
+extern "C" int nerrf_lstm_input_grad_workspace_bytes(int64_t B, int T, int D_in, int H_, int num_layers, size_t* bytes) {
+    size_t need_tape = 0, need_ws = 0;
+    NERRF_REQUIRE(bytes, "null out");
+    const int rc = nerrf_lstm_train_workspace_bytes(B, T, D_in, H_, num_layers, &need_tape, &need_ws);
     if (rc) return rc;
-    for (int l = num_layers - 1; l >= 0; --l) {
-        float* gates = tp.gates(tf, l);
-        const float* out_l = tp.out(tf, l);
-        const float* in_l = l ? tp.out(tf, l - 1) : seq;
-        const int D = l ? 2 * H : D_in;
-        const bool top = l == num_layers - 1;
-        lstm_bwd_rec_kernel<<<dim3((unsigned)((B + BS - 1) / BS), 2), H, REC_SMEM, st>>>(
-            len, B, T, W_hh[2 * l], W_hh[2 * l + 1], gates, tp.cell(tf, l), top ? nullptr : dout, top ? dhfin : nullptr);
-        rc = launch_status("lstm_bwd_rec_kernel");
-        if (rc) return rc;
-        rc = weight_grad(gates, in_l, D, 0, D, 0, len, B, T, p, part, dbpart, dW_ih[2 * l], dW_ih[2 * l + 1], db[2 * l],
-                         db[2 * l + 1], st);
-        if (rc) return rc;
-        // h_prev: out_l one step earlier in each direction's order (forward half t-1, backward half t+1), zero at the start
-        rc = weight_grad(gates, out_l, 2 * H, H, H, 1, len, B, T, p, part, dbpart, dW_hh[2 * l], dW_hh[2 * l + 1], nullptr,
-                         nullptr, st);
-        if (rc) return rc;
-        if (l > 0 || dseq) {
-            float* din = l ? dout : dseq;          // the recurrence of layer l has consumed dout: overwrite it
-            lstm_bwd_din_kernel<<<dim3((unsigned)((BT + GT - 1) / GT), (D + GT - 1) / GT), 256, 0, st>>>(
-                gates, W_ih[2 * l], W_ih[2 * l + 1], din, D, D, BT);
-            rc = launch_status("lstm_bwd_din_kernel");
-            if (rc) return rc;
-        }
-    }
+    *bytes = bwd_plan(B, T, D_in, num_layers).dout_bytes;
     return NERRF_OK;
+}
+
+extern "C" int nerrf_lstm_input_grad(const float* seq, const int32_t* len, int64_t B, int T, int D_in, int H_, int num_layers,
+                                     const float* const* W_ih, const float* const* W_hh, void* tape, size_t tape_bytes,
+                                     const float* dhfin, float* dseq, void* workspace, size_t workspace_bytes,
+                                     nerrf_stream_t stream) {
+    size_t need_tape = 0, need_ws = 0, need = 0;
+    int rc = nerrf_lstm_train_workspace_bytes(B, T, D_in, H_, num_layers, &need_tape, &need_ws);
+    if (rc) return rc;
+    rc = nerrf_lstm_input_grad_workspace_bytes(B, T, D_in, H_, num_layers, &need);
+    if (rc) return rc;
+    if (B == 0) return NERRF_OK;
+    NERRF_REQUIRE(seq && len && W_ih && W_hh && tape && dhfin && dseq && workspace, "null pointer");
+    NERRF_REQUIRE(((uintptr_t)tape & 15) == 0 && ((uintptr_t)workspace & 15) == 0, "tape and workspace must be 16-byte aligned");
+    if (tape_bytes < need_tape) {
+        set_error("lstm tape too small: need %zu bytes, got %zu", need_tape, tape_bytes);
+        return NERRF_ERR_WORKSPACE;
+    }
+    if (workspace_bytes < need) {
+        set_error("lstm input-gradient workspace too small: need %zu bytes, got %zu", need, workspace_bytes);
+        return NERRF_ERR_WORKSPACE;
+    }
+    for (int i = 0; i < 2 * num_layers; ++i) NERRF_REQUIRE(W_ih[i] && W_hh[i], "null weight pointer");
+    return backward(seq, len, B, T, D_in, num_layers, W_ih, W_hh, tape, dhfin, dseq, nullptr, nullptr, nullptr, workspace, false,
+                    (cudaStream_t)stream);
 }

@@ -11,6 +11,10 @@ dh^L = w_n on the target rows (nerrf_sage_layer_bwd_ex, which accumulates d_ew),
 Neighbourhoods are disjoint blocks of one batched graph, so one target's gradient never reaches another's edges.
 A target whose neighbourhood holds more than max_edges_per_target edges is explained the same way on the whole graph
 (at most max_full_graph_targets of them per call); past that cap it gets no evidence and a reason.  CUDA tensors only.
+
+The BiLSTM half of a file reversion's confidence is explained the same way over the file's event sequence (DESIGN.md
+1.2.1, explain_sequences): a_t = x_t . dz/dx_t for the encrypt logit z, through nerrf_lstm_forward_train,
+nerrf_lstm_input_grad and nerrf_lstm_explain_steps, each step mapped to the event that made it.
 """
 from __future__ import annotations
 
@@ -201,13 +205,133 @@ def explain_nodes(g, model, nodes, k: int = 8, max_edges_per_target: int = DEFAU
     return res
 
 
-def attach_events(g, explained: list) -> list:
+def lstm_forward_tape(seq_model, weights, seq, ln):
+    """nerrf_lstm_forward_train (the fp32 CUDA-core forward) over one batch: -> (hfin fp32 [B, 2H], tape) CUDA tensors.
+    weights = _seq_weights(seq_model, device)."""
+    wih_t, whh_t, bias = weights[:3]
+    B, T, D = seq.shape
+    H, nl = seq_model.hidden, seq_model.num_layers
+    tb, wb = C.c_size_t(), C.c_size_t()
+    L.check(L.lib().nerrf_lstm_train_workspace_bytes(B, T, D, H, nl, C.byref(tb), C.byref(wb)), "nerrf_lstm_train_workspace_bytes")
+    tape = torch.empty(max(tb.value, 16), dtype=torch.uint8, device=seq.device)
+    hfin = torch.empty(B, 2 * H, dtype=torch.float32, device=seq.device)
+    with torch.cuda.device(seq.device):
+        L.check(L.lib().nerrf_lstm_forward_train(L.ptr(seq), L.ptr(ln), B, T, D, H, nl, L.ptr_array(wih_t), L.ptr_array(whh_t),
+                                                 L.ptr_array(bias), L.ptr(hfin), L.ptr(tape), tape.numel(),
+                                                 L.current_stream_ptr()), "nerrf_lstm_forward_train")
+    return hfin, tape
+
+
+def lstm_input_grad(seq_model, weights, seq, ln, tape):
+    """dseq fp32 [B, T, D] = dz/dseq of the encrypt logit z = head_W[0] . hfin + head_b[0]: nerrf_lstm_input_grad over
+    the tape of lstm_forward_tape (which it consumes), seeded with dhfin = head_W[0] on every row."""
+    W_ih, W_hh, hw = weights[3:]
+    B, T, D = seq.shape
+    H, nl = seq_model.hidden, seq_model.num_layers
+    gb = C.c_size_t()
+    L.check(L.lib().nerrf_lstm_input_grad_workspace_bytes(B, T, D, H, nl, C.byref(gb)), "nerrf_lstm_input_grad_workspace_bytes")
+    ws = torch.empty(max(gb.value, 16), dtype=torch.uint8, device=seq.device)
+    dseq = torch.empty_like(seq)
+    dhfin = hw[0].expand(B, 2 * H).contiguous()
+    with torch.cuda.device(seq.device):
+        L.check(L.lib().nerrf_lstm_input_grad(L.ptr(seq), L.ptr(ln), B, T, D, H, nl, L.ptr_array(W_ih), L.ptr_array(W_hh),
+                                              L.ptr(tape), tape.numel(), L.ptr(dhfin), L.ptr(dseq), L.ptr(ws), ws.numel(),
+                                              L.current_stream_ptr()), "nerrf_lstm_input_grad")
+    return dseq
+
+
+def lstm_input_grad_chunk(seq_model, weights, seq, ln):
+    """One batch of the encrypt-logit gradient: -> (hfin fp32 [B, 2H], dseq fp32 [B, T, D]) CUDA tensors."""
+    hfin, tape = lstm_forward_tape(seq_model, weights, seq, ln)
+    return hfin, lstm_input_grad(seq_model, weights, seq, ln, tape)
+
+
+def explain_steps(seq, dseq, ln, step_event, k: int):
+    """-> (step int32 [B, k], attr fp32, feature int32, event int64) CUDA tensors (nerrf_lstm_explain_steps)"""
+    B, T, D = seq.shape
+    dev = seq.device
+    os_ = torch.empty(B, k, dtype=torch.int32, device=dev)
+    oa = torch.empty(B, k, dtype=torch.float32, device=dev)
+    of = torch.empty(B, k, dtype=torch.int32, device=dev)
+    ov = torch.empty(B, k, dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        L.check(L.lib().nerrf_lstm_explain_steps(L.ptr(seq), L.ptr(dseq), L.ptr(ln), B, T, D, L.ptr(step_event), k, L.ptr(os_),
+                                                 L.ptr(oa), L.ptr(of), L.ptr(ov), L.current_stream_ptr()), "nerrf_lstm_explain_steps")
+    return os_, oa, of, ov
+
+
+def _seq_weights(seq_model, dev):
+    """the forward's pre-transposed weights and the backward's torch-layout ones, and head_W, on `dev`"""
+    from .ai.autograd import lstm_params
+    wih_t, whh_t, bias, hw, _ = seq_model._pack(dev)
+    params = lstm_params(seq_model)
+    nl2 = 2 * seq_model.num_layers
+    W_ih = [params[4 * i].detach().to(device=dev, dtype=torch.float32).contiguous() for i in range(nl2)]
+    W_hh = [params[4 * i + 1].detach().to(device=dev, dtype=torch.float32).contiguous() for i in range(nl2)]
+    return wih_t, whh_t, bias, W_ih, W_hh, hw
+
+
+def explain_sequences(seq_model, seq, lengths, k: int = 8, step_event=None, max_batch: int = 512) -> list:
+    """Evidence for the encrypt logit z = head_W[0] . hfin + head_b[0] of each sequence (DESIGN.md 1.2.1):
+        a_t = sum_d x[t,d] * dz/dx[t,d]   over the valid steps t < len
+    -> a list, in sequence order, of {"logit": z, "steps": [{"t", "attr": a_t, "feature": dominant feature index (-1 when
+    every term is 0), "event": step_event[b, t] (-1 without a map)}]} (at most k steps, |attr| descending, ties to the
+    lower t).  seq fp32 [B, T, D_in] and lengths [B] (numpy or torch; moved to the model's device, which must be CUDA);
+    step_event int64 [B, T] or None.  z is evaluated in float64 over the fp32 CUDA-core forward's hfin.  The sequences
+    run max_batch at a time; every kernel on this path treats sequences independently, so the result does not depend on
+    max_batch."""
+    dev = seq_model.head.weight.device
+    if dev.type != "cuda":
+        raise L.NerrfError("explain_sequences needs a CUDA model (no CPU fallback)")
+    if not 1 <= int(k) <= 1024:
+        raise ValueError("k must lie in 1..1024")
+    if int(max_batch) < 1:
+        raise ValueError("max_batch must be >= 1")
+    seq = torch.as_tensor(seq).to(device=dev)
+    if seq.dtype != torch.float32 or seq.dim() != 3 or seq.shape[2] != seq_model.in_dim:
+        raise ValueError(f"seq must be float32 [B,T,{seq_model.in_dim}]")
+    seq = seq.contiguous()
+    B, T, _ = seq.shape
+    ln = torch.as_tensor(lengths).to(device=dev, dtype=torch.int32).contiguous()
+    if ln.numel() != B:
+        raise ValueError("lengths must have B entries")
+    ev = None
+    if step_event is not None:
+        ev = torch.as_tensor(step_event).to(device=dev, dtype=torch.int64).contiguous()
+        if tuple(ev.shape) != (B, T):
+            raise ValueError("step_event must be int64 [B, T]")
+    out = []
+    if B == 0:
+        return out
+    weights = _seq_weights(seq_model, dev)
+    w0 = seq_model.head.weight.detach()[0].double().cpu().numpy()
+    b0 = float(seq_model.head.bias.detach()[0].double())
+    for s in range(0, B, int(max_batch)):
+        e = min(s + int(max_batch), B)
+        sq, lc = seq[s:e], ln[s:e]
+        hfin, dseq = lstm_input_grad_chunk(seq_model, weights, sq, lc)
+        st, at, ft, vt = explain_steps(sq, dseq, lc, None if ev is None else ev[s:e], int(k))
+        z = (hfin.double().cpu().numpy() * w0).sum(1) + b0          # per row, a fixed order: independent of the chunking
+        st, at, ft, vt = (a.cpu().numpy() for a in (st, at, ft, vt))
+        for i in range(e - s):
+            keep = np.nonzero(st[i] >= 0)[0]
+            out.append({"logit": float(z[i]),
+                        "steps": [{"t": int(st[i, j]), "attr": float(at[i, j]), "feature": int(ft[i, j]), "event": int(vt[i, j])}
+                                  for j in keep]})
+    return out
+
+
+def attach_events(g, explained: list, sequences: list | None = None):
     """Resolve each evidence edge's event through g.meta["event_info"] (event index -> {time, pid, syscall, path[, source]})
     and its two endpoints through g.meta["names"]: -> the same list with "event" replaced by the record (None without one)
-    and "src_name" / "dst_name" added."""
+    and "src_name" / "dst_name" added.  sequences: explain_sequences results, resolved in the same single event_info call
+    (over the union of the ids of both kinds of evidence); then -> (explained, sequences), each step's "event" replaced by
+    its record."""
     info = g.meta.get("event_info")
     names = g.meta.get("names")
-    ids = sorted({e["event"] for r in explained if r and r.get("edges") for e in r["edges"] if e["event"] >= 0})
+    ids = {e["event"] for r in explained if r and r.get("edges") for e in r["edges"] if e["event"] >= 0}
+    ids |= {s["event"] for r in (sequences or []) if r and r.get("steps") for s in r["steps"] if s["event"] >= 0}
+    ids = sorted(ids)
     rec = dict(zip(ids, info(np.asarray(ids, np.int64)))) if (info is not None and ids) else {}
     nid = sorted({v for r in explained if r and r.get("edges") for e in r["edges"] for v in (e["src"], e["dst"])})
     nm = dict(zip(nid, names.take(nid) if hasattr(names, "take") else [names[i] for i in nid])) if names is not None else {}
@@ -219,4 +343,11 @@ def attach_events(g, explained: list) -> list:
         r = dict(r)
         r["edges"] = [dict(e, event=rec.get(e["event"]), src_name=nm.get(e["src"]), dst_name=nm.get(e["dst"])) for e in r["edges"]]
         out.append(r)
-    return out
+    if sequences is None:
+        return out
+    seq_out = []
+    for r in sequences:
+        if r is not None and r.get("steps"):
+            r = dict(r, steps=[dict(s, event=rec.get(s["event"])) for s in r["steps"]])
+        seq_out.append(r)
+    return out, seq_out

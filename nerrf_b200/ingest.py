@@ -353,10 +353,13 @@ def graph_from_columns(cols: EventColumns, merge_renames=True, window=None, devi
     return G.TemporalGraph(rowptr, col, ew, x, meta)
 
 
-def sequences_from_columns(cols: EventColumns, merge_renames=True, t_max=None, observable=False, only_nodes=None):
+def sequences_from_columns(cols: EventColumns, merge_renames=True, t_max=None, observable=False, only_nodes=None,
+                           return_events=False):
     """Per-file event sequences for the LSTM without per-event Python: the same arrays as
     pipeline.file_sequences(events_from_columns(cols), graph) -- seq fp32 [n_files, t_max, 16], lengths int32, node ids --
-    (the last t_max events of every file node, oldest first; feature layout: pipeline.file_sequences)."""
+    (the last t_max events of every file node, oldest first; feature layout: pipeline.file_sequences).
+    return_events: also the event of each step (sequences_core), a row of the path-resolved columns -- the ids
+    graph_from_columns' meta["edge_event"] / meta["event_info"] use."""
     cols = resolve_columns(cols)
     n = cols.n
     ts = cols.timestamp
@@ -364,13 +367,17 @@ def sequences_from_columns(cols: EventColumns, merge_renames=True, t_max=None, o
     t0 = float(ts[order[0]]) if n else 0.0
     span = max(float(ts[order[-1]]) - t0, 1e-6) if n else 1.0
     _, node_f, _, kind, _, _ = intern_nodes(cols, order, merge_renames)
-    return sequences_core(cols, order, node_f[order].astype(np.int64), ts[order], t0, span, kind.shape[0], t_max, observable, only_nodes)
+    return sequences_core(cols, order, node_f[order].astype(np.int64), ts[order], t0, span, kind.shape[0], t_max, observable, only_nodes,
+                          return_events)
 
 
-def sequences_core(cols: EventColumns, order, F, tt, t0, span, n_nodes, t_max=None, observable=False, only_nodes=None):
+def sequences_core(cols: EventColumns, order, F, tt, t0, span, n_nodes, t_max=None, observable=False, only_nodes=None,
+                   return_events=False):
     """The sequence builder proper, on already interned events: `order` = stored indices of the events in time order,
     F = their file node ids, tt = their absolute timestamps (both in that order).  Used by sequences_from_columns and by the
-    device stream (stream.DeviceStream), whose interning ran on the GPU."""
+    device stream (stream.DeviceStream), whose interning ran on the GPU.
+    return_events: a fourth array, int64 [n_files, t_max], the stored index (`order` entry) of the event of each step,
+    -1 at padded steps."""
     from .ai.models import lstm
     t_max = t_max or lstm.T_MAX
     n = int(F.shape[0])
@@ -382,7 +389,8 @@ def sequences_core(cols: EventColumns, order, F, tt, t0, span, n_nodes, t_max=No
         order, F, tt = order[sel_ev], F[sel_ev], tt[sel_ev]
         n = int(F.shape[0])
     if n == 0:
-        return np.zeros((0, t_max, lstm.D_IN), np.float32), np.zeros(0, np.int32), np.zeros(0, np.int64)
+        empty = (np.zeros((0, t_max, lstm.D_IN), np.float32), np.zeros(0, np.int32), np.zeros(0, np.int64))
+        return empty + (np.zeros((0, t_max), np.int64),) if return_events else empty
     # group by file node, keeping time order inside a group
     by_file = np.argsort(F, kind="stable")
     Fg = F[by_file]
@@ -408,6 +416,10 @@ def sequences_core(cols: EventColumns, order, F, tt, t0, span, n_nodes, t_max=No
     pf = cols.path_flags[order][ev]
     seq[row, k, 11] = (pf & 1) != 0
     seq[row, k, 12] = (pf & 4) != 0
+    if return_events:
+        events = np.full((nodes.size, t_max), -1, np.int64)
+        events[row, k] = np.asarray(order, np.int64)[ev]
+        return seq, lengths, nodes.astype(np.int64), events
     return seq, lengths, nodes.astype(np.int64)
 
 

@@ -24,11 +24,14 @@ _SEQ_EVENT_SLOT = {"file_created": 0, "file_encrypt_start": 1, "file_encrypt_com
                    "openat": 4, "write": 5, "rename": 6}
 
 
-def file_sequences(events, g: G.TemporalGraph, t_max=lstm.T_MAX, observable=False):
+def file_sequences(events, g: G.TemporalGraph, t_max=lstm.T_MAX, observable=False, return_events=False):
     """Per-file event sequences for the LSTM (the last `t_max` events of each file node, oldest first).
-    Features (D_in = 16): one-hot event kind (8), log1p(size)/20, dt to the previous event of the file (s, clipped),
-    time since trace start / window, .lockbit flag, /tmp|/proc flag, 3 spare (the simulator's `phase` annotation is
-    ground truth, not an observable: it is deliberately NOT a feature, so wire-format traces give the same sequences)."""
+    Features (D_in = 16, named by lstm.FEATURE_NAMES): one-hot event kind (8), log1p(size)/20, dt to the previous event of
+    the file (s, clipped), time since trace start / window, .lockbit flag, /tmp|/proc flag, 3 spare (the simulator's
+    `phase` annotation is ground truth, not an observable: it is deliberately NOT a feature, so wire-format traces give
+    the same sequences).  return_events: a fourth array, int64 [n_files, t_max], the event of each step as an index into
+    graph.resolve_event_paths(events) (the ids graph_from_events' meta["edge_event"] / meta["event_info"] use), -1 at
+    padded steps."""
     merge = g.meta.get("merge_renames", True)
     keys = g.meta.get("file_keys")
     if keys is None:                                       # graphs from the columnar constructor: rebuild the key map from the names
@@ -38,19 +41,21 @@ def file_sequences(events, g: G.TemporalGraph, t_max=lstm.T_MAX, observable=Fals
     t0 = G._parse_ts(evs[0]["timestamp"]) if evs else 0.0
     span = max(G._parse_ts(evs[-1]["timestamp"]) - t0, 1e-6) if evs else 1.0
     per_file: dict = {}
-    for e in evs:
+    for j, e in enumerate(evs):
         node = keys.get(key_of(e["path"]))
         if node is None or g.meta["node_kind"][node] != 0:
             continue
-        per_file.setdefault(node, []).append(e)
+        per_file.setdefault(node, []).append((j, e))
     nodes = sorted(per_file)
     seq = np.zeros((len(nodes), t_max, lstm.D_IN), np.float32)
     lengths = np.zeros(len(nodes), np.int32)
+    step_event = np.full((len(nodes), t_max), -1, np.int64)
     for i, n in enumerate(nodes):
         es = per_file[n][-t_max:]
         lengths[i] = len(es)
         prev = None
-        for k, e in enumerate(es):
+        for k, (j, e) in enumerate(es):
+            step_event[i, k] = j
             t = G._parse_ts(e["timestamp"])
             slot = _SEQ_EVENT_SLOT.get(e["event"], 7)
             seq[i, k, G.OBSERVABLE_SLOT[slot] if observable else slot] = 1.0
@@ -60,6 +65,8 @@ def file_sequences(events, g: G.TemporalGraph, t_max=lstm.T_MAX, observable=Fals
             seq[i, k, 11] = 1.0 if ".lockbit" in e["path"] else 0.0
             seq[i, k, 12] = 1.0 if e["path"].startswith(("/tmp", "/proc")) else 0.0
             prev = t
+    if return_events:
+        return seq, lengths, np.asarray(nodes, np.int64), step_event
     return seq, lengths, np.asarray(nodes, np.int64)
 
 
@@ -80,6 +87,8 @@ class PipelineResult:
     actions: Actions | None = None    # the action set the plan was made over (cand[i] is the node of action i)
     evidence: dict | None = None      # run(explain=k): node id of each planned node step -> its explanation
                                       # (explain.explain_nodes + explain.attach_events); None when not asked for
+    sequence_evidence: dict | None = None   # run(explain_sequences=k): node id of each planned file step -> the BiLSTM
+                                            # explanation of its sequence (explain.explain_sequences); None when not asked for
 
 
 @dataclass
@@ -254,7 +263,8 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
         plan_steps=None, n_rollouts=4096, depth=50, iterations=16, device="cuda", exclude=None, commit_per_search=1,
         dist_ctx: DistContext | None = None, kill_candidates: bool = False, restore_candidates: bool = False,
         max_restores: int = 4, min_restore_files: int = 8, explain: int = 0,
-        explain_max_edges: int | None = None, explain_max_full_graph: int | None = None) -> PipelineResult:
+        explain_max_edges: int | None = None, explain_max_full_graph: int | None = None, explain_sequences: int = 0,
+        seq_events=None) -> PipelineResult:
     """seq/lengths/seq_nodes: LSTM inputs for (a superset of) the candidate file nodes (file_sequences()).
     seq may instead be a CALLABLE nodes -> (seq, lengths, nodes_with_sequences): the sequences are then built only for
     the top-A candidates (large windows: a million file nodes, a few thousand candidates); seq_nodes = the file nodes.
@@ -271,10 +281,16 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
     res.restores lists the applied restores.
     explain = k > 0: after planning, res.evidence holds each planned node's k strongest GraphSAGE-T edge attributions with
     their events (nerrf_b200.explain; a kill step explains its process node, restores carry none).  The plan is the
-    plan of explain=0.  One GPU only."""
+    plan of explain=0.  One GPU only.
+    explain_sequences = k > 0: res.sequence_evidence holds, for each planned file step, the k steps of its event sequence
+    that drove the BiLSTM's encrypt logit most (explain.explain_sequences), with their events; kills and restores carry
+    none.  seq_events: the event of each step of `seq` (int64 [len(seq), T], file_sequences(return_events=True)); a
+    callable `seq` is then called as seq(nodes, events=True) and returns a fourth value, the same for its sequences.
+    Events of both kinds of evidence are resolved in one g.meta["event_info"] call.  The plan is the plan of
+    explain_sequences=0.  One GPU only."""
     if restore_candidates and dist_ctx is not None and dist_ctx.world > 1:
         raise NotImplementedError("restore candidates are planned on one GPU (dist_ctx.world > 1 is not supported)")
-    if explain and dist_ctx is not None and dist_ctx.world > 1:
+    if (explain or explain_sequences) and dist_ctx is not None and dist_ctx.world > 1:
         raise NotImplementedError("explanations are computed on one GPU (dist_ctx.world > 1 is not supported)")
     dev = torch.device(device)
     tm = {}
@@ -303,20 +319,28 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
     sync(); tm["top_a"] = (time.perf_counter() - t0) * 1e3
 
     t0 = time.perf_counter()
+    ev_sel = None
     if callable(seq):
         want = candidates.cpu().numpy()
-        sq, ln, have = seq(want)                                       # sequences of the candidates only
+        if explain_sequences:
+            sq, ln, have, ev = seq(want, events=True)                  # ... and the event of every step
+        else:
+            sq, ln, have = seq(want)                                   # sequences of the candidates only
         if have is None:                                               # already in candidate order (device builder: CUDA tensors)
             seq_sel, len_sel = sq, ln
+            ev_sel = ev if explain_sequences else None
         else:                                                          # sorted by node id (host builder)
             pos = np.searchsorted(have, want)
             assert have.shape[0] == want.shape[0] and np.array_equal(have[pos], want), "every candidate file has events"
             seq_sel, len_sel = sq[pos], ln[pos]
+            ev_sel = ev[pos] if explain_sequences else None
         tm["sequences"] = (time.perf_counter() - t0) * 1e3
         t0 = time.perf_counter()
     else:
         cl = cand_local.cpu().numpy()
         seq_sel, len_sel = seq[cl], lengths[cl]
+        if explain_sequences and seq_events is not None:
+            ev_sel = np.asarray(seq_events)[cl]
     probs = _lstm_probs(seq_model, seq_sel, len_sel, dev, dist_ctx)
     sync(); tm["lstm"] = (time.perf_counter() - t0) * 1e3
 
@@ -402,16 +426,40 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
                 res.restores.append({"position": k, "dir": d, "dir_hash": int(r_dirs[i - n_kill]), "covers": [int(c) for c in covers]})
     if confidence is None and kill_candidates:
         res.kill_attribution = "writer" if edge_attack is None else "edges"
-    if explain:
+    if explain or explain_sequences:
         from . import explain as X
         t0 = time.perf_counter()
         todo = list(dict.fromkeys(res.plan_nodes))
-        kw = {}
-        if explain_max_edges is not None:
-            kw["max_edges_per_target"] = explain_max_edges
-        if explain_max_full_graph is not None:
-            kw["max_full_graph_targets"] = explain_max_full_graph
-        ex = X.explain_nodes(G.TemporalGraph(rp, col, ew, x, g.meta), model, todo, k=int(explain), **kw)
-        res.evidence = dict(zip(todo, X.attach_events(g, ex)))
-        sync(); tm["explain"] = (time.perf_counter() - t0) * 1e3
+        ex = []
+        if explain:
+            kw = {}
+            if explain_max_edges is not None:
+                kw["max_edges_per_target"] = explain_max_edges
+            if explain_max_full_graph is not None:
+                kw["max_full_graph_targets"] = explain_max_full_graph
+            ex = X.explain_nodes(G.TemporalGraph(rp, col, ew, x, g.meta), model, todo, k=int(explain), **kw)
+            sync()
+        t1 = time.perf_counter()
+        files, sx = [], None
+        if explain_sequences:
+            row = {int(c): j for j, c in enumerate(candidates.cpu().numpy().tolist())}   # a file step's row of seq_sel
+            files = [n for n in todo if n in row]
+            idx = np.asarray([row[n] for n in files], np.int64)
+            take = lambda a: a[torch.from_numpy(idx).to(a.device)] if torch.is_tensor(a) else np.asarray(a)[idx]
+            sx = X.explain_sequences(seq_model, take(seq_sel), take(len_sel), k=int(explain_sequences),
+                                     step_event=None if ev_sel is None else take(ev_sel))
+            sync()
+        t2 = time.perf_counter()
+        if sx is None:
+            ex = X.attach_events(g, ex)
+        else:
+            ex, sx = X.attach_events(g, ex, sx)                        # one event_info call for both kinds of evidence
+            res.sequence_evidence = dict(zip(files, sx))
+        if explain:
+            res.evidence = dict(zip(todo, ex))
+        t3 = time.perf_counter()
+        if explain:
+            tm["explain"] = (t1 - t0 + t3 - t2) * 1e3
+        if explain_sequences:
+            tm["explain_sequences"] = (t2 - t1 + (0.0 if explain else t3 - t2)) * 1e3
     return res

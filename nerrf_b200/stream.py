@@ -753,10 +753,12 @@ class DeviceStream:
             out.append(rec)
         return out
 
-    def sequences_device(self, g: G.TemporalGraph, only_nodes):
+    def sequences_device(self, g: G.TemporalGraph, only_nodes, events=False):
         """LSTM sequences of the given file nodes of window graph `g`, built ON THE DEVICE (nerrf_trace_sequences) from the
         resident columns and the graph's own CSR rows: -> (seq fp32 [A, T_MAX, 16], lengths int32 [A]) CUDA tensors in the
-        order of `only_nodes`.  Needs the two-edges-per-event graph of merge mode (g.meta['perm'])."""
+        order of `only_nodes`.  Needs the two-edges-per-event graph of merge mode (g.meta['perm']).
+        events=True: also the stream row of each step's event (int64 [A, T_MAX], -1 at padded steps; the ids of
+        g.meta["edge_event"] / event_records), from nerrf_trace_sequences_ex."""
         import ctypes as C
         from . import _lib
         from .ai.models import lstm
@@ -772,16 +774,19 @@ class DeviceStream:
         A = int(cand.shape[0])
         seq = torch.empty(A, lstm.T_MAX, lstm.D_IN, dtype=torch.float32, device=self.dev)
         ln = torch.empty(A, dtype=torch.int32, device=self.dev)
+        ev = torch.empty(A, lstm.T_MAX, dtype=torch.int64, device=self.dev) if events else None
         with torch.cuda.device(self.dev):
-            _lib.check(_lib.lib().nerrf_trace_sequences(_lib.ptr(cand), A, _lib.ptr(g.rowptr), int(g.rowptr.dtype == torch.int64),
-                                                        _lib.ptr(perm), _lib.ptr(self.d_order[lo:hi]), _lib.ptr(self.d_ts),
-                                                        _lib.ptr(self.d_slot), _lib.ptr(self.d_bytes), _lib.ptr(self.d_pf_raw),
-                                                        float(g.meta["t0"]), float(g.meta["span"]), lstm.T_MAX, _lib.ptr(seq),
-                                                        _lib.ptr(ln), _lib.current_stream_ptr()), "nerrf_trace_sequences")
-        return seq, ln
+            _lib.check(_lib.lib().nerrf_trace_sequences_ex(_lib.ptr(cand), A, _lib.ptr(g.rowptr), int(g.rowptr.dtype == torch.int64),
+                                                           _lib.ptr(perm), _lib.ptr(self.d_order[lo:hi]), _lib.ptr(self.d_ts),
+                                                           _lib.ptr(self.d_slot), _lib.ptr(self.d_bytes), _lib.ptr(self.d_pf_raw),
+                                                           float(g.meta["t0"]), float(g.meta["span"]), lstm.T_MAX, _lib.ptr(seq),
+                                                           _lib.ptr(ln), _lib.ptr(ev), _lib.current_stream_ptr()),
+                       "nerrf_trace_sequences_ex")
+        return (seq, ln, ev) if events else (seq, ln)
 
-    def sequences(self, g: G.TemporalGraph, only_nodes):
-        """LSTM sequences of the given file nodes of window graph `g` (ingest.sequences_core on the window's events)."""
+    def sequences(self, g: G.TemporalGraph, only_nodes, events=False):
+        """LSTM sequences of the given file nodes of window graph `g` (ingest.sequences_core on the window's events);
+        events=True: also the stream row of each step's event (sequences_core(return_events=True))."""
         if self.cols is None:
             from . import _lib
             raise _lib.NerrfError("a live stream builds its sequences on the device (sequences_device)")
@@ -790,7 +795,7 @@ class DeviceStream:
         if "_F_host" not in g.meta:
             g.meta["_F_host"] = self.node_f[self.d_order[lo:hi]].cpu().numpy().astype(np.int64)
         return ingest.sequences_core(self.cols, order, g.meta["_F_host"], self.ts_sorted[lo:hi], g.meta["t0"], g.meta["span"],
-                                     g.num_nodes, None, self.observable, only_nodes)
+                                     g.num_nodes, None, self.observable, only_nodes, events)
 
 
 @dataclass
@@ -805,6 +810,8 @@ class TickResult:
     restored: list = field(default_factory=list)   # directories this tick's plan restores from the snapshot
     evidence: dict = field(default_factory=dict)   # StreamingPlanner(explain=k): plan key of each node step this tick
                                                    # planned (as in `planned`, kills included) -> its explanation
+    sequence_evidence: dict = field(default_factory=dict)   # StreamingPlanner(explain_sequences=k): plan key of each file
+                                                            # step this tick planned -> the BiLSTM explanation of its sequence
 
 
 @dataclass
@@ -826,6 +833,7 @@ class StreamingPlanner:
     max_restores: int = 4
     min_restore_files: int = 8
     explain: int = 0               # k > 0: each tick's TickResult.evidence explains its new steps (pipeline.run(explain=k))
+    explain_sequences: int = 0     # k > 0: TickResult.sequence_evidence explains its new file steps' sequences (one GPU)
     device: str = "cuda"
     dist_ctx: object = None        # pipeline.DistContext for the multi-GPU form
     reverted: set = field(default_factory=set)
@@ -952,7 +960,7 @@ class StreamingPlanner:
         multi = ctx is not None and ctx.world > 1
         if multi and self.restore_candidates:
             raise NotImplementedError("restore candidates are planned on one GPU (dist_ctx.world > 1 is not supported)")
-        if multi and self.explain:
+        if multi and (self.explain or self.explain_sequences):
             raise NotImplementedError("explanations are computed on one GPU (dist_ctx.world > 1 is not supported)")
         lead = not multi or ctx.rank == 0
         dev = torch.device(self.device)
@@ -1024,8 +1032,11 @@ class StreamingPlanner:
         nodes = np.nonzero(kind == 0)[0]
 
         # LSTM sequences are built lazily, for the top-A candidates only (a window holds ~10^6 file nodes)
-        def seq(cand, g=g):
+        def seq(cand, g=g, events=False):
             if lead and not multi:                      # built on the device from the resident columns, in candidate order
+                if events:                              # (explain_sequences: one GPU, so never the multi-GPU branch below)
+                    sq_d, ln_d, ev_d = ds.sequences_device(g, cand, events=True)
+                    return sq_d, ln_d, None, ev_d
                 sq_d, ln_d = ds.sequences_device(g, cand)
                 return sq_d, ln_d, None
             if lead:
@@ -1037,7 +1048,7 @@ class StreamingPlanner:
                 return sq_t.cpu().numpy(), ln_t.cpu().numpy(), hv_t.cpu().numpy()
             return sq, ln, have
 
-        new, truncated, restored, evidence = [], False, [], {}
+        new, truncated, restored, evidence, seq_evidence = [], False, [], {}, {}
         for rnd in range(4):
             # a planning pass proposes at most 32 process kills (planner spec v1: guards live in state word 0); a tick
             # with more suspicious processes than that plans again over what is still unreverted
@@ -1053,7 +1064,8 @@ class StreamingPlanner:
                                depth=self.depth, iterations=self.iterations, device=self.device, exclude=skip,
                                commit_per_search=self.commit_per_search, dist_ctx=self.dist_ctx,
                                kill_candidates=self.kill_candidates, restore_candidates=self.restore_candidates,
-                               max_restores=self.max_restores, min_restore_files=self.min_restore_files, explain=self.explain)
+                               max_restores=self.max_restores, min_restore_files=self.min_restore_files, explain=self.explain,
+                               explain_sequences=self.explain_sequences)
             for k, v in res.timings_ms.items():
                 tm[k] = tm.get(k, 0.0) + float(v)
             got = []
@@ -1084,6 +1096,11 @@ class StreamingPlanner:
                     for n, nm in zip(res.plan_nodes, plan_names):
                         if key(n, nm) in fresh and key(n, nm) not in evidence:
                             evidence[key(n, nm)] = res.evidence.get(n)
+                if res.sequence_evidence is not None:
+                    fresh = set(got)
+                    for n, nm in zip(res.plan_nodes, plan_names):
+                        if key(n, nm) in fresh and key(n, nm) not in seq_evidence and n in res.sequence_evidence:
+                            seq_evidence[key(n, nm)] = res.sequence_evidence[n]
                 new += got
                 for r in res.restores:                         # a restored directory brings back every file it covers
                     cov = revert(r["covers"], names.take(r["covers"]))
@@ -1097,4 +1114,5 @@ class StreamingPlanner:
             truncated = truncated or bool(res.plan.truncated)
             if not more:
                 break
-        self.ticks.append(TickResult(t_hi - t0, n_events, g.num_nodes, g.num_edges, new, tm, truncated, restored, evidence))
+        self.ticks.append(TickResult(t_hi - t0, n_events, g.num_nodes, g.num_edges, new, tm, truncated, restored, evidence,
+                                     seq_evidence))

@@ -4,6 +4,7 @@ ROADMAP.md:28,86 -- scheduled, never written).
     python -m nerrf_b200.undo --trace events.pb   --weights weights.pt --out plan.json --shell plan.sh
     python -m nerrf_b200.undo --trace trace.jsonl --train-epochs 25    --out plan.json
     python -m nerrf_b200.undo --trace trace.jsonl --train-epochs 25    --out plan.json --explain 8
+    python -m nerrf_b200.undo --trace trace.jsonl --train-epochs 25    --out plan.json --explain-sequences 8
     python -m nerrf_b200.undo --trace nodeA=a.pb --trace nodeB=b.pb --weights weights.pt --out plan.json --shell-dir DIR
 
 trace: serialized nerrf.trace.EventBatch bytes (*.pb; proto/trace.proto:47-49, e.g. a buffered StreamEvents stream) or
@@ -55,8 +56,9 @@ def check_outputs(traces, shell, shell_dir):
         raise SystemExit("--shell-dir names its scripts by host: give the trace as --trace HOST=PATH")
 
 
-def load_hosts(paths, device="cuda"):
-    """several hosts' EventBatch files as one stream, source id k = the k-th file -> (graph, seq, lengths, seq_nodes, n)"""
+def load_hosts(paths, device="cuda", events=False):
+    """several hosts' EventBatch files as one stream, source id k = the k-th file -> (graph, seq, lengths, seq_nodes, n)
+    (events=True: and the event of each sequence step, last)"""
     parts = []
     for k, path in enumerate(paths):
         if not path.endswith(".pb"):
@@ -65,22 +67,22 @@ def load_hosts(paths, device="cuda"):
             parts.append(with_source(ingest.decode_event_batch(f.read()), k))
     cols = concat_columns(parts)
     g = ingest.graph_from_columns(cols, device=device, observable=True)
-    seq, lengths, nodes = ingest.sequences_from_columns(cols, observable=True)
-    return g, seq, lengths, nodes, cols.n
+    seq, lengths, nodes, *ev = ingest.sequences_from_columns(cols, observable=True, return_events=events)
+    return (g, seq, lengths, nodes, cols.n, *ev)
 
 
-def load_trace(path: str, device="cuda"):
-    """-> (graph, seq, lengths, seq_nodes, n_events)"""
+def load_trace(path: str, device="cuda", events=False):
+    """-> (graph, seq, lengths, seq_nodes, n_events) (events=True: and the event of each sequence step, last)"""
     if path.endswith(".jsonl") or path.endswith(".json"):
-        events = G.read_trace_jsonl(path)
-        g = G.graph_from_events(events, observable=True)          # the features ai/train.py trains on
-        seq, lengths, nodes = pipeline.file_sequences(events, g, observable=True)
-        return g, seq, lengths, nodes, len(events)
+        evs = G.read_trace_jsonl(path)
+        g = G.graph_from_events(evs, observable=True)             # the features ai/train.py trains on
+        seq, lengths, nodes, *ev = pipeline.file_sequences(evs, g, observable=True, return_events=events)
+        return (g, seq, lengths, nodes, len(evs), *ev)
     with open(path, "rb") as f:
         cols = ingest.decode_event_batch(f.read())
     g = ingest.graph_from_columns(cols, device=device, observable=True)
-    seq, lengths, nodes = ingest.sequences_from_columns(cols, observable=True)
-    return g, seq, lengths, nodes, cols.n
+    seq, lengths, nodes, *ev = ingest.sequences_from_columns(cols, observable=True, return_events=events)
+    return (g, seq, lengths, nodes, cols.n, *ev)
 
 
 def load_models(weights: str | None, train_epochs: int, layers: int = 2, log=print):
@@ -117,6 +119,8 @@ def main(argv=None) -> dict:
     ap.add_argument("--shell-dir", default=None, help="write DIR/<host>.sh per --trace HOST=PATH")
     ap.add_argument("--explain", type=int, default=0, metavar="K",
                     help="attach to every node step the K trace events whose edges drove its GraphSAGE-T score most")
+    ap.add_argument("--explain-sequences", type=int, default=0, metavar="K",
+                    help="attach to every file step the K events of its history that drove its BiLSTM encrypt score most")
     ap.add_argument("--device", default="cuda")
     a = ap.parse_args(argv)
     traces = parse_traces(a.trace)
@@ -126,15 +130,17 @@ def main(argv=None) -> dict:
         raise SystemExit("nerrf_b200.undo needs a CUDA device (no CPU fallback for the hot path)")
     log = lambda *m: print(*m, file=sys.stderr)
     t0 = time.perf_counter()
+    want_ev = a.explain_sequences > 0
     if hosts is None:
-        g, seq, lengths, nodes, n_events = load_trace(traces[0][1], a.device)
+        g, seq, lengths, nodes, n_events, *ev = load_trace(traces[0][1], a.device, events=want_ev)
     else:
-        g, seq, lengths, nodes, n_events = load_hosts([p for _, p in traces], a.device)
+        g, seq, lengths, nodes, n_events, *ev = load_hosts([p for _, p in traces], a.device, events=want_ev)
     t_ingest = (time.perf_counter() - t0) * 1e3
     model, scorer = load_models(a.weights, a.train_epochs, log=log)
     model.to(a.device); scorer.to(a.device)
     res = pipeline.run(g, seq, lengths, nodes, model, scorer, top_a=min(a.top_a, 4096), n_rollouts=a.rollouts, depth=a.depth,
-                       iterations=a.iterations, plan_steps=a.max_steps, device=a.device, explain=a.explain)
+                       iterations=a.iterations, plan_steps=a.max_steps, device=a.device, explain=a.explain,
+                       explain_sequences=a.explain_sequences, seq_events=ev[0] if ev else None)
     plan = emit.from_pipeline(g, res, attack_id=a.id, host_names=hosts)
     plan["stats"] = {"events": int(n_events), "nodes": int(g.num_nodes), "edges": int(g.num_edges),
                      "candidates": int(len(res.candidates)), "ingest_ms": t_ingest,
