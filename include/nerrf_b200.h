@@ -196,6 +196,41 @@ int nerrf_lstm_explain_steps(const float* seq, const float* dseq, const int32_t*
                              const int64_t* step_event, int k, int32_t* out_step, float* out_attr, int32_t* out_feature,
                              int64_t* out_event, nerrf_stream_t stream);
 
+/* ------------------------------------------------------------------ incidents (DESIGN.md 1.4)
+ * Flagged files and their owners: F = {v : node_kind[v] == 0 and score[v] >= tau} plus the file nodes `seeds` (int64
+ * [n_seeds], may repeat), in ascending node id -> out_files int32 [|F|].  Per flagged file f (row v = out_files[f] of the
+ * CSR-by-destination graph, rowptr int32 or int64):
+ *   owner o = the source of the last process in-edge of the row (edge_attack == NULL), or the process source with the
+ *     highest edge_attack[e] (NaN above every number), ties to the later position; -1 when the row has no process source;
+ *   first / last = the lowest / highest position of the row whose source is o (the row's first / last position when
+ *     o = -1, -1 when the row is empty); later = the positions p > first whose source is a process other than o (0 when
+ *     o = -1);
+ *   out_int int64 [n_nodes, 6] rows (o, first, last, later, edge_event[first], edge_event[last]) and out_real float64
+ *   [n_nodes, 2] rows (edge_time[first], edge_time[last]); events -1 and times NaN where the position is -1 or the array
+ *   is NULL.  Only the first |F| rows are written.
+ * The call waits for `stream` once, to return |F| in *n_flagged (host) and to report bad input as NERRF_ERR_INVALID:
+ * node_kind values other than 0 / 1, seeds outside [0, n_nodes) or not file nodes, any col id (all rowptr[n_nodes] of them) outside [0, n_nodes), tau NaN.
+ * One warp per flagged row.  workspace: nerrf_incident_files_workspace_bytes.  All pointers device except n_flagged. */
+int nerrf_incident_files_workspace_bytes(int64_t n_nodes, size_t* bytes);
+int nerrf_incident_files(const void* rowptr, int rowptr_is64, const int32_t* col, int64_t n_nodes, const int8_t* node_kind,
+                         const float* score, float tau, const int64_t* seeds, int64_t n_seeds, const float* edge_attack,
+                         const double* edge_time, const int64_t* edge_event, int32_t* out_files, int64_t* out_int,
+                         double* out_real, int64_t* n_flagged, void* workspace, size_t workspace_bytes, nerrf_stream_t stream);
+/* Incidents of the n_flagged files of nerrf_incident_files (files, file_int, file_real as it wrote them): one per key
+ * (node_source[file] (NULL = 0), owner), owner -1 = the source's unattributed incident.  Per incident, ordered by
+ * (onset, source, owner; NaN onsets after every number, owner -1 last): inc_int int64 [n_flagged, 7] rows (source, owner,
+ * offset of its files in grouped_files, n_files, onset event, end event, sum of `later`) and inc_real float64
+ * [n_flagged, 4] rows (onset = min file onset, ties to the lower node id; end = max file end, same ties; NaN times never
+ * win; sum of size_mb[file] as float64; max of score[file], NaN ignored).  grouped_files int32 [n_flagged]: each
+ * incident's files in ascending node id; file_incident int32 [n_flagged]: each flagged file's incident index;
+ * *n_incidents (device int32): the count.  Per-incident reductions run in a fixed lane order without atomics: two runs
+ * give the same bits.  Asynchronous; workspace: nerrf_incident_group_workspace_bytes.  All pointers device. */
+int nerrf_incident_group_workspace_bytes(int64_t n_flagged, size_t* bytes);
+int nerrf_incident_group(const int32_t* files, const int64_t* file_int, const double* file_real, int64_t n_flagged,
+                         const int32_t* node_source, const float* size_mb, const float* score, int32_t* n_incidents,
+                         int64_t* inc_int, double* inc_real, int32_t* grouped_files, int32_t* file_incident,
+                         void* workspace, size_t workspace_bytes, nerrf_stream_t stream);
+
 /* The normalised edge weights of the graph, for t_w above: a[e] = ew[e] * (1 / max(weight sum of e's destination row,
  * 1e-12)), edges in CSR-by-destination order (rowptr [n+1], int32 or int64 when rowptr_is64; ew, a [E]).  The weight sum
  * is taken in the order nerrf_sage_aggregate takes it, so the entries are the forward's to the bit.  No atomics:

@@ -41,6 +41,11 @@ SIGNATURES = {
                                               vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]),
     "nerrf_explain_topk": (C.c_int, [vp, C.c_int64, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]),
     "nerrf_lstm_explain_steps": (C.c_int, [vp, vp, vp, C.c_int64, C.c_int, C.c_int, vp, C.c_int, vp, vp, vp, vp, vp]),
+    "nerrf_incident_files_workspace_bytes": (C.c_int, [C.c_int64, C.POINTER(C.c_size_t)]),
+    "nerrf_incident_files": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, C.c_float, vp, C.c_int64, vp, vp, vp, vp, vp, vp,
+                                       C.POINTER(C.c_int64), vp, C.c_size_t, vp]),
+    "nerrf_incident_group_workspace_bytes": (C.c_int, [C.c_int64, C.POINTER(C.c_size_t)]),
+    "nerrf_incident_group": (C.c_int, [vp, vp, vp, C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]),
     "nerrf_sage_edge_head_bwd_workspace_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "nerrf_sage_edge_head_bwd": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, C.c_size_t,
                                            C.c_int64, C.c_int, vp]),

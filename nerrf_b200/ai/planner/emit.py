@@ -120,9 +120,34 @@ def evidence_fields(ex, host_names=None) -> dict:
     return r
 
 
+def incident_fields(inc, host_names=None) -> dict:
+    """The plan record of one incident (incident.incidents): {"id", "host", "process", "files" (node ids), "n_files",
+    "onset" / "end": {"time", "event"}, "size_mb", "later_other_events", "max_score"}; "hostile_name" when an event's
+    path or syscall holds a control character."""
+    hostile = False
+    r = {"id": str(inc["id"]), "host": None if inc.get("host") is None else check_host_name(inc["host"]),
+         "process": inc.get("process"), "files": [int(v) for v in inc["files"]], "n_files": int(inc["n_files"])}
+    for k in ("onset", "end"):
+        rec, bad = event_fields(inc.get(k + "_event"), host_names)
+        hostile = hostile or bad
+        r[k] = {"time": inc.get(k), "event": rec}
+    r.update(size_mb=float(inc["size_mb"]), later_other_events=int(inc["later_other_events"]), max_score=inc.get("max_score"))
+    if hostile:
+        r["hostile_name"] = True
+    return r
+
+
+def recovery_point(rec, host_names=None):
+    """A file's recovery point (pipeline.PipelineResult.file_recovery[node] = (onset, event, later)) -> (the plan field
+    {"before": onset, "event", "later_other_events"}, hostile)"""
+    onset, ev, later = rec
+    e, bad = event_fields(ev, host_names)
+    return {"before": onset, "event": e, "later_other_events": int(later)}, bad
+
+
 def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node_score=None, truncated=False,
               remaining_candidates=0, restores=None, hosts=None, evidence=None, host_names=None,
-              sequence_evidence=None) -> dict:
+              sequence_evidence=None, incidents=None, step_incident=None, file_recovery=None) -> dict:
     """names: node id -> path (TemporalGraph.meta['names']); plan_nodes: node ids to revert, in plan order
     (PipelineResult.plan_nodes); scores: Plan.scores (exact reward after each commit, scores[0] = before).
     truncated / remaining_candidates: the planner stopped at its step limit while improving candidates remained --
@@ -134,7 +159,12 @@ def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node
     evidence: node id -> explanation (pipeline.PipelineResult.evidence): each node step found there gets the fields of
     evidence_fields (host_names: source id -> host name for its events).  None: no evidence fields.
     sequence_evidence: node id -> sequence explanation (pipeline.PipelineResult.sequence_evidence): each file step found
-    there gets the fields of sequence_evidence_fields.  None: no sequence evidence fields.  to_shell reads neither."""
+    there gets the fields of sequence_evidence_fields.  None: no sequence evidence fields.
+    incidents / step_incident / file_recovery (pipeline.PipelineResult, run(incidents=True)): a top-level "incidents"
+    table (incident_fields), "incident" (id or None) on every node step, "incidents" (the ids of its covers) on a restore,
+    and "recovery_point" (recovery_point) on every file step found in file_recovery; a restore's is its earliest cover's
+    point (ties to the lower node id) with later_other_events summed over the covers.  None: none of these fields.
+    to_shell reads none of the evidence or incident fields."""
     host_of = (lambda n: check_host_name(hosts[int(n)])) if hosts is not None else None
     at = {int(r["position"]): r for r in (restores or [])}
     total = len(plan_nodes) + len(at)
@@ -151,6 +181,18 @@ def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node
                 step["host"] = on[0]
             if scores is not None and k + 1 < len(scores):
                 step["reward_after"] = float(scores[k + 1])
+            if step_incident is not None:
+                step["incidents"] = sorted({step_incident.get(int(c)) for c in r["covers"]} - {None})
+            if file_recovery is not None:
+                pts = sorted((file_recovery[int(c)][0], int(c)) for c in r["covers"]
+                             if int(c) in file_recovery and file_recovery[int(c)][0] is not None)
+                if pts:
+                    onset, ev, _ = file_recovery[pts[0][1]]
+                    later = sum(int(file_recovery[int(c)][2]) for c in r["covers"] if int(c) in file_recovery)
+                    rp_, bad = recovery_point((onset, ev, later), host_names)
+                    step["recovery_point"] = rp_
+                    if bad:
+                        step["hostile_name"] = True
             steps.append(step)
             continue
         n = int(next(nodes))
@@ -171,10 +213,19 @@ def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node
             if sf.pop("hostile_name", False):
                 step["hostile_name"] = True
             step.update(sf)
+        if step_incident is not None:
+            step["incident"] = step_incident.get(n)
+        if file_recovery is not None and n in file_recovery:
+            rp_, bad = recovery_point(file_recovery[n], host_names)
+            step["recovery_point"] = rp_
+            if bad:
+                step["hostile_name"] = True
         steps.append(step)
     out = {"version": PLAN_VERSION, "kind": "nerrf.undo_plan", "attack_id": attack_id, "steps": steps,
            "approve_if": "all_checks_pass" if not truncated else "all_checks_pass_and_operator_confirms_partial_plan",
            "truncated": bool(truncated), "remaining_candidates": int(remaining_candidates)}
+    if incidents is not None:
+        out["incidents"] = [incident_fields(i, host_names) for i in incidents]
     if scores:
         out["reward_before"] = float(scores[0])
         out["reward_after"] = float(scores[min(total, len(scores) - 1)])
@@ -221,4 +272,6 @@ def from_pipeline(g, result, attack_id=None, host_names=None) -> dict:
                      remaining_candidates=getattr(result.plan, "remaining_candidates", 0),
                      restores=getattr(result, "restores", None), hosts=hosts,
                      evidence=getattr(result, "evidence", None), host_names=host_names,
-                     sequence_evidence=getattr(result, "sequence_evidence", None))
+                     sequence_evidence=getattr(result, "sequence_evidence", None),
+                     incidents=getattr(result, "incidents", None), step_incident=getattr(result, "step_incident", None),
+                     file_recovery=getattr(result, "file_recovery", None))

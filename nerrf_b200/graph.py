@@ -340,10 +340,12 @@ def graph_from_events(events, merge_renames=True, window=None, observable=False)
     file_keys = {k[1]: v for k, v in node_id.items() if k[0] == "f"}      # merge key (or path) -> node, incl. rename aliases
     # edge_event: the event (index into the time-sorted, path-resolved events) that made each CSR edge
     edge_event = np.asarray(eid, np.int64)[np.lexsort((tt, dst))]
+    # edge_time: the trace-clock seconds of that event (float64, the time event_info reports), computed when asked for
+    edge_time = lambda: np.asarray([_parse_ts(e["timestamp"]) for e in evs], np.float64)[edge_event]
     return TemporalGraph(rowptr, col, ew, x, {"kind": "trace", "names": names, "node_kind": np.asarray(kinds),
                                               "label": y, "size_mb": size_mb, "t0": t0, "span": span,
                                               "file_keys": file_keys, "merge_renames": bool(merge_renames),
-                                              "edge_label": edge_label, "edge_event": edge_event,
+                                              "edge_label": edge_label, "edge_event": edge_event, "edge_time": edge_time,
                                               "event_info": lambda ids: [event_record(evs[int(i)]) for i in ids]})
 
 

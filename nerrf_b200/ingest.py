@@ -313,7 +313,11 @@ def graph_from_columns(cols: EventColumns, merge_renames=True, window=None, devi
                 return torch.zeros(0, dtype=torch.int64, device=perm.device)
             ev = up(np.repeat(order, 4)[keep], np.int64)                      # edge in constructor order -> event row
             return ev[perm.long() & 0xffffffff]
-        meta.update(edge_event=edge_event, event_info=lambda ids, cols=cols: column_event_records(cols, ids))
+
+        def edge_time(ts=ts):
+            """the trace-clock seconds (float64) of the event that made each CSR edge"""
+            return up(ts, np.float64)[edge_event()]
+        meta.update(edge_event=edge_event, edge_time=edge_time, event_info=lambda ids, cols=cols: column_event_records(cols, ids))
         lab = label.cpu().numpy().astype(np.int64)
         if observable:                                        # the kernel saw the folded slots: labels come from the annotations
             lab = (np.bincount(F[(raw_slot == 1) | (raw_slot == 2)], minlength=N) > 0).astype(np.int64)

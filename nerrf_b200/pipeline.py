@@ -89,6 +89,11 @@ class PipelineResult:
                                       # (explain.explain_nodes + explain.attach_events); None when not asked for
     sequence_evidence: dict | None = None   # run(explain_sequences=k): node id of each planned file step -> the BiLSTM
                                             # explanation of its sequence (explain.explain_sequences); None when not asked for
+    incidents: list | None = None     # run(incidents=True): the window's incidents (incident.incidents), onset order
+    step_incident: dict | None = None  # run(incidents=True): node id of each planned node step and of each file an applied
+                                       # restore covers -> its incident id (a kill: the incident its process owns, or None)
+    file_recovery: dict | None = None  # run(incidents=True): node id of each flagged file -> (onset, event record, later
+                                       # events of other processes)
 
 
 @dataclass
@@ -154,12 +159,21 @@ def process_kill_candidates(g: G.TemporalGraph, candidates: np.ndarray, max_kill
     ties to the latest edge: a backup agent or scanner that opened an encrypted file after the ransomware is then not
     taken for its writer.
     -> (pid_nodes [k], guard [A] = index into pid_nodes of the owner of each candidate file, or -1)."""
+    return _owners_to_kills(file_owners(g, candidates, edge_attack), max_kills)
+
+
+def file_owners(g: G.TemporalGraph, files, edge_attack=None) -> np.ndarray:
+    """The process node that owns each of `files` (int64 [len(files)], -1 when its row has no process source): the source
+    of its last process in-edge (rows are time-sorted: its last writer), or, given `edge_attack` (P(attack) [E] per CSR
+    edge), the process source in its row with the highest P(attack), ties to the later edge.  The attribution rule of
+    process_kill_candidates and of incidents (DESIGN.md 1.4)."""
     kind = torch.as_tensor(np.asarray(g.meta["node_kind"]))
     rp = (g.rowptr.cpu() if torch.is_tensor(g.rowptr) else torch.from_numpy(np.asarray(g.rowptr))).long()
     col = (g.col.cpu() if torch.is_tensor(g.col) else torch.from_numpy(np.asarray(g.col))).long()
-    cand = torch.from_numpy(np.asarray(candidates, np.int64))
+    cand = torch.from_numpy(np.asarray(files, np.int64))
     if edge_attack is not None:
-        return _owners_to_kills(_edge_owners(kind, rp, col, cand, np.asarray(edge_attack, np.float32)), max_kills)
+        ea = edge_attack.detach().cpu().numpy() if torch.is_tensor(edge_attack) else edge_attack
+        return _edge_owners(kind, rp, col, cand, np.asarray(ea, np.float32))
     # the most recent in-edge of a file node (rows are time-sorted) whose source is a process = its last writer
     owner = np.full(cand.shape[0], -1, np.int64)
     last = rp[cand + 1] - 1
@@ -171,7 +185,7 @@ def process_kill_candidates(g: G.TemporalGraph, candidates: np.ndarray, max_kill
         n = int(cand[i]); s_ = col[rp[n]:rp[n + 1]]; s_ = s_[kind[s_] == 1]
         if s_.numel():
             owner[i] = int(s_[-1])
-    return _owners_to_kills(owner, max_kills)
+    return owner
 
 
 def _owners_to_kills(owner: np.ndarray, max_kills: int):
@@ -264,7 +278,7 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
         dist_ctx: DistContext | None = None, kill_candidates: bool = False, restore_candidates: bool = False,
         max_restores: int = 4, min_restore_files: int = 8, explain: int = 0,
         explain_max_edges: int | None = None, explain_max_full_graph: int | None = None, explain_sequences: int = 0,
-        seq_events=None) -> PipelineResult:
+        seq_events=None, incidents: bool = False, incident_tau: float = 0.5, host_names=None) -> PipelineResult:
     """seq/lengths/seq_nodes: LSTM inputs for (a superset of) the candidate file nodes (file_sequences()).
     seq may instead be a CALLABLE nodes -> (seq, lengths, nodes_with_sequences): the sequences are then built only for
     the top-A candidates (large windows: a million file nodes, a few thousand candidates); seq_nodes = the file nodes.
@@ -287,7 +301,15 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
     none.  seq_events: the event of each step of `seq` (int64 [len(seq), T], file_sequences(return_events=True)); a
     callable `seq` is then called as seq(nodes, events=True) and returns a fourth value, the same for its sequences.
     Events of both kinds of evidence are resolved in one g.meta["event_info"] call.  The plan is the plan of
-    explain_sequences=0.  One GPU only."""
+    explain_sequences=0.  One GPU only.
+    incidents=True: res.incidents holds the window's incidents (DESIGN.md 1.4; incident.incidents over the files scored
+    >= incident_tau plus the plan's file steps and the files its applied restores cover, so every file step has one),
+    res.step_incident each planned node step's incident id and res.file_recovery each flagged file's recovery point.
+    Files are attributed by the edge head exactly when the kill attribution is (a model marked edge_head_trained).
+    host_names: source id -> host name, the prefix of incident ids on a graph of several sources.  The plan is the plan
+    of incidents=False.  One GPU only."""
+    if incidents and dist_ctx is not None and dist_ctx.world > 1:
+        raise NotImplementedError("incidents are computed on one GPU (dist_ctx.world > 1 is not supported)")
     if restore_candidates and dist_ctx is not None and dist_ctx.world > 1:
         raise NotImplementedError("restore candidates are planned on one GPU (dist_ctx.world > 1 is not supported)")
     if (explain or explain_sequences) and dist_ctx is not None and dist_ctx.world > 1:
@@ -357,11 +379,11 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
         r_dirs, r_coll, r_slot = propose_restores(node_dir_hashes(g, cand), file_dir, np.asarray(size_all_nodes, np.float32)[files],
                                                   is_cand, min(max_restores, 32), min_restore_files)
     n_restore = int(r_dirs.shape[0])
+    edge_attack = None                                                 # P(attack) per CSR edge when the edge head attributes
     if confidence is not None:
         p = np.asarray(confidence, np.float32)[cand]
         actions = Actions(p, size_mb, np.ones(a, np.float32))
     elif kill_candidates:
-        edge_attack = None
         if getattr(model, "edge_head_trained", False) and h_final is not None and model.edge_W is not None:
             # files are attributed to processes by the trained edge head (P(attack) of each CSR edge)
             _, el = model.heads(h_final, rp, col, return_edge_logits=True)
@@ -426,6 +448,9 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
                 res.restores.append({"position": k, "dir": d, "dir_hash": int(r_dirs[i - n_kill]), "covers": [int(c) for c in covers]})
     if confidence is None and kill_candidates:
         res.kill_attribution = "writer" if edge_attack is None else "edges"
+    if incidents:
+        tm["incidents"] = _label_incidents(res, g, (rp, col, ew, x), model, h_final, score, incident_tau, host_names,
+                                           edge_attack)
     if explain or explain_sequences:
         from . import explain as X
         t0 = time.perf_counter()
@@ -463,3 +488,35 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
         if explain_sequences:
             tm["explain_sequences"] = (t2 - t1 + (0.0 if explain else t3 - t2)) * 1e3
     return res
+
+
+def _label_incidents(res: PipelineResult, g, g_dev, model, h_final, score, tau, host_names, edge_attack=None):
+    """fill res.incidents / step_incident / file_recovery (run(incidents=True)) -> the time it took (ms).  edge_attack: the
+    P(attack) the kill attribution used, if it ran; otherwise the edge head's is computed here when the model has one."""
+    from . import incident as I
+    rp, col, ew, x = g_dev
+    t0 = time.perf_counter()
+    kind = np.asarray(g.meta["node_kind"])
+    seeds = [n for n in res.plan_nodes if kind[n] == 0] + [c for r in res.restores for c in r["covers"]]
+    if edge_attack is None and getattr(model, "edge_head_trained", False) and h_final is not None and model.edge_W is not None:
+        _, el = model.heads(h_final, rp, col, return_edge_logits=True)
+        edge_attack = torch.softmax(el, 1)[:, 0].contiguous()
+    recs, per_file = I.incidents(G.TemporalGraph(rp, col, ew, x, g.meta), score, tau=tau, seeds=np.unique(np.asarray(seeds, np.int64)),
+                                 edge_attack=edge_attack, host_names=host_names, return_files=True)
+    res.incidents = recs
+    res.step_incident = step_incidents(res.plan_nodes, res.restores, kind, recs, per_file)
+    res.file_recovery = {v: (f["onset"], f["event"], f["later"]) for v, f in per_file.items()}
+    torch.cuda.synchronize()
+    return (time.perf_counter() - t0) * 1e3
+
+
+def step_incidents(plan_nodes, restores, node_kind, recs, per_file) -> dict:
+    """node id -> incident id, for every planned node step (a file: its own incident; a kill: the incident whose owner is
+    the killed process, or None) and every file an applied restore covers (covered files are not plan nodes: the emitter
+    labels a restore with its covers' incidents)"""
+    by_owner = {r["owner"]: r["id"] for r in recs if r["owner"] >= 0}
+    out = {int(n): (per_file[int(n)]["incident"] if node_kind[n] == 0 else by_owner.get(int(n))) for n in plan_nodes}
+    for r in restores:
+        for c in r["covers"]:
+            out[int(c)] = per_file[int(c)]["incident"]
+    return out

@@ -721,7 +721,11 @@ class DeviceStream:
                 return torch.zeros(0, dtype=torch.int64, device=self.dev)
             rank = torch.arange(nw, device=self.dev).repeat_interleave(per_event)
             return sel[(rank if keep is None else rank[keep])[perm.long() & 0xffffffff]]
-        meta.update(edge_event=edge_event, event_info=self.event_records)
+
+        def edge_time():
+            """the trace-clock seconds (float64) of the event that made each CSR edge, gathered on the device"""
+            return self.d_ts[edge_event()]
+        meta.update(edge_event=edge_event, edge_time=edge_time, event_info=self.event_records)
         if edge_labels:
             meta["edge_label"] = G.edge_labels_device(P, F, self.d_raw_slot[sel], rowptr, col, N)
         return G.TemporalGraph(rowptr, col, ew, x, meta)
@@ -812,6 +816,10 @@ class TickResult:
                                                    # planned (as in `planned`, kills included) -> its explanation
     sequence_evidence: dict = field(default_factory=dict)   # StreamingPlanner(explain_sequences=k): plan key of each file
                                                             # step this tick planned -> the BiLSTM explanation of its sequence
+    incidents: dict = field(default_factory=dict)   # StreamingPlanner(incidents=True): incident id -> this tick's record
+                                                    # (incident.incidents; "files" as plan keys)
+    step_incident: dict = field(default_factory=dict)   # StreamingPlanner(incidents=True): plan key of each step this tick
+                                                        # planned (as in `planned`, kills included) -> its incident id
 
 
 @dataclass
@@ -834,6 +842,11 @@ class StreamingPlanner:
     min_restore_files: int = 8
     explain: int = 0               # k > 0: each tick's TickResult.evidence explains its new steps (pipeline.run(explain=k))
     explain_sequences: int = 0     # k > 0: TickResult.sequence_evidence explains its new file steps' sequences (one GPU)
+    incidents: object = False      # True: ticks label their steps with incidents (pipeline.run(incidents=True), one GPU);
+                                   # then, from construction on, the running incidents: id -> {"id", "host", "process",
+                                   # "onset" / "onset_event" (min over ticks), "end" / "end_event" (max), "files" (union
+                                   # of plan keys), "n_files"}
+    incident_tau: float = 0.5
     device: str = "cuda"
     dist_ctx: object = None        # pipeline.DistContext for the multi-GPU form
     reverted: set = field(default_factory=set)
@@ -852,6 +865,10 @@ class StreamingPlanner:
     _host_keys: bool = None        # plan names are (host, name) pairs: fixed by the first tick, for the planner's lifetime
     _t0: float = None
     _t_hi: float = None
+
+    def __post_init__(self):
+        if isinstance(self.incidents, bool):
+            self.incidents = {} if self.incidents else None
 
     def add_source(self, name: str) -> int:
         """Register a source (a host's tracker stream) -> its id (the next free one; an existing name keeps its id).
@@ -962,6 +979,8 @@ class StreamingPlanner:
             raise NotImplementedError("restore candidates are planned on one GPU (dist_ctx.world > 1 is not supported)")
         if multi and (self.explain or self.explain_sequences):
             raise NotImplementedError("explanations are computed on one GPU (dist_ctx.world > 1 is not supported)")
+        if multi and self.incidents is not None:
+            raise NotImplementedError("incidents are computed on one GPU (dist_ctx.world > 1 is not supported)")
         lead = not multi or ctx.rank == 0
         dev = torch.device(self.device)
         if multi:
@@ -1048,7 +1067,15 @@ class StreamingPlanner:
                 return sq_t.cpu().numpy(), ln_t.cpu().numpy(), hv_t.cpu().numpy()
             return sq, ln, have
 
-        new, truncated, restored, evidence, seq_evidence = [], False, [], {}, {}
+        new, truncated, restored, evidence, seq_evidence, tick_inc, step_inc = [], False, [], {}, {}, {}, {}
+        tick_nodes = {}                                  # incident id -> node ids of its tick record
+        want_inc = self.incidents is not None
+        if lead and self._host_keys is None:             # decided once per planner, so reverted / killed hold one form
+            self._host_keys = len(self.sources) > 1 or ds.multi_source
+        inc_hosts = None
+        if want_inc and lead and self._host_keys:
+            node_src = np.asarray(g.meta["node_source"])
+            inc_hosts = [self.host_name(s_) for s_ in range(max(len(self._names), int(node_src.max(initial=0)) + 1))]
         for rnd in range(4):
             # a planning pass proposes at most 32 process kills (planner spec v1: guards live in state word 0); a tick
             # with more suspicious processes than that plans again over what is still unreverted
@@ -1065,14 +1092,13 @@ class StreamingPlanner:
                                commit_per_search=self.commit_per_search, dist_ctx=self.dist_ctx,
                                kill_candidates=self.kill_candidates, restore_candidates=self.restore_candidates,
                                max_restores=self.max_restores, min_restore_files=self.min_restore_files, explain=self.explain,
-                               explain_sequences=self.explain_sequences)
+                               explain_sequences=self.explain_sequences, incidents=want_inc, incident_tau=self.incident_tau,
+                               host_names=inc_hosts)
             for k, v in res.timings_ms.items():
                 tm[k] = tm.get(k, 0.0) + float(v)
             got = []
             if lead:
                 node_src = g.meta.get("node_source")
-                if self._host_keys is None:              # decided once per planner, so reverted / killed hold one form
-                    self._host_keys = len(self.sources) > 1 or ds.multi_source
                 multi_src = self._host_keys
                 # several sources: a file or process is named (host, name), and its hash is qualified by its source
                 key = (lambda n, nm: (self.host_name(int(node_src[n])), nm)) if multi_src else (lambda n, nm: nm)
@@ -1101,6 +1127,8 @@ class StreamingPlanner:
                     for n, nm in zip(res.plan_nodes, plan_names):
                         if key(n, nm) in fresh and key(n, nm) not in seq_evidence and n in res.sequence_evidence:
                             seq_evidence[key(n, nm)] = res.sequence_evidence[n]
+                if res.incidents is not None:
+                    self._note_incidents(res, g, names, key, set(got) | set(fresh_kills), plan_names, tick_inc, tick_nodes, step_inc)
                 new += got
                 for r in res.restores:                         # a restored directory brings back every file it covers
                     cov = revert(r["covers"], names.take(r["covers"]))
@@ -1115,4 +1143,50 @@ class StreamingPlanner:
             if not more:
                 break
         self.ticks.append(TickResult(t_hi - t0, n_events, g.num_nodes, g.num_edges, new, tm, truncated, restored, evidence,
-                                     seq_evidence))
+                                     seq_evidence, tick_inc, step_inc))
+
+    _RUNNING_FIELDS = ("id", "host", "process", "onset", "onset_event", "end", "end_event", "files", "n_files")
+
+    def _note_incidents(self, res, g, names, key, fresh, plan_names, tick_inc, tick_nodes, step_inc):
+        """this planning pass's incidents -> the tick's records (files as plan keys), the fresh steps' incident ids, and the
+        running records.  A later pass of the same tick (same window, more seeds) folds its new files into the tick's
+        record: n_files, size_mb, later_other_events and max_score over the union, onset min, end max.  Running records
+        keep the fields that fold across windows: onset min, end max, files (plan keys) union."""
+        size = np.asarray(g.meta["size_mb"], np.float32)
+        score = res.node_score.detach().cpu().numpy()
+        for r in res.incidents:
+            files = [key(v, nm) for v, nm in zip(r["files"], names.take(r["files"]))]
+            rec = dict(r, files=files)
+            if r["id"] not in tick_inc:
+                tick_inc[r["id"]] = rec
+                tick_nodes[r["id"]] = set(r["files"])
+            else:
+                t = tick_inc[r["id"]]
+                extra = sorted(set(r["files"]) - tick_nodes[r["id"]])
+                tick_nodes[r["id"]].update(extra)
+                _fold_span(t, rec)
+                t["files"] = t["files"] + [key(v, nm) for v, nm in zip(extra, names.take(extra))]
+                t["n_files"] = len(t["files"])
+                t["size_mb"] = float(t["size_mb"]) + sum(float(size[v]) for v in extra)
+                t["later_other_events"] = int(t["later_other_events"]) + sum(int(res.file_recovery[v][2]) for v in extra)
+                ms = [float(score[v]) for v in extra if not np.isnan(score[v])] + ([] if t["max_score"] is None else [t["max_score"]])
+                t["max_score"] = max(ms) if ms else None
+            run = self.incidents.get(r["id"])
+            if run is None:
+                run = self.incidents[r["id"]] = {k: rec[k] for k in self._RUNNING_FIELDS}
+                run["files"] = []
+            _fold_span(run, rec)
+            run["files"] = sorted(set(run["files"]) | set(files), key=str)
+            run["n_files"] = len(run["files"])
+        for n, nm in zip(res.plan_nodes, plan_names):
+            k = key(n, nm)
+            if k in fresh and k not in step_inc:
+                step_inc[k] = res.step_incident.get(int(n))
+
+
+def _fold_span(into: dict, rec: dict):
+    """an incident record's onset / end widened by another record of the same incident (earliest onset, latest end)"""
+    if rec["onset"] is not None and (into["onset"] is None or rec["onset"] < into["onset"]):
+        into["onset"], into["onset_event"] = rec["onset"], rec["onset_event"]
+    if rec["end"] is not None and (into["end"] is None or rec["end"] > into["end"]):
+        into["end"], into["end_event"] = rec["end"], rec["end_event"]

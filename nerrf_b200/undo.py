@@ -6,6 +6,8 @@ ROADMAP.md:28,86 -- scheduled, never written).
     python -m nerrf_b200.undo --trace trace.jsonl --train-epochs 25    --out plan.json --explain 8
     python -m nerrf_b200.undo --trace trace.jsonl --train-epochs 25    --out plan.json --explain-sequences 8
     python -m nerrf_b200.undo --trace nodeA=a.pb --trace nodeB=b.pb --weights weights.pt --out plan.json --shell-dir DIR
+    python -m nerrf_b200.undo --trace events.pb   --weights weights.pt --out plan.json --incidents
+    python -m nerrf_b200.undo --trace events.pb   --weights weights.pt --out plan.json --incident pid:454
 
 trace: serialized nerrf.trace.EventBatch bytes (*.pb; proto/trace.proto:47-49, e.g. a buffered StreamEvents stream) or
 the simulator's TRACE json lines (*.jsonl; benchmarks/m1/scripts/sim_lockbit_m1.py:24-36).  Stages: ingest -> temporal
@@ -17,14 +19,21 @@ are per host (source ids in argument order); every step of the plan names its "h
 DIR/<host>.sh per host (--shell is refused: one script would hold every host's commands, and the hosts share file
 names).  A bare `--trace PATH`, or a single `--trace HOST=PATH`, is one source, as before: no host fields, and
 --shell-dir needs the HOST name.
+
+--incidents groups the plan's steps by the process that attacked their files (DESIGN.md 1.4): a top-level "incidents"
+table, the "incident" of every step and the "recovery_point" of every file step.  --incident ID plans that incident
+alone (ids are "pid:N", "unattributed", or "HOST/pid:N" with several hosts): the full plan is labelled first, then
+planned again with every file outside the incident excluded.
 """
 from __future__ import annotations
 
 import argparse
+import math
 import os
 import sys
 import time
 
+import numpy as np
 import torch
 
 from . import graph as G, ingest, pipeline
@@ -54,6 +63,17 @@ def check_outputs(traces, shell, shell_dir):
         raise SystemExit("--shell with several --trace HOST=PATH: use --shell-dir (one script per host)")
     if shell_dir and traces[0][0] is None:
         raise SystemExit("--shell-dir names its scripts by host: give the trace as --trace HOST=PATH")
+
+
+def check_incident_args(a):
+    """--incident-threshold needs --incidents or --incident, and is a number; --incident takes a non-empty id"""
+    if a.incident_threshold is not None:
+        if not (a.incidents or a.incident is not None):
+            raise SystemExit("--incident-threshold needs --incidents or --incident ID")
+        if math.isnan(a.incident_threshold):
+            raise SystemExit("--incident-threshold must be a number")
+    if a.incident is not None and not a.incident:
+        raise SystemExit("--incident needs an incident id (pid:N, unattributed, or HOST/pid:N)")
 
 
 def load_hosts(paths, device="cuda", events=False):
@@ -121,10 +141,16 @@ def main(argv=None) -> dict:
                     help="attach to every node step the K trace events whose edges drove its GraphSAGE-T score most")
     ap.add_argument("--explain-sequences", type=int, default=0, metavar="K",
                     help="attach to every file step the K events of its history that drove its BiLSTM encrypt score most")
+    ap.add_argument("--incidents", action="store_true",
+                    help="group the steps into incidents (one per attacking process) with per-file recovery points")
+    ap.add_argument("--incident-threshold", type=float, default=None, metavar="T",
+                    help="anomaly score at or above which a file belongs to an incident (default 0.5)")
+    ap.add_argument("--incident", default=None, metavar="ID", help="plan only the incident ID (pid:N, or HOST/pid:N)")
     ap.add_argument("--device", default="cuda")
     a = ap.parse_args(argv)
     traces = parse_traces(a.trace)
     check_outputs(traces, a.shell, a.shell_dir)
+    check_incident_args(a)
     hosts = [h for h, _ in traces] if len(traces) > 1 else None     # host fields only with several sources
     if not torch.cuda.is_available():
         raise SystemExit("nerrf_b200.undo needs a CUDA device (no CPU fallback for the hot path)")
@@ -138,10 +164,23 @@ def main(argv=None) -> dict:
     t_ingest = (time.perf_counter() - t0) * 1e3
     model, scorer = load_models(a.weights, a.train_epochs, log=log)
     model.to(a.device); scorer.to(a.device)
-    res = pipeline.run(g, seq, lengths, nodes, model, scorer, top_a=min(a.top_a, 4096), n_rollouts=a.rollouts, depth=a.depth,
-                       iterations=a.iterations, plan_steps=a.max_steps, device=a.device, explain=a.explain,
-                       explain_sequences=a.explain_sequences, seq_events=ev[0] if ev else None)
-    plan = emit.from_pipeline(g, res, attack_id=a.id, host_names=hosts)
+    want_inc = a.incidents or a.incident is not None
+    tau = 0.5 if a.incident_threshold is None else a.incident_threshold
+    run = lambda exclude=None: pipeline.run(g, seq, lengths, nodes, model, scorer, top_a=min(a.top_a, 4096), n_rollouts=a.rollouts,
+                                            depth=a.depth, iterations=a.iterations, plan_steps=a.max_steps, device=a.device,
+                                            explain=a.explain, explain_sequences=a.explain_sequences,
+                                            seq_events=ev[0] if ev else None, exclude=exclude, incidents=want_inc,
+                                            incident_tau=tau, host_names=hosts)
+    res = run()
+    attack_id = a.id
+    if a.incident is not None:
+        known = {r["id"]: r for r in (res.incidents or [])}            # None: no candidate file had a sequence
+        if a.incident not in known:
+            raise SystemExit("unknown incident %r; this trace's incidents: %s" % (a.incident, ", ".join(known) or "(none)"))
+        mine = np.asarray(known[a.incident]["files"], np.int64)
+        res = run(exclude=~np.isin(np.asarray(nodes, np.int64), mine))   # every file outside the incident is excluded
+        attack_id = a.incident if a.id is None else a.id
+    plan = emit.from_pipeline(g, res, attack_id=attack_id, host_names=hosts)
     plan["stats"] = {"events": int(n_events), "nodes": int(g.num_nodes), "edges": int(g.num_edges),
                      "candidates": int(len(res.candidates)), "ingest_ms": t_ingest,
                      "timings_ms": {k: float(v) for k, v in res.timings_ms.items()}}
