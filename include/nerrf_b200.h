@@ -231,6 +231,39 @@ int nerrf_incident_group(const int32_t* files, const int64_t* file_int, const do
                          int64_t* inc_int, double* inc_real, int32_t* grouped_files, int32_t* file_incident,
                          void* workspace, size_t workspace_bytes, nerrf_stream_t stream);
 
+/* ------------------------------------------------------------------ contamination (DESIGN.md 1.5)
+ * Time-respecting causal closure over a CSR-by-destination graph (rowptr int32 or int64, col, node_kind 0 file /
+ * 1 process as nerrf_incident_files).  Edge p of row v with source u = col[p] is open when its flow byte edge_flow[p]
+ * (bit 0 process -> file, bit 1 file -> process; nerrf_trace_flow_class) has the bit of the pair's direction and
+ * edge_time[p] (float64) is not NaN.  Seeds: distinct node ids (int64 [n_seeds]) with a seed time (float64, not NaN,
+ * -inf / +inf allowed) and a label (int32 >= 0).
+ *   phase 1: T0 = seed time (+inf elsewhere); Jacobi rounds: the (t, position)-smallest open edge of a row with
+ *            T[col[p]] <= t_p replaces T[v] when t_p < T[v]; at most max_hops rounds (-1: until a round changes nothing);
+ *   phase 2: level 0 = the seeds with T = their seed time; level k + 1 = the unlevelled nodes with T < +inf and a tight
+ *            in-edge (open, T[col[p]] <= t_p = T[v]) from a level-k node; pred = the lowest such position, label =
+ *            label[col[pred]].
+ * Outputs, over the levelled nodes in ascending node id (n_nodes capacity each): out_nodes int32, out_time float64 (T),
+ * out_level int32, out_pred int64 (-1 at level 0), out_label int32; *n_tainted, *n_rounds (rounds run) and *n_levels
+ * (non-empty levels) on the host; stage_ms (host double [4], may be NULL): the host-clock milliseconds of validation,
+ * phase 1, phase 2 and compaction, each ending in a stream wait.  The call waits once after validation, once per round
+ * and per level, and once after compaction.  Bad input
+ * is NERRF_ERR_INVALID: col ids outside [0, n_nodes) (all rowptr[n_nodes] of them), node_kind other than 0 / 1, flow
+ * bytes above 3, seed ids out of range or repeated, NaN seed times, negative labels, max_hops < -1.  Results are
+ * functions of the inputs alone (no atomics on values): two runs give the same bits.
+ * workspace: nerrf_taint_closure_workspace_bytes.  All pointers device except the counts and stage_ms. */
+int nerrf_taint_closure_workspace_bytes(int64_t n_nodes, size_t* bytes);
+int nerrf_taint_closure(const void* rowptr, int rowptr_is64, const int32_t* col, int64_t n_nodes, const int8_t* node_kind,
+                        const uint8_t* edge_flow, const double* edge_time, const int64_t* seeds, const double* seed_time,
+                        const int32_t* seed_label, int64_t n_seeds, int max_hops, int32_t* out_nodes, double* out_time,
+                        int32_t* out_level, int64_t* out_pred, int32_t* out_label, int64_t* n_tainted, int32_t* n_rounds,
+                        int32_t* n_levels, double* stage_ms, void* workspace, size_t workspace_bytes, nerrf_stream_t stream);
+/* The flow class of every event (the table of DESIGN.md 1.5) from its raw event slot (uint8), open flags and return
+ * value: nerrf_trace_flow_class takes host columns (flags int64), nerrf_trace_flow_class_device device columns (flags
+ * int32, the live decoder's); both evaluate the same definition.  The device call is asynchronous. */
+int nerrf_trace_flow_class(const uint8_t* event_slot, const int64_t* flags, const int64_t* ret_val, int64_t n, uint8_t* flow_out);
+int nerrf_trace_flow_class_device(const uint8_t* event_slot, const int32_t* flags, const int64_t* ret_val, int64_t n,
+                                  uint8_t* flow_out, nerrf_stream_t stream);
+
 /* The normalised edge weights of the graph, for t_w above: a[e] = ew[e] * (1 / max(weight sum of e's destination row,
  * 1e-12)), edges in CSR-by-destination order (rowptr [n+1], int32 or int64 when rowptr_is64; ew, a [E]).  The weight sum
  * is taken in the order nerrf_sage_aggregate takes it, so the entries are the forward's to the bit.  No atomics:

@@ -46,6 +46,11 @@ SIGNATURES = {
                                        C.POINTER(C.c_int64), vp, C.c_size_t, vp]),
     "nerrf_incident_group_workspace_bytes": (C.c_int, [C.c_int64, C.POINTER(C.c_size_t)]),
     "nerrf_incident_group": (C.c_int, [vp, vp, vp, C.c_int64, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]),
+    "nerrf_taint_closure_workspace_bytes": (C.c_int, [C.c_int64, C.POINTER(C.c_size_t)]),
+    "nerrf_taint_closure": (C.c_int, [vp, C.c_int, vp, C.c_int64, vp, vp, vp, vp, vp, vp, C.c_int64, C.c_int, vp, vp, vp, vp, vp,
+                                      C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.POINTER(C.c_int32), vp, vp, C.c_size_t, vp]),
+    "nerrf_trace_flow_class": (C.c_int, [vp, vp, vp, C.c_int64, vp]),
+    "nerrf_trace_flow_class_device": (C.c_int, [vp, vp, vp, C.c_int64, vp, vp]),
     "nerrf_sage_edge_head_bwd_workspace_bytes": (C.c_int, [C.c_int64, C.c_int, C.POINTER(C.c_size_t)]),
     "nerrf_sage_edge_head_bwd": (C.c_int, [vp, vp, vp, vp, C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, C.c_size_t,
                                            C.c_int64, C.c_int, vp]),

@@ -137,6 +137,28 @@ def incident_fields(inc, host_names=None) -> dict:
     return r
 
 
+def contaminated_fields(c, host_names=None) -> dict:
+    """The plan record of one contaminated node (taint.contamination): {"node", "name", "kind", "since", "since_event",
+    "hops", "via" (the events that carried the taint to it, oldest first)}; a file also gets "recovery_point":
+    {"before": since, "event": since_event} (restoring it to before the event that tainted it).  "hostile_name" when its
+    name or any event's path or syscall holds a control character."""
+    ev, hostile = event_fields(c.get("since_event"), host_names)
+    via = []
+    for e in c.get("via", []):
+        rec, bad = event_fields(e, host_names)
+        hostile = hostile or bad
+        via.append(rec)
+    name = None if c.get("name") is None else str(c["name"])
+    hostile = hostile or (name is not None and _has_control_chars(name))
+    r = {"node": int(c["node"]), "name": name, "kind": str(c["kind"]), "since": float(c["since"]), "since_event": ev,
+         "hops": int(c["hops"]), "via": via}
+    if r["kind"] == "file":
+        r["recovery_point"] = {"before": r["since"], "event": ev}
+    if hostile:
+        r["hostile_name"] = True
+    return r
+
+
 def recovery_point(rec, host_names=None):
     """A file's recovery point (pipeline.PipelineResult.file_recovery[node] = (onset, event, later)) -> (the plan field
     {"before": onset, "event", "later_other_events"}, hostile)"""
@@ -147,7 +169,7 @@ def recovery_point(rec, host_names=None):
 
 def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node_score=None, truncated=False,
               remaining_candidates=0, restores=None, hosts=None, evidence=None, host_names=None,
-              sequence_evidence=None, incidents=None, step_incident=None, file_recovery=None) -> dict:
+              sequence_evidence=None, incidents=None, step_incident=None, file_recovery=None, contamination=None) -> dict:
     """names: node id -> path (TemporalGraph.meta['names']); plan_nodes: node ids to revert, in plan order
     (PipelineResult.plan_nodes); scores: Plan.scores (exact reward after each commit, scores[0] = before).
     truncated / remaining_candidates: the planner stopped at its step limit while improving candidates remained --
@@ -164,6 +186,8 @@ def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node
     table (incident_fields), "incident" (id or None) on every node step, "incidents" (the ids of its covers) on a restore,
     and "recovery_point" (recovery_point) on every file step found in file_recovery; a restore's is its earliest cover's
     point (ties to the lower node id) with later_other_events summed over the covers.  None: none of these fields.
+    contamination: incident id -> contaminated nodes (pipeline.PipelineResult.contamination): each incident of the table
+    gets "contaminated" (contaminated_fields, [] when it reached nothing).  None: no such field.
     to_shell reads none of the evidence or incident fields."""
     host_of = (lambda n: check_host_name(hosts[int(n)])) if hosts is not None else None
     at = {int(r["position"]): r for r in (restores or [])}
@@ -226,6 +250,9 @@ def undo_plan(names, plan_nodes, scores=None, attack_id=None, size_mb=None, node
            "truncated": bool(truncated), "remaining_candidates": int(remaining_candidates)}
     if incidents is not None:
         out["incidents"] = [incident_fields(i, host_names) for i in incidents]
+        if contamination is not None:
+            for rec in out["incidents"]:
+                rec["contaminated"] = [contaminated_fields(c, host_names) for c in contamination.get(rec["id"], [])]
     if scores:
         out["reward_before"] = float(scores[0])
         out["reward_after"] = float(scores[min(total, len(scores) - 1)])
@@ -274,4 +301,5 @@ def from_pipeline(g, result, attack_id=None, host_names=None) -> dict:
                      evidence=getattr(result, "evidence", None), host_names=host_names,
                      sequence_evidence=getattr(result, "sequence_evidence", None),
                      incidents=getattr(result, "incidents", None), step_incident=getattr(result, "step_incident", None),
-                     file_recovery=getattr(result, "file_recovery", None))
+                     file_recovery=getattr(result, "file_recovery", None),
+                     contamination=getattr(result, "contamination", None))

@@ -12,7 +12,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(CSRC, "libnerrf_b200.so")
-SOURCES = ["api.cu", "sage.cu", "sage_umma.cu", "sage_bwd.cu", "sage_edge_bwd.cu", "explain.cu", "incident.cu", "mcts.cu", "lstm.cu", "lstm_bwd.cu", "lstm_umma.cu", "graph.cu", "ingest.cu", "intern_device.cu", "live_stream.cu"]
+SOURCES = ["api.cu", "sage.cu", "sage_umma.cu", "sage_bwd.cu", "sage_edge_bwd.cu", "explain.cu", "incident.cu", "taint.cu", "mcts.cu", "lstm.cu", "lstm_bwd.cu", "lstm_umma.cu", "graph.cu", "ingest.cu", "intern_device.cu", "live_stream.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

@@ -171,6 +171,14 @@ extern "C" int nerrf_trace_path_flags(const int64_t* off, const uint8_t* data, i
     return NERRF_OK;
 }
 
+// information-flow class of every event (wire::flow_class; DESIGN.md 1.5) from host columns
+extern "C" int nerrf_trace_flow_class(const uint8_t* event_slot, const int64_t* flags, const int64_t* ret_val, int64_t n,
+                                      uint8_t* flow_out) {
+    NERRF_REQUIRE(n >= 0 && (n == 0 || (event_slot && flags && ret_val && flow_out)), "null pointer");
+    for (int64_t i = 0; i < n; ++i) flow_out[i] = wire::flow_class(event_slot[i], flags[i], ret_val[i]);
+    return NERRF_OK;
+}
+
 // Node interning in event order `order` (NULL = identity): one node per pid and one per file identity, ids in
 // order of first appearance over the interleaved (process, file[, rename target]) sequence -- exactly the numbering
 // of graph.py graph_from_events.  merge_renames: a file and its renamed / encrypted twin share the node (key = path

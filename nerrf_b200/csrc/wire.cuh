@@ -158,5 +158,18 @@ NERRF_HD int event_slot(const uint8_t* s, uint64_t n) {
     return 7;
 }
 
+// information-flow class of an event (DESIGN.md 1.5) from its raw slot (event_slot above, not the observable fold), its
+// open flags and its return value: bit 0 = process -> file, bit 1 = file -> process.  The one definition of the table:
+// the host columns (nerrf_trace_flow_class) and the live stream's device columns (nerrf_trace_flow_class_device) use it.
+constexpr uint8_t FLOW_P2F = 1, FLOW_F2P = 2;
+NERRF_HD uint8_t flow_class(int slot, int64_t flags, int64_t ret_val) {
+    if (ret_val < 0) return 0;                                   // the syscall failed: nothing moved
+    switch (slot) {
+    case 0: case 1: case 2: case 3: case 5: case 6: return FLOW_P2F;   // created, encrypt_*, note, write, rename
+    case 4: return flags == 0 ? FLOW_F2P : flags == 1 ? FLOW_P2F : (uint8_t)(FLOW_P2F | FLOW_F2P);   // openat
+    default: return 0;                                           // slot 7: recon *_enum, unlink, ...
+    }
+}
+
 }  // namespace wire
 }  // namespace nerrf

@@ -342,11 +342,29 @@ def graph_from_events(events, merge_renames=True, window=None, observable=False)
     edge_event = np.asarray(eid, np.int64)[np.lexsort((tt, dst))]
     # edge_time: the trace-clock seconds of that event (float64, the time event_info reports), computed when asked for
     edge_time = lambda: np.asarray([_parse_ts(e["timestamp"]) for e in evs], np.float64)[edge_event]
+    # edge_flow: the information-flow class of that event (DESIGN.md 1.5; the raw kind, not the observable fold)
+    edge_flow = lambda: event_flow([_EVENT_SLOT.get(e["event"], _N_EVENT_SLOTS - 1) for e in evs],
+                                   [int(e.get("flags", 0)) for e in evs], [int(e.get("ret_val", 0)) for e in evs])[edge_event]
     return TemporalGraph(rowptr, col, ew, x, {"kind": "trace", "names": names, "node_kind": np.asarray(kinds),
                                               "label": y, "size_mb": size_mb, "t0": t0, "span": span,
                                               "file_keys": file_keys, "merge_renames": bool(merge_renames),
                                               "edge_label": edge_label, "edge_event": edge_event, "edge_time": edge_time,
+                                              "edge_flow": edge_flow,
                                               "event_info": lambda ids: [event_record(evs[int(i)]) for i in ids]})
+
+
+def event_flow(event_slot, flags, ret_val) -> np.ndarray:
+    """uint8 flow class of every event (DESIGN.md 1.5: bit 0 process -> file, bit 1 file -> process) from its raw event
+    slot, open flags and return value, by the library's one definition of the table (nerrf_trace_flow_class)"""
+    slot = np.ascontiguousarray(event_slot, np.uint8)
+    fl = np.ascontiguousarray(flags, np.int64)
+    rv = np.ascontiguousarray(ret_val, np.int64)
+    import ctypes
+    from . import _lib
+    out = np.zeros(slot.shape[0], np.uint8)
+    p = lambda a: a.ctypes.data_as(ctypes.c_void_p)
+    _lib.check(_lib.lib().nerrf_trace_flow_class(p(slot), p(fl), p(rv), slot.shape[0], p(out)), "nerrf_trace_flow_class")
+    return out
 
 
 def event_record(e) -> dict:

@@ -317,7 +317,12 @@ def graph_from_columns(cols: EventColumns, merge_renames=True, window=None, devi
         def edge_time(ts=ts):
             """the trace-clock seconds (float64) of the event that made each CSR edge"""
             return up(ts, np.float64)[edge_event()]
-        meta.update(edge_event=edge_event, edge_time=edge_time, event_info=lambda ids, cols=cols: column_event_records(cols, ids))
+
+        def edge_flow():
+            """the information-flow class (uint8, DESIGN.md 1.5) of the event that made each CSR edge"""
+            return up(column_flow(cols), np.uint8)[edge_event()]
+        meta.update(edge_event=edge_event, edge_time=edge_time, edge_flow=edge_flow,
+                    event_info=lambda ids, cols=cols: column_event_records(cols, ids))
         lab = label.cpu().numpy().astype(np.int64)
         if observable:                                        # the kernel saw the folded slots: labels come from the annotations
             lab = (np.bincount(F[(raw_slot == 1) | (raw_slot == 2)], minlength=N) > 0).astype(np.int64)
@@ -354,7 +359,16 @@ def graph_from_columns(cols: EventColumns, merge_renames=True, window=None, devi
 
     meta.update(label=label, size_mb=size_mb)
     rowptr, col, ew = G.csr_from_edges(src, dst, tt, conf, N, t_ref=float(span), tau=G.TAU)
+    # the event (row of the path-resolved columns) that made each CSR edge, its time and its flow class, as on the device
+    edge_event = np.repeat(order, 4)[keep].astype(np.int64)[np.lexsort((tt, dst))]
+    meta.update(edge_event=edge_event, edge_time=lambda: ts[edge_event].astype(np.float64),
+                edge_flow=lambda: column_flow(cols)[edge_event], event_info=lambda ids, cols=cols: column_event_records(cols, ids))
     return G.TemporalGraph(rowptr, col, ew, x, meta)
+
+
+def column_flow(cols: EventColumns) -> np.ndarray:
+    """uint8 flow class of every row (graph.event_flow of its raw slot, flags and ret_val)"""
+    return G.event_flow(cols.event_slot, cols.flags.astype(np.int64), cols.ret_val)
 
 
 def sequences_from_columns(cols: EventColumns, merge_renames=True, t_max=None, observable=False, only_nodes=None,

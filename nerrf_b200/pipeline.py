@@ -89,6 +89,7 @@ class PipelineResult:
                                       # (explain.explain_nodes + explain.attach_events); None when not asked for
     sequence_evidence: dict | None = None   # run(explain_sequences=k): node id of each planned file step -> the BiLSTM
                                             # explanation of its sequence (explain.explain_sequences); None when not asked for
+    contamination: dict | None = None  # run(contamination=True): incident id -> its contaminated nodes (taint.contamination)
     incidents: list | None = None     # run(incidents=True): the window's incidents (incident.incidents), onset order
     step_incident: dict | None = None  # run(incidents=True): node id of each planned node step and of each file an applied
                                        # restore covers -> its incident id (a kill: the incident its process owns, or None)
@@ -278,7 +279,8 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
         dist_ctx: DistContext | None = None, kill_candidates: bool = False, restore_candidates: bool = False,
         max_restores: int = 4, min_restore_files: int = 8, explain: int = 0,
         explain_max_edges: int | None = None, explain_max_full_graph: int | None = None, explain_sequences: int = 0,
-        seq_events=None, incidents: bool = False, incident_tau: float = 0.5, host_names=None) -> PipelineResult:
+        seq_events=None, incidents: bool = False, incident_tau: float = 0.5, host_names=None, contamination: bool = False,
+        contamination_hops: int = -1, contamination_only=None) -> PipelineResult:
     """seq/lengths/seq_nodes: LSTM inputs for (a superset of) the candidate file nodes (file_sequences()).
     seq may instead be a CALLABLE nodes -> (seq, lengths, nodes_with_sequences): the sequences are then built only for
     the top-A candidates (large windows: a million file nodes, a few thousand candidates); seq_nodes = the file nodes.
@@ -307,7 +309,14 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
     res.step_incident each planned node step's incident id and res.file_recovery each flagged file's recovery point.
     Files are attributed by the edge head exactly when the kill attribution is (a model marked edge_head_trained).
     host_names: source id -> host name, the prefix of incident ids on a graph of several sources.  The plan is the plan
-    of incidents=False.  One GPU only."""
+    of incidents=False.  One GPU only.
+    contamination=True (needs incidents=True): res.contamination holds what each incident's attack spread to (DESIGN.md
+    1.5; taint.contamination over at most contamination_hops hops, -1 = unbounded; contamination_only=ID seeds that
+    incident alone).  The plan is the plan of contamination=False.  One GPU only."""
+    if contamination and not incidents:
+        raise ValueError("contamination=True needs incidents=True (the closure is seeded by the incidents)")
+    if contamination and dist_ctx is not None and dist_ctx.world > 1:
+        raise NotImplementedError("contamination is computed on one GPU (dist_ctx.world > 1 is not supported)")
     if incidents and dist_ctx is not None and dist_ctx.world > 1:
         raise NotImplementedError("incidents are computed on one GPU (dist_ctx.world > 1 is not supported)")
     if restore_candidates and dist_ctx is not None and dist_ctx.world > 1:
@@ -451,6 +460,11 @@ def run(g: G.TemporalGraph, seq, lengths, seq_nodes, model: GraphSAGE_T, seq_mod
     if incidents:
         tm["incidents"] = _label_incidents(res, g, (rp, col, ew, x), model, h_final, score, incident_tau, host_names,
                                            edge_attack)
+        if contamination:
+            t0 = time.perf_counter()
+            res.contamination = contamination_of(G.TemporalGraph(rp, col, ew, x, g.meta), res, contamination_hops,
+                                                 contamination_only)
+            tm["contamination"] = (time.perf_counter() - t0) * 1e3
     if explain or explain_sequences:
         from . import explain as X
         t0 = time.perf_counter()
@@ -508,6 +522,18 @@ def _label_incidents(res: PipelineResult, g, g_dev, model, h_final, score, tau, 
     res.file_recovery = {v: (f["onset"], f["event"], f["later"]) for v, f in per_file.items()}
     torch.cuda.synchronize()
     return (time.perf_counter() - t0) * 1e3
+
+
+def contamination_of(g, res: PipelineResult, max_hops=-1, only=None, device="cuda") -> dict:
+    """taint.contamination seeded by a run(incidents=True) result: its incidents, and each flagged file at its recovery
+    point (res.file_recovery).  `g` is uploaded to `device` when its arrays are on the host."""
+    from . import taint
+    if not torch.is_tensor(g.rowptr):
+        dev = torch.device(device)
+        up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+        g = G.TemporalGraph(up(g.rowptr), up(g.col), up(g.ew), up(g.x), g.meta)
+    per_file = {int(v): {"onset": r[0]} for v, r in (res.file_recovery or {}).items()}
+    return taint.contamination(g, res.incidents or [], per_file, max_hops=max_hops, only=only)
 
 
 def step_incidents(plan_nodes, restores, node_kind, recs, per_file) -> dict:

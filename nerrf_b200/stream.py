@@ -450,6 +450,7 @@ class DeviceStream:
             pf = pf | (ingest.path_flags_of(goff, gdata) & np.uint8(1))
         self.d_pf = up(pf, np.uint8)
         self.d_pf_raw = up(cols.path_flags, np.uint8)         # the sequences use the event's own path flags
+        self._flow = None                                     # the flow class of every event, on first use (flow())
         self.cap = max((2 if self.merge else 3) * n, 1)
         self.node_p = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
         self.node_f = torch.empty_like(self.node_p); self.node_g = torch.empty_like(self.node_p)
@@ -590,6 +591,7 @@ class DeviceStream:
         self.d_pid, self.d_poff, self.d_pdata, self.d_goff, self.d_gdata = dc.s["pid"], res_off, res_data, goff, gdata
         self.d_source = dc.source
         self.d_raw_slot, self.d_slot, self.d_bytes, self.d_pf, self.d_pf_raw = dc.s["event_slot"], slot, dc.s["bytes"], pf, pf_raw
+        self._flow = None                                      # rows changed: flow() recomputes on first use
         if n_keep:
             lohi = torch.stack([ts_sorted[0], ts_sorted[n_keep - 1]]).cpu().numpy()
             self._span = (float(lohi[0]), float(lohi[1]))
@@ -598,6 +600,25 @@ class DeviceStream:
         self._alloc_intern(max(n, 1))
         ev1.synchronize()
         self.timings_ms["rebuild_ms"] = self.timings_ms.get("rebuild_ms", 0.0) + ev0.elapsed_time(ev1)
+
+    def flow(self):
+        """uint8 [rows] the information-flow class of every stored event (DESIGN.md 1.5), kept resident once asked for:
+        uploaded from the host columns of a whole-trace stream, computed on the device from the live decoder's
+        event_slot / flags / ret_val columns (nerrf_trace_flow_class_device) until the stream changes"""
+        if self._flow is None:
+            torch = self.torch
+            if self.cols is not None:
+                self._flow = torch.from_numpy(ingest.column_flow(self.cols)).to(self.dev)
+            else:
+                from . import _lib
+                dc, n = self._dc, self.n
+                flow = torch.empty(max(n, 1), dtype=torch.uint8, device=self.dev)
+                with torch.cuda.device(self.dev):
+                    _lib.check(_lib.lib().nerrf_trace_flow_class_device(_lib.ptr(dc.s["event_slot"]), _lib.ptr(dc.s["flags"]),
+                                                                        _lib.ptr(dc.s["ret_val"]), n, _lib.ptr(flow),
+                                                                        _lib.current_stream_ptr()), "nerrf_trace_flow_class_device")
+                self._flow = flow
+        return self._flow
 
     def _alloc_intern(self, n):
         """node tables and interning workspace for windows of up to n events"""
@@ -725,7 +746,11 @@ class DeviceStream:
         def edge_time():
             """the trace-clock seconds (float64) of the event that made each CSR edge, gathered on the device"""
             return self.d_ts[edge_event()]
-        meta.update(edge_event=edge_event, edge_time=edge_time, event_info=self.event_records)
+
+        def edge_flow():
+            """the information-flow class (uint8, DESIGN.md 1.5) of the event that made each CSR edge, gathered on the device"""
+            return self.flow()[edge_event()]
+        meta.update(edge_event=edge_event, edge_time=edge_time, edge_flow=edge_flow, event_info=self.event_records)
         if edge_labels:
             meta["edge_label"] = G.edge_labels_device(P, F, self.d_raw_slot[sel], rowptr, col, N)
         return G.TemporalGraph(rowptr, col, ew, x, meta)
@@ -820,6 +845,8 @@ class TickResult:
                                                     # (incident.incidents; "files" as plan keys)
     step_incident: dict = field(default_factory=dict)   # StreamingPlanner(incidents=True): plan key of each step this tick
                                                         # planned (as in `planned`, kills included) -> its incident id
+    contamination: dict = field(default_factory=dict)   # StreamingPlanner(contamination=True): incident id -> this tick's
+                                                        # contaminated nodes (taint.contamination; "key" = the node's plan key)
 
 
 @dataclass
@@ -847,6 +874,10 @@ class StreamingPlanner:
                                    # "onset" / "onset_event" (min over ticks), "end" / "end_event" (max), "files" (union
                                    # of plan keys), "n_files"}
     incident_tau: float = 0.5
+    contamination: object = False  # True (needs incidents): TickResult.contamination lists what each incident spread to
+                                   # (pipeline.run(contamination=True)); then, from construction on, the running records:
+                                   # incident id -> {node key: record with the earliest "since" over ticks}
+    contamination_hops: int = -1
     device: str = "cuda"
     dist_ctx: object = None        # pipeline.DistContext for the multi-GPU form
     reverted: set = field(default_factory=set)
@@ -869,6 +900,10 @@ class StreamingPlanner:
     def __post_init__(self):
         if isinstance(self.incidents, bool):
             self.incidents = {} if self.incidents else None
+        if isinstance(self.contamination, bool):
+            if self.contamination and self.incidents is None:
+                raise ValueError("contamination=True needs incidents=True (the closure is seeded by the incidents)")
+            self.contamination = {} if self.contamination else None
 
     def add_source(self, name: str) -> int:
         """Register a source (a host's tracker stream) -> its id (the next free one; an existing name keeps its id).
@@ -1069,6 +1104,8 @@ class StreamingPlanner:
 
         new, truncated, restored, evidence, seq_evidence, tick_inc, step_inc = [], False, [], {}, {}, {}, {}
         tick_nodes = {}                                  # incident id -> node ids of its tick record
+        tick_cont = {}                                   # incident id -> {node key: contaminated record}
+        want_cont = self.contamination is not None
         want_inc = self.incidents is not None
         if lead and self._host_keys is None:             # decided once per planner, so reverted / killed hold one form
             self._host_keys = len(self.sources) > 1 or ds.multi_source
@@ -1093,7 +1130,7 @@ class StreamingPlanner:
                                kill_candidates=self.kill_candidates, restore_candidates=self.restore_candidates,
                                max_restores=self.max_restores, min_restore_files=self.min_restore_files, explain=self.explain,
                                explain_sequences=self.explain_sequences, incidents=want_inc, incident_tau=self.incident_tau,
-                               host_names=inc_hosts)
+                               host_names=inc_hosts, contamination=want_cont, contamination_hops=self.contamination_hops)
             for k, v in res.timings_ms.items():
                 tm[k] = tm.get(k, 0.0) + float(v)
             got = []
@@ -1129,6 +1166,8 @@ class StreamingPlanner:
                             seq_evidence[key(n, nm)] = res.sequence_evidence[n]
                 if res.incidents is not None:
                     self._note_incidents(res, g, names, key, set(got) | set(fresh_kills), plan_names, tick_inc, tick_nodes, step_inc)
+                if res.contamination is not None:
+                    self._note_contamination(res, key, tick_cont)
                 new += got
                 for r in res.restores:                         # a restored directory brings back every file it covers
                     cov = revert(r["covers"], names.take(r["covers"]))
@@ -1142,8 +1181,23 @@ class StreamingPlanner:
             truncated = truncated or bool(res.plan.truncated)
             if not more:
                 break
+        tick_cont = {i: sorted(recs.values(), key=lambda r: (r["since"], str(r["key"]))) for i, recs in tick_cont.items()}
         self.ticks.append(TickResult(t_hi - t0, n_events, g.num_nodes, g.num_edges, new, tm, truncated, restored, evidence,
-                                     seq_evidence, tick_inc, step_inc))
+                                     seq_evidence, tick_inc, step_inc, tick_cont))
+
+    def _note_contamination(self, res, key, tick_cont):
+        """this planning pass's contamination -> the tick's records (a later pass of the same tick adds its new nodes and
+        keeps the earlier "since" of a node both passes reach) and the running records (earliest "since" per (incident,
+        node key) over ticks)"""
+        for i, recs in res.contamination.items():
+            tick = tick_cont.setdefault(i, {})
+            run = self.contamination.setdefault(i, {})
+            for r in recs:
+                k = key(r["node"], r["name"])
+                rec = dict(r, key=k)
+                for into in (tick, run):
+                    if k not in into or rec["since"] < into[k]["since"]:
+                        into[k] = rec
 
     _RUNNING_FIELDS = ("id", "host", "process", "onset", "onset_event", "end", "end_event", "files", "n_files")
 

@@ -8,6 +8,7 @@ ROADMAP.md:28,86 -- scheduled, never written).
     python -m nerrf_b200.undo --trace nodeA=a.pb --trace nodeB=b.pb --weights weights.pt --out plan.json --shell-dir DIR
     python -m nerrf_b200.undo --trace events.pb   --weights weights.pt --out plan.json --incidents
     python -m nerrf_b200.undo --trace events.pb   --weights weights.pt --out plan.json --incident pid:454
+    python -m nerrf_b200.undo --trace events.pb   --weights weights.pt --out plan.json --incidents --contamination
 
 trace: serialized nerrf.trace.EventBatch bytes (*.pb; proto/trace.proto:47-49, e.g. a buffered StreamEvents stream) or
 the simulator's TRACE json lines (*.jsonl; benchmarks/m1/scripts/sim_lockbit_m1.py:24-36).  Stages: ingest -> temporal
@@ -23,7 +24,10 @@ names).  A bare `--trace PATH`, or a single `--trace HOST=PATH`, is one source, 
 --incidents groups the plan's steps by the process that attacked their files (DESIGN.md 1.4): a top-level "incidents"
 table, the "incident" of every step and the "recovery_point" of every file step.  --incident ID plans that incident
 alone (ids are "pid:N", "unattributed", or "HOST/pid:N" with several hosts): the full plan is labelled first, then
-planned again with every file outside the incident excluded.
+planned again with every file outside the incident excluded.  --contamination adds to every incident of the table the
+nodes its attack spread to (DESIGN.md 1.5: files written and processes that read after the taint arrived, each with
+the events that carried it and, for a file, its recovery point); with --incident ID the closure is seeded by that
+incident alone.  --contamination-hops H bounds the closure to H hops.  Plan steps are unchanged.
 """
 from __future__ import annotations
 
@@ -74,6 +78,17 @@ def check_incident_args(a):
             raise SystemExit("--incident-threshold must be a number")
     if a.incident is not None and not a.incident:
         raise SystemExit("--incident needs an incident id (pid:N, unattributed, or HOST/pid:N)")
+
+
+def check_contamination_args(a):
+    """--contamination needs --incidents or --incident; --contamination-hops needs --contamination and is >= -1"""
+    if a.contamination and not (a.incidents or a.incident is not None):
+        raise SystemExit("--contamination needs --incidents or --incident ID")
+    if a.contamination_hops is not None:
+        if not a.contamination:
+            raise SystemExit("--contamination-hops needs --contamination")
+        if a.contamination_hops < -1:
+            raise SystemExit("--contamination-hops must be -1 (unbounded) or >= 0")
 
 
 def load_hosts(paths, device="cuda", events=False):
@@ -146,11 +161,16 @@ def main(argv=None) -> dict:
     ap.add_argument("--incident-threshold", type=float, default=None, metavar="T",
                     help="anomaly score at or above which a file belongs to an incident (default 0.5)")
     ap.add_argument("--incident", default=None, metavar="ID", help="plan only the incident ID (pid:N, or HOST/pid:N)")
+    ap.add_argument("--contamination", action="store_true",
+                    help="list under each incident what its attack spread to: derived files and processes that read them")
+    ap.add_argument("--contamination-hops", type=int, default=None, metavar="H",
+                    help="bound the contamination closure to H hops (default -1: unbounded)")
     ap.add_argument("--device", default="cuda")
     a = ap.parse_args(argv)
     traces = parse_traces(a.trace)
     check_outputs(traces, a.shell, a.shell_dir)
     check_incident_args(a)
+    check_contamination_args(a)
     hosts = [h for h, _ in traces] if len(traces) > 1 else None     # host fields only with several sources
     if not torch.cuda.is_available():
         raise SystemExit("nerrf_b200.undo needs a CUDA device (no CPU fallback for the hot path)")
@@ -170,7 +190,10 @@ def main(argv=None) -> dict:
                                             depth=a.depth, iterations=a.iterations, plan_steps=a.max_steps, device=a.device,
                                             explain=a.explain, explain_sequences=a.explain_sequences,
                                             seq_events=ev[0] if ev else None, exclude=exclude, incidents=want_inc,
-                                            incident_tau=tau, host_names=hosts)
+                                            incident_tau=tau, host_names=hosts,
+                                            contamination=a.contamination and a.incident is None and exclude is None,
+                                            contamination_hops=hops)
+    hops = -1 if a.contamination_hops is None else a.contamination_hops
     res = run()
     attack_id = a.id
     if a.incident is not None:
@@ -178,8 +201,11 @@ def main(argv=None) -> dict:
         if a.incident not in known:
             raise SystemExit("unknown incident %r; this trace's incidents: %s" % (a.incident, ", ".join(known) or "(none)"))
         mine = np.asarray(known[a.incident]["files"], np.int64)
+        full = res
         res = run(exclude=~np.isin(np.asarray(nodes, np.int64), mine))   # every file outside the incident is excluded
         attack_id = a.incident if a.id is None else a.id
+        if a.contamination:                                            # seeded by the incident alone, as the full plan found it
+            res.contamination = pipeline.contamination_of(g, full, hops, only=a.incident, device=a.device)
     plan = emit.from_pipeline(g, res, attack_id=attack_id, host_names=hosts)
     plan["stats"] = {"events": int(n_events), "nodes": int(g.num_nodes), "edges": int(g.num_edges),
                      "candidates": int(len(res.candidates)), "ingest_ms": t_ingest,
